@@ -2,6 +2,7 @@
 """Benchmark of the detection hot path (BASELINE.json metric: images/sec).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--workload frcnn_r50|frcnn_r101|ssd] [--impl ours|reference]
+                  [--dump-outputs DIR]
 
 A "step" = one pass of the forward hot path over one batch of synthetic images
 (N=1 workload: BASELINE.json configs[1] -- Faster R-CNN ResNet-50, COCO config,
@@ -13,6 +14,9 @@ NCCL once, every step all-gathers the padded detection records.
            on the engine's stream, max over ranks).
 `e2e`    : the same through the public host-buffer call (pinned host images ->
            H2D -> forward -> D2H of boxes/scores/labels/counts inside the timed region).
+`--dump-outputs DIR`: after the timed device steps, the outputs of the last step (boxes, scores, labels, counts of
+           rank 0's images; with N > 1 also `records`, the all-gathered {count, boxes, scores, labels} rows of every
+           image) as DIR/<name>.npy in float32; inputs and weights are seeded, so two builds compare output for output.
 `--impl reference`: the CPU oracle port of the reference forward (TF1 itself cannot be
            installed here) on all host cores, one image per step (a bounded sample).
 """
@@ -52,8 +56,9 @@ def peaks():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get('hbm_gbs', 6650.0), d.get('bf16_tflops_sustained', 1400.0), 'measured (MEASURED_PEAKS.json)'
-    return 6650.0, 1400.0, 'fallback (B200_PROFILING.md)'
+        if 'hbm_gbs' in d and 'bf16_tflops_sustained' in d:
+            return d['hbm_gbs'], d['bf16_tflops_sustained'], 'measured (MEASURED_PEAKS.json)'
+    return 3350.0, 989.0, 'NVIDIA H100 SXM data sheet (HBM3, dense FP16; not measured)'
 
 
 class ClockSampler(threading.Thread):
@@ -93,25 +98,6 @@ class ClockSampler(threading.Thread):
         reasons = [n for i, n in enumerate(names) if any(len(s) >= 6 and s[2 + i].lower().startswith('active') for s in self.samples)]
         return {'sm_mhz': float(np.median(sm)) if sm else None, 'sm_max_mhz': max(mx) if mx else None,
                 'reasons': reasons, 'samples': len(sm)}
-
-
-def conv_traffic(workload):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the conv_tc launches of one step.  ncu cannot run inside a
-    timed bench, so the figure comes from the committed `ncu --set full` capture of `bench.py --ncu-range`
-    (scripts/gpu_evidence.sh -> scripts/ncu_step_summary.py) and is stamped with the commit and date of that capture,
-    so a stale profile is visible as stale; None if this workload was never captured."""
-    here = os.path.dirname(os.path.abspath(__file__))
-    for name in ('r2_ncu_step_summary.json', 'r1_ncu_step_summary.json'):
-        try:
-            j = json.load(open(os.path.join(here, 'profiles', name)))
-            d = j[workload]['conv_tc_kernel']
-            stamp = j.get('_capture', {})
-            return d['dram_bytes'], ('sum of dram__bytes_read+write over the %d conv_tc launches of one step '
-                                     '(profiles/%s, captured at commit %s on %s)'
-                                     % (d['launches'], name, stamp.get('commit', 'round-1 final'), stamp.get('date', '2026-09-22')))
-        except Exception:
-            continue
-    return None, 'not captured'
 
 
 def build_config(wl):
@@ -324,6 +310,16 @@ def run_ours(args, wl):
         time.sleep(0.3)
     ms_dev = timed(step_device, args.steps, args.warmup)
     ms_dev_local = timed.local_ms
+    if args.dump_outputs and rank == 0:
+        # what the timed path returned in its last step (before the e2e / profiling passes reuse the buffers)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        # N > 1: the caller of the step receives the all-gathered detection records of every rank; rank 0's own
+        # boxes / scores / labels / counts are its shard of them
+        outs = [('boxes', boxes), ('scores', scores), ('labels', labels), ('counts', counts)]
+        if world > 1:
+            outs.append(('records', gathered))
+        for name, t in outs:
+            np.save(os.path.join(args.dump_outputs, name + '.npy'), t.float().cpu().numpy())
     launches = eng.last_launch_count
     clocks = sampler.finish() if sampler else None
     ms_e2e = timed(step_host, args.steps, max(3, args.warmup))
@@ -363,14 +359,13 @@ def run_ours(args, wl):
         roof = None
         if tc_ms > 0:
             ach = tc_flops / (tc_ms * 1e-3) / 1e12
-            roof = {'kernel': 'conv_tc_kernel (tcgen05 implicit-GEMM conv, all instances of one step)',
+            roof = {'kernel': 'conv_tc_kernel (wgmma implicit-GEMM conv, all instances of one step)',
                     'bound': 'tensor', 'achieved': ach, 'peak': tf, 'unit': 'TFLOP/s', 'frac': ach / tf,
-                    'peak_source': src + ', bf16 sustained', 'traffic': conv_traffic(args.workload)[0],
-                    'traffic_note': conv_traffic(args.workload)[1],
+                    'peak_source': src,
                     'launches_per_step': tc_spans / args.steps,
                     'algorithmic_gflop_per_step': tc_flops / args.steps / 1e9,
                     'ms_per_step': tc_ms / args.steps,
-                    'note': 'fp32-class accuracy is bought with 3 kind::f16 MMAs per algorithmic MAC '
+                    'note': 'fp32-class accuracy is bought with 3 fp16 wgmma MACs per algorithmic MAC '
                             '(fp16x2 operand split): the tensor pipe does 3x the algorithmic FLOPs, so frac <= 1/3'}
             for cat, key, note in (('roi_pool', 'roi_pool_hbm', 'ROI crop+max-pool(+mean) kernel; gather is L1/issue-bound, not HBM-bound'),
                                    ('rpn_proposals', 'rpn_nms_hbm', 'RPN decode+sort+bitmask NMS chain (bitmask-algorithm bytes)')):
@@ -382,12 +377,12 @@ def run_ours(args, wl):
         out = {
             'metric': 'images/sec', 'value': v, 'unit': 'images/s', 'n_gpus': world, 'steps': args.steps,
             'warmup': args.warmup, 'ms_per_step': ms_dev / args.steps, 'higher_is_better': True, 'scaling': 'weak',
-            'vs_baseline': None, 'dtype': 'f32 (fp16x2-split operands on tcgen05 kind::f16, fp32 accumulate)',
+            'vs_baseline': None, 'dtype': 'f32 (fp16x2-split operands on fp16 wgmma, fp32 accumulate)',
             'data': 'synthetic',
             'config': {'workload': wl['name'] + (' [batch overridden to %d]' % B if args.per_gpu_batch else ''),
                        'global_batch': total_imgs, 'per_gpu_batch': B,
                        'parallelism': 'dp%d (images sharded, NCCL weight broadcast + detection all-gather)' % world,
-                       'l2': 'inputs rotate over %d distinct batches (%.0f MB > 126 MB L2); per-step activation '
+                       'l2': 'inputs rotate over %d distinct batches (%.0f MB > 50 MB L2); per-step activation '
                              'working set is several GB' % (NROT, NROT * B * H * W * 3 / 1e6),
                        'weights': 'random-init (synthetic, seed 0, "peaky" profile)'},
             'e2e': {'value': e2e_v, 'unit': 'images/s', 'h2d_bytes_per_step': B * H * W * 3,
@@ -438,6 +433,8 @@ def main():
                     help='override the workload batch (latency studies; the headline number uses the default)')
     ap.add_argument('--layers', action='store_true', help='add a per-conv-layer timing table to the JSON line')
     ap.add_argument('--ncu-unpiped', action='store_true', help='with --ncu-range: single-stream forward')
+    ap.add_argument('--dump-outputs', default='', metavar='DIR',
+                    help='write the last timed step\'s outputs as DIR/<name>.npy (float32)')
     ap.add_argument('--ncu-range', action='store_true',
                     help='run warm-up, then one step inside cudaProfilerStart/Stop (for ncu --profile-from-start off)')
     args = ap.parse_args()

@@ -1,7 +1,7 @@
-/* luminoth_b200 -- C ABI of the B200-native detection inference engine.
+/* luminoth_b200 -- C ABI of the H100-native (sm_90a) detection inference engine.
  *
  * Drop-in boundary for the Faster R-CNN / SSD predict path of tryolabs/luminoth
- * (reference = /root/reference/luminoth).  The reference is pure Python on top
+ * (the reference).  The reference is pure Python on top
  * of TensorFlow 1.x: its "FFI" for this path is the TF session boundary in
  *   utils/predicting.py:20-107   graph build + weight restore   -> lumi_create / lumi_set_weight / lumi_finalize
  *   utils/predicting.py:109-112  session.run(fetches, {image})  -> lumi_predict
@@ -98,10 +98,10 @@ const char* lumi_profile_read(lumi_engine* e);
 const char* lumi_profile_read_layers(lumi_engine* e);
 
 /* Choose the convolution implementation: 0 = fp32 SIMT implicit GEMM everywhere,
- * 1 = tcgen05 fp16x2-split tensor-core kernel wherever the layer qualifies (default). */
+ * 1 = wgmma fp16x2-split tensor-core kernel wherever the layer qualifies (default). */
 int lumi_set_conv_impl(lumi_engine* e, int impl);
 
-/* Work scheduling of the tcgen05 convolution: 0 = whole output tiles only, 1 (default) = stream-K (the
+/* Work scheduling of the tensor-core convolution: 0 = whole output tiles only, 1 (default) = stream-K (the
  * K loops of all tiles cut into equal per-SM ranges, partial tiles summed in a fixed order) for layers whose
  * tile count would leave SMs idle in the last wave, 2 = stream-K wherever it is applicable. Results
  * are deterministic in every mode; modes differ in fp32 summation order only. */
@@ -144,8 +144,11 @@ const char* lumi_op_last_error(void);      /* message of the last failed lumi_op
 /* conv2d NHWC fp32 in/out (converted to/from the fp16x2 split planes internally).
  * w: TF layout [kh,kw,cin,cout] fp32 on DEVICE.  scale/bias [cout] or NULL.
  * residual NHWC fp32 [n,ho,wo,cout] or NULL.  act: 0 none, 1 relu, 2 relu6.
- * padding: 0 VALID, 1 SAME, 2 explicit slim conv2d_same.  impl: 0 SIMT, 1 tcgen05
- * (whole-tile schedule), 2 tcgen05 with the stream-K schedule forced. */
+ * padding: 0 VALID, 1 SAME, 2 explicit slim conv2d_same.  impl: 0 SIMT, 1 wgmma
+ * (whole-tile schedule), 2 wgmma with the stream-K schedule forced; 3-11 write the fp16x2 split planes the engine
+ * passes between layers: 3 two consumer warpgroups, 4 / 5 four warpgroups on short-K layers (5: + stream-K),
+ * 6 / 7 2-CTA clusters multicasting the weight tile (7: + stream-K), 8 / 9 halo-patch kernels on 3x3 stride-1 layers
+ * (9: + stream-K), 10 / 11 halo patches on 2-CTA clusters (11: + stream-K). */
 int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout,
                    int stride, int rate, int padding, const float* scale, const float* bias,
                    const float* residual, int act, int impl, float* y, int* ho, int* wo, void* stream);
@@ -194,20 +197,7 @@ int lumi_decode_jpeg(const unsigned char* data, size_t nbytes, int device, unsig
                      int out_on_device, int* height, int* width);
 const char* lumi_jpeg_last_error(void);
 
-/* ---- measurement hook (no reference counterpart, not on the predict path): cost of one tcgen05.mma kind::f16
- * 128 x n x 16 in SM clocks, averaged over all SMs, for `iters` stages of twelve MMAs.  mode: 0 every MMA accumulates
- * into the same TMEM tile, 1 the conv kernel's D1 / D2 / D2 pattern, 2 round-robin over three tiles, 3 over four.
- * shifted_a: A descriptors of the halo kernels (start 128 B past the swizzle boundary, 1280 B group stride).
- * fill: a second thread streams bulk copies into shared memory meanwhile; *fill_bytes_per_clk = its achieved rate.
- * ldtm_warps (0-8): that many warps keep reading another TMEM tile with tcgen05.ld.32x32b.x32 meanwhile, pausing
- * ldtm_gap clocks between reads; *ldtm_bytes_per_clk = their achieved rate per SM.
- * sync: 0 none, 1 one tcgen05.commit per stage, 2 the conv kernel's operand ring of depth `ring` without the copies
- * (commit -> empty barrier -> helper warp -> full barrier -> issuer).  mmas_per_stage: 12, or 4 (hi*hi only).
- * flags: 1 no tcgen05.fence after the ring wait, 2 spin on mbarrier.test_wait, 4 two issuing warps (hi*hi / cross terms). */
-int lumi_op_mma_probe(int mode, int n, int iters, int shifted_a, int fill, int ldtm_warps, int ldtm_gap,
-                      int sync, int ring, int mmas_per_stage, int flags, double* clk_per_mma,
-                      double* fill_bytes_per_clk, double* ldtm_bytes_per_clk);
-/* Second measurement hook: do the 32 lanes of one `mbarrier.try_wait` warp instruction ever get different answers?  One CTA
+/* ---- measurement hook (no reference counterpart, not on the predict path): do the 32 lanes of one `mbarrier.try_wait` warp instruction ever get different answers?  One CTA
  * per SM, `rounds` barrier phases; *diverged_rounds = rounds (summed over CTAs) in which the lanes' attempt counts differed. */
 int lumi_op_trywait_probe(int rounds, unsigned* diverged_rounds, unsigned* max_spread, unsigned* mean_attempts);
 

@@ -1,4 +1,4 @@
-"""luminoth_b200: B200-native (sm_100a) inference engine for the Faster R-CNN /
+"""luminoth_b200: H100-native (sm_90a) inference engine for the Faster R-CNN /
 SSD predict path of tryolabs/luminoth, behind Luminoth's own
 PredictorNetwork / config-YAML surface.  No CPU fallback."""
 from .config import get_config, default_config, override_config_params, set_prediction_filters  # noqa: F401

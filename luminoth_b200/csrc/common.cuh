@@ -1,4 +1,4 @@
-// Shared device/host helpers for the luminoth_b200 kernels (sm_100a only).
+// Shared device/host helpers for the luminoth_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -38,7 +38,7 @@ inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 // ---------------------------------------------------------------- activation tensors
 // Activations travel between layers as two fp16 planes (hi, lo) with
 // x ~= hi + lo (22-bit mantissa, "fp16x2 split"): same HBM bytes as fp32 and
-// directly consumable by tcgen05 kind::f16 through TMA.  NHWC, planes contiguous.
+// directly consumable by wgmma (fp16 operands) through TMA.  NHWC, planes contiguous.
 struct Act {
   __half* hi = nullptr;
   __half* lo = nullptr;
@@ -57,26 +57,16 @@ __device__ __forceinline__ void split_f32(float x, __half& hi, __half& lo) {
 __device__ __forceinline__ float join_f16(__half hi, __half lo) {
   return __half2float(hi) + __half2float(lo);
 }
-// x - float(h) in one mixed-precision FHFMA (sm_100: fma.f32.f16).  With h = rn16(x) the difference is
-// exactly representable in fp32, so this equals the two-instruction cvt + sub bit for bit.
-__device__ __forceinline__ float sub_f32_f16(float x, __half h) {
-  float d;
-  asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(d) : "h"(__half_as_ushort(h)), "h"((unsigned short)0xBC00), "f"(x));
-  return d;
-}
-// x + (hi + lo) in two mixed-precision FMAs (the 2^-11-times-smaller lo plane first): replaces two conversions and
-// two adds of `x + join_f16(hi, lo)` in the conv epilogue's residual add; differs from it by at most one rounding
-// of the partial sum (|lo| <= ulp16(hi) / 2, so x + lo is exact or within 1/2 ulp of x).
+// x + (hi + lo) with the 2^-11-times-smaller lo plane added first (the conv epilogue's residual add): differs from
+// `x + join_f16(hi, lo)` by at most one rounding of the partial sum (|lo| <= ulp16(hi) / 2, so x + lo is exact or
+// within 1/2 ulp of x).
 __device__ __forceinline__ float add_f16_pair(float x, __half hi, __half lo) {
-  float t, d;
-  asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(t) : "h"(__half_as_ushort(lo)), "h"((unsigned short)0x3C00), "f"(x));
-  asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(d) : "h"(__half_as_ushort(hi)), "h"((unsigned short)0x3C00), "f"(t));
-  return d;
+  return __fadd_rn(__fadd_rn(x, __half2float(lo)), __half2float(hi));
 }
 // two values per cvt.rn.f16x2.f32: hi = rn16(v), lo = rn16(v - hi)   (same results as split_f32)
 __device__ __forceinline__ void split2_f32(float a, float b, __half2& hi, __half2& lo) {
   hi = __floats2half2_rn(a, b);
-  lo = __floats2half2_rn(sub_f32_f16(a, __low2half(hi)), sub_f32_f16(b, __high2half(hi)));
+  lo = __floats2half2_rn(a - __low2float(hi), b - __high2float(hi));
 }
 __device__ __forceinline__ float apply_act(float v, int act) {
   if (act == ACT_RELU) return fmaxf(v, 0.f);
@@ -84,7 +74,7 @@ __device__ __forceinline__ float apply_act(float v, int act) {
   return v;
 }
 
-// ---------------------------------------------------------------- sm_100a PTX wrappers
+// ---------------------------------------------------------------- sm_90a PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }
@@ -148,6 +138,31 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const void* tmap, uint64_
       "l"((uint64_t)tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// ---------------------------------------------------------------- 2-CTA clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the same box into the same shared-memory offset of every CTA in cta_mask; each CTA's barrier at `bar`'s offset
+// receives the bytes that land in that CTA
+__device__ __forceinline__ void tma_load_2d_mc(void* dst, const void* tmap, uint64_t* bar, int c0, int c1,
+                                               uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, "
+      "%4}], [%2], %5;" ::"r"(smem_u32(dst)), "l"((uint64_t)tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
+      : "memory");
+}
+// arrive on the barrier at `bar`'s offset in cluster CTA `cta`
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
+}
 // smem -> global bulk tensor store (bulk async-group completion)
 __device__ __forceinline__ void tma_store_4d(const void* tmap, const void* src, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
@@ -160,153 +175,60 @@ __device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
+// ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
+// K-major, SWIZZLE_128B shared-memory matrix descriptor: rows of 128 B (64 fp16 of K) as TMA's SWIZZLE_128B writes
+// them, 8-row groups `sbo` bytes apart (1024 = consecutive swizzle atoms), leading byte offset unused for swizzled
+// K-major (= 1), matrix base offset 0.  The start address of a K = 16 slice inside the atom is the row start + 32 B
+// per slice.
+__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr, uint32_t sbo = 1024) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);      // start address       [0,14)
+  d |= (uint64_t)1 << 16;                           // leading byte offset [16,30)
+  d |= (uint64_t)(sbo >> 4) << 32;                  // stride byte offset  [32,46)
+  d |= (uint64_t)1 << 62;                           // layout: SWIZZLE_128B [62,64)
+  return d;
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; fp16 operands, fp32 accumulate, single CTA.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
+// hand registers from the producer warpgroup to the consumer warpgroups (whole warpgroup, compile-time counts)
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D(64 x N, fp32 registers of the warpgroup) (+)= A(64 x 16, smem desc) * B(16 x N, smem desc), both K-major fp16;
+// scale_d = 0 overwrites D.  Fragment: thread t holds rows 16 (t / 32) + (t % 32) / 4 (+ 8), columns 8 j + 2 (t % 4) (+ 1).
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once every previously issued tcgen05.mma of this thread has completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread = TMEM lane).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-// ---------------------------------------------------------------- CTA pair (cta_group::2) wrappers
-// Two CTAs of a 2-CTA cluster (same TPC) execute one M=256 MMA: each holds 128 rows of A, HALF the rows of B and its
-// own 128 x N fp32 accumulator in TMEM; the leader (cluster rank 0) issues.  Within such a pair the peer's shared
-// memory is the own window with bit 24 of the shared-space address flipped; clearing that bit addresses CTA 0.
-constexpr uint32_t LUMI_PEER_BIT_MASK = 0xFEFFFFFFu;
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA loads of either CTA of the pair; completion bytes are signalled on the LEADER's mbarrier (same smem offset)
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const void* tmap, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"((uint64_t)tmap), "r"(smem_u32(bar) & LUMI_PEER_BIT_MASK), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2,
-                                                int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-      "%6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"((uint64_t)tmap), "r"(smem_u32(bar) & LUMI_PEER_BIT_MASK), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-// arrive on the leader CTA's copy of `bar` (from either CTA of the pair)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & LUMI_PEER_BIT_MASK) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[128 rows per CTA] * B[N/2 rows per CTA]; issued by the leader CTA only
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  const uint32_t z = 0u;
+__device__ __forceinline__ void wgmma_m64n64k16_f16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(z)
-      : "memory");
-}
-// mbarrier `bar` of the CTAs in `cta_mask` arrives once every previously issued MMA of this thread has completed
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(cta_mask)
-               : "memory");
-}
-
-// One lane of the (converged) warp, chosen by the hardware.  ptxas knows that a branch on elect.sync runs in exactly one
-// thread and issues the uniform-operand instructions inside (UTCHMMA, UTMALDG, UTCBAR) directly; a branch on
-// `lane == 0` gets an elect-and-loop wrapper around every one of them.
-__device__ __forceinline__ bool elect_one() {
-#ifdef LUMI_NO_ELECT
-  return (threadIdx.x & 31u) == 0u;
-#endif
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_100 "version 1"):
-// rows of 128 B, 8-row swizzle atoms 1024 B apart (SBO), LBO unused (=1).
-__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);      // start address   [0,14)
-  d |= (uint64_t)1 << 16;                           // leading byte offset (ignored for swizzled K-major)
-  d |= (uint64_t)(1024 >> 4) << 32;                 // stride byte offset  [32,46)
-  d |= (uint64_t)1 << 46;                           // descriptor version 1 (Blackwell)
-  d |= (uint64_t)2 << 61;                           // SWIZZLE_128B
-  return d;
-}
-// The same with an explicit stride between the 8-row groups and a start address that need not sit on a 1024 B
-// boundary (shifted views into a halo patch, conv.cu HALO kernels).  base_off = matrix base offset field [49,52):
-// the phase of the start address inside the 1024 B swizzle pattern ((addr >> 7) & 7) when the hardware expects it there.
-__device__ __forceinline__ uint64_t make_sw128_kmajor_desc_sbo(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t base_off) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)(base_off & 7u) << 49;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// kind::f16 instruction descriptor: A,B = F16 (K-major), D = F32, M x N.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int m, int n) {
-  return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
 
 }  // namespace lumi

@@ -3,21 +3,17 @@
 //  * conv_simt_kernel : fp32 implicit GEMM on CUDA cores. Handles every shape
 //    (C_in = 3 stem, stride 2, FC layers); also the on-GPU cross-check of the
 //    tensor-core kernel.
-//  * conv_tc_kernel   : tcgen05 implicit GEMM, stride 1 or 2, C_in % 64 == 0.
+//  * conv_tc_kernel   : wgmma (sm_90a) implicit GEMM, stride 1 or 2, C_in % 64 == 0.
 //    Activations and weights are fp16 (hi, lo) split planes; each K=16 slice
-//    issues three kind::f16 MMAs  Ahi*Bhi + Ahi*Blo + Alo*Bhi  into fp32 TMEM
-//    accumulators (hi*hi into a double-buffered tile D1 that the epilogue warps
-//    drain in short chunks, the cross terms into D2 -- fp32-class accuracy,
-//    DESIGN section 3).  im2col is fused: the producer issues one 4-D TMA box
-//    {64 ch, tw, th, nb} per filter tap at shifted (possibly negative)
-//    coordinates; out-of-bounds elements are zero-filled by TMA, which IS the
-//    TF SAME zero padding.  Persistent CTAs (whole tiles or stream-K), warp
-//    roles: warp 0 TMA producer, warp 1 MMA issuer + TMEM owner (both walk the
-//    schedule as whole warps, one elected lane issues), 8 or 16 epilogue warps
-//    (TMEM -> regs -> scale/bias (folded BN) -> +residual -> relu/relu6 ->
-//    hi/lo split -> swizzled staging -> TMA store), one residual-slab producer
-//    lane in the RES kernels.  Variants: CTA pairs (tcgen05 cta_group::2) and
-//    the halo-patch kernels for 3x3 layers (DESIGN section 4.1).
+//    issues three wgmma  Ahi*Bhi + Ahi*Blo + Alo*Bhi  into fp32 register
+//    accumulators that are folded into an fp32 running sum once per 64-deep
+//    K slice (fp32-class accuracy, DESIGN section 3).  im2col is fused: a TMA
+//    producer thread issues one 4-D box {64 ch, tw, th, nb} per filter tap at
+//    shifted (possibly negative) coordinates; out-of-bounds elements are
+//    zero-filled by TMA, which IS the TF SAME zero padding.  Persistent CTAs
+//    (whole tiles or stream-K) of one producer and two or four consumer
+//    warpgroups, mbarrier operand ring.  Variants: 2-CTA clusters that
+//    multicast the weight tile, and halo-patch kernels for 3x3 layers.
 //
 // Replaces slim conv2d+batch_norm+relu (luminoth/models/base/base_network.py:143-151),
 // snt.Conv2D (models/fasterrcnn/rpn.py:69-90, models/ssd/ssd.py:83-96,
@@ -200,12 +196,10 @@ void launch_conv_simt(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
 }
 
 // =====================================================================================
-// tcgen05 implicit GEMM (fp16x2 split operands, fp32 TMEM accumulators)
+// wgmma implicit GEMM (fp16x2 split operands, fp32 register accumulators)
 // =====================================================================================
 struct TcArgs {
   CUtensorMap tm_a_hi, tm_a_lo, tm_b_hi, tm_b_lo;
-  CUtensorMap tm_o_hi, tm_o_lo;    // output planes, box {32 ch, tw, th, nb}, SWIZZLE_64B (split outputs only)
-  CUtensorMap tm_r_hi, tm_r_lo;    // residual planes, box {32 ch, tw*rs, th*rs, nb} with traversal stride rs (RES kernels)
   const float* scale; const float* bias;
   __half* out_hi; __half* out_lo; float* out_f32;
   const __half* res_hi; const __half* res_lo;
@@ -216,11 +210,6 @@ struct TcArgs {
   int tiles_w, tiles_h, tiles_n;   // M tiles per row / column / image groups
   int n_tiles;                     // C_out tiles (cout_pad / BN)
   int stride;                      // TMA traversal stride of the activation map (1 or 2)
-  int chunk_head, chunk_tail;      // D1 chunk schedule, see tc_chunk_end()
-  int halo_baseoff;                // HALO kernels: 1 = write the start address' swizzle phase into the descriptors
-  int dbg;                         // timing experiments (results are WRONG when set; env LUMI_CONV_DBG): 1 operand loads only for
-                                   // the first ring fill, 2 D1 drains without tcgen05.ld / adds, 4 no cross-term MMAs,
-                                   // 8 no output stores; 16 (results stay right) no tcgen05.fence after the operand-ring wait
   int* overflow;
   // stream-K (sk_mode != 0): the K loops of all tiles form one unit sequence that is cut into gridDim.x equal
   // contiguous ranges; a CTA that starts in the middle of a tile writes its partial accumulators to
@@ -237,7 +226,6 @@ struct TcItem { int tile, k0, k1; };
 struct TcSched {
   int mode, total_tiles, n_iters, t, bid, nblk;
   long long u, u_end;
-  // bid / nblk: this CTA's (or CTA pair's) index and the number of them -- blockIdx.x / gridDim.x for single CTAs
   __device__ TcSched(int mode_, int total_tiles_, int n_iters_, int bid_, int nblk_)
       : mode(mode_), total_tiles(total_tiles_), n_iters(n_iters_), bid(bid_), nblk(nblk_) {
     t = bid;
@@ -266,157 +254,100 @@ struct TcSched {
 };
 
 constexpr int TC_A_BYTES = 128 * 128;       // 128 pixel rows x 64 fp16 (one 128 B swizzle row each)
-// The tensor core adds each MMA's products into the fp32 accumulator with TRUNCATION (measured:
-// ~7e-8 relative, biased toward zero, per tcgen05.mma), so one long accumulation chain drifts by
-// ~1e-4 at K = 9216.  Two-level accumulation keeps fp32-class accuracy: the dominant hi*hi
-// products go to a double-buffered TMEM accumulator D1 that the epilogue warps drain into fp32
-// registers (round-to-nearest adds on the CUDA cores) every TC_CHUNK_STAGES pipeline stages; the
-// 2^-11-times-smaller cross terms hi*lo + lo*hi accumulate in their own TMEM tile D2 for the whole
-// K loop (their truncation error is 2^-11 times smaller still).
-constexpr int TC_CHUNK_STAGES = 4;          // 16 hi*hi MMAs per D1 chunk (the first `chunk_head` stages of a work item)
-// D1 chunk schedule of a work item (deterministic: a function of the stage index only, shared by the MMA issuer and
-// the epilogue warps).  The first chunk_head stages run in TC_CHUNK_STAGES-stage chunks -- the previous tile's
-// epilogue is still occupying the drain warps then, and two 4-stage chunks are what the two D1 buffers can absorb --
-// the remaining stages in chunk_tail-stage chunks.  Truncation error grows with the MMAs per chunk (CPU model of the
-// truncating accumulator, DESIGN 3): 16 MMAs ~5e-7 relative per layer, 8 ~2.8e-7, 4 ~1.8e-7; fp32 FMA chains of a CPU
-// conv sit at ~2e-7.
-__device__ __forceinline__ int tc_chunk_end(int rel, int n_rel, int head, int tail) {
-  // short work items (<= 4 stages: the 1x1 layers with C_in <= 256) fit the two D1 buffers whole, so they can use
-  // 1- or 2-stage chunks without shortening the MMA issuer's lead over the epilogue
-  const int head_len = n_rel <= 2 ? 1 : (n_rel <= 4 ? 2 : TC_CHUNK_STAGES);
-  const int len = rel < head ? head_len : tail;
-  const int e = rel + len;
-  return e < n_rel ? e : n_rel;
-}
+// HALO (3x3, stride 1, rate 1): the nine taps of a 64-channel slice read the SAME input pixels, shifted.  The HALO
+// kernels fetch the (th + 2) x (8 + 2)-pixel patch of the slice ONCE (one TMA box per patch row and plane, zero-filled
+// outside the image = SAME padding) and hand the tensor core nine shifted VIEWS of it: M tile = th rows x 8 pixels,
+// 8-row group g = image row g, so a view is the K-major SWIZZLE_128B matrix that starts at patch pixel (r, s) with a
+// group stride of one patch row.  The tensor core applies the 128 B swizzle to the absolute shared-memory address,
+// as TMA does when it writes the patch, so a view may start at any 128 B row; patch rows sit 2048 B apart so that every
+// row starts at the same phase of the pattern.  Only the weights stream per tap.
+constexpr int TC_HALO_TW = 8;                              // tile width: one 8-row group per image row
+constexpr int TC_HALO_PITCH = 2048;                        // bytes per patch row (10 pixels x 128 B, padded)
+constexpr int TC_HALO_ROWS = 16 + 2;                       // th <= 16
+constexpr int TC_HALO_PLANE_BYTES = TC_HALO_ROWS * TC_HALO_PITCH;
 
-// PAIR: two CTAs of a 2-CTA cluster share one 256 x BN tile (tcgen05 cta_group::2): each stages its own 128 rows of A and
-// HALF of the B tile, the leader issues M = 256 MMAs that read both CTAs' shared memory and write both CTAs' TMEM.
-// Operand bytes per CTA and stage drop from 64 KB to 48 KB, which buys a fourth stage: the long-K layers are bound by
-// the operand bytes in flight per SM.
-//
-// HALO (3x3, stride 1, rate 1): the nine taps of a 64-channel slice read the SAME input pixels, shifted.  The generic
-// kernel fetches them nine times from L2 (one im2col box per tap), and the long-K layers are bound by exactly that
-// L2 -> shared-memory operand traffic (64 KB per 12 MMAs; ~6300 B/clk for the whole chip).  The HALO kernels fetch the
-// (th+2) x (8+2)-pixel patch of the slice ONCE (one TMA box per plane, zero-filled outside the image = SAME padding)
-// and hand the tensor core nine shifted VIEWS of it: M tile = th rows x 8 pixels, 8-row group g = image row g, so a
-// view is the K-major SWIZZLE_128B matrix that starts at patch pixel (r, s) with a group stride of one patch row
-// (10 pixels = 1280 B).  Only the weights stream per tap.  A traffic drops ~6x, total operand traffic 1.7x (BN = 128)
-// to 2.3x (BN = 64).
-constexpr int TC_HALO_TW = 8;                              // tile width: one 8-row swizzle group per image row
-constexpr int TC_HALO_PITCH = (TC_HALO_TW + 2) * 128;      // bytes per patch row (10 pixels x 64 fp16)
-constexpr int TC_HALO_PLANE_BYTES = ((16 + 2) * TC_HALO_PITCH + 1023) / 1024 * 1024;   // th <= 16
-
-template <int BN, int STAGES, bool RES = false, int NSPLIT = 2, bool INPLACE = false, bool PAIR = false,
-          bool HALO = false>
+// NCWG consumer warpgroups: 2 (each 64 rows x BN columns) or 4 (64 rows x BN / 2 columns each; sixteen epilogue warps
+// with half the accumulator registers each, for the short-K layers whose time is mostly epilogue).
+// PAIR: a 2-CTA cluster shares one N tile between two M tiles; each CTA loads HALF of the weight tile and multicasts
+// it into both CTAs' shared memory, halving the weight traffic from L2.
+template <int BN, int STAGES, int NCWG = 2, bool PAIR = false, bool HALO = false>
 struct TcCfg {
-  static_assert((BN / NSPLIT) % 32 == 0, "each epilogue part owns whole 32-channel slabs");
-  static_assert(!INPLACE || (RES && BN / NSPLIT == 32), "in-place residual needs exactly one slab per part");
-  static_assert(!PAIR || (!RES && BN == 128), "the CTA-pair kernel exists for BN = 128 without residual");
-  static_assert(!HALO || !RES, "the halo kernels have no residual input (conv2 of a bottleneck, RPN conv, VGG)");
-  static constexpr int B_BYTES = PAIR ? BN * 64 : BN * 128;       // rows of B staged by THIS CTA x 128 B
-  static constexpr int A_STAGE_BYTES = HALO ? 0 : 2 * TC_A_BYTES; // HALO: A lives in the patch buffers, stages hold B only
-  static constexpr int STAGE_BYTES = A_STAGE_BYTES + 2 * B_BYTES;
-  static constexpr int PATCH_BYTES = HALO ? 2 * TC_HALO_PLANE_BYTES : 0;      // one patch buffer: hi + lo plane
-  static constexpr int OUT_STAGE_BYTES = NSPLIT * 2 * 128 * 64;   // per column part: hi + lo slabs of 128 rows x 32 ch
-  // RES: the whole residual tile (BN/32 slabs x {hi, lo} x 128 rows x 64 B) is TMA-prefetched at tile start
-  static constexpr int RES_STAGE_BYTES = (RES && !INPLACE) ? (BN / 32) * 2 * 128 * 64 : 0;
-  static constexpr int SMEM_BYTES =
-      2 * PATCH_BYTES + STAGES * STAGE_BYTES + OUT_STAGE_BYTES + RES_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(NCWG == 2 || NCWG == 4, "two or four consumer warpgroups");
+  static_assert(!PAIR || BN == 128, "the cluster pair exists for BN = 128");
+  static constexpr int WN = BN * 2 / NCWG;                         // columns per consumer warpgroup
+  static constexpr int B_BYTES = BN * 128;                         // BN weight rows x 64 fp16
+  static constexpr int A_STAGE_BYTES = HALO ? 0 : 2 * TC_A_BYTES;  // HALO: A lives in the patch buffers
+  static constexpr int STAGE_BYTES = A_STAGE_BYTES + 2 * B_BYTES;  // A hi, A lo, B hi, B lo
+  static constexpr int PATCH_BYTES = HALO ? 2 * TC_HALO_PLANE_BYTES : 0;   // one patch buffer: hi + lo plane
+  static constexpr int SMEM_BYTES = 2 * PATCH_BYTES + STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 232448, "shared memory per CTA");
-  static constexpr int TMEM_COLS = 4 * BN;          // D1[0], D1[1], D2[0], D2[1]  (256 or 512 columns)
-  static constexpr int EPI_WARPS = 4 * NSPLIT;
-  static constexpr int RES_WARP = 2 + EPI_WARPS;    // residual-tile TMA producer (RES kernels)
-  static constexpr int THREADS = (2 + EPI_WARPS + (RES ? 1 : 0)) * 32;   // warp 0 TMA, warp 1 MMA, then the epilogue warps
+  static constexpr int THREADS = (1 + NCWG) * 128;   // warpgroup 0: TMA producer (one thread), then the consumers
+  // register split: the producer warpgroup keeps the minimum and hands the rest to the consumers.  setmaxnreg.inc
+  // can only take what the CTA's own warpgroups released, so the total stays within the launch allocation (the
+  // per-thread count __launch_bounds__ allows, rounded down to a multiple of 8, times THREADS)
+  static constexpr int LAUNCH_REGS = (65536 / THREADS) / 8 * 8;
+  static constexpr int PRODUCER_REGS = NCWG == 2 ? 40 : 24;
+  static constexpr int CONSUMER_REGS = NCWG == 2 ? 232 : 112;
+  static_assert(128 * (PRODUCER_REGS + NCWG * CONSUMER_REGS) <= THREADS * LAUNCH_REGS, "register budget of the CTA");
 };
 
-
-// Persistent: grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x, += gridDim.x.  The
-// TMA producer, the MMA issuer and the epilogue warps each iterate the same tile sequence with
-// free-running stage / chunk counters, so the producer prefetches the next tile's operands and the
-// tensor core starts the next tile while the epilogue warps are still storing the previous one
-// (D1 and D2 are double-buffered in TMEM).
-template <int BN, int STAGES, bool RES, int NSPLIT, bool INPLACE, bool PAIR, bool HALO>
-__global__ void __launch_bounds__(TcCfg<BN, STAGES, RES, NSPLIT, INPLACE, PAIR, HALO>::THREADS, 1)
+// Persistent: grid = min(#tiles, #SMs) (or #SMs for stream-K); every CTA (or CTA pair) walks its schedule.  One
+// producer thread keeps a ring of STAGES (tap, 64-channel) K slices in flight with TMA: im2col is fused -- one 4-D box
+// {64 ch, tw, th, nb} per filter tap at shifted (possibly negative) coordinates, zero-filled outside the map, which IS
+// the TF SAME zero padding.  Per K slice each consumer warpgroup issues, for each K = 16 step, the three products
+// Ahi*Blo + Alo*Bhi + Ahi*Bhi  into a fresh fp32 register tile (the lo*lo term is below fp32 resolution), waits for
+// them and adds the tile into the running fp32 sum with round-to-nearest adds: the tensor core's own accumulation
+// chain never spans more than one 64-deep slice, which keeps fp32-class accuracy at K = 9216 (DESIGN section 3).
+// Epilogue: scale/bias (folded BN) -> +residual -> relu/relu6 -> fp32 or hi/lo split.
+template <int BN, int STAGES, int NCWG, bool PAIR, bool HALO>
+__global__ void __launch_bounds__(TcCfg<BN, STAGES, NCWG, PAIR, HALO>::THREADS, 1)
 conv_tc_kernel(const __grid_constant__ TcArgs a) {
-  using Cfg = TcCfg<BN, STAGES, RES, NSPLIT, INPLACE, PAIR, HALO>;
-  constexpr int EPI_WARPS = Cfg::EPI_WARPS;
-  // CTA pair: rank inside the 2-CTA cluster (0 = leader: arms the stage barriers, issues every MMA); scheduling unit =
-  // the pair (sched_id of sched_n); logical tile t = (pair of M tiles, N tile), this CTA's M tile = 2 * pair + rank
-  // (warp-uniform values are routed through a shuffle so that the compiler KNOWS they are uniform: the TMA / MMA issue
-  // instructions take their operands from uniform registers.  Inside `if (lane == 0)` every operand counts as
-  // thread-varying and each UTCHMMA / UTMALDG gets a loop of ELECT + five R2UR around it; with the whole warp walking
-  // the schedule and an elect.sync branch around the issue itself, the twelve MMAs of a stage are twelve consecutive
-  // UTCHMMA instructions.  Measured: conv_tc 3.62 -> 3.42 ms per step for the uniform operands alone.)
-  const int pair_rank = PAIR ? __shfl_sync(0xffffffffu, (int)cluster_ctarank(), 0) : 0;
+  using Cfg = TcCfg<BN, STAGES, NCWG, PAIR, HALO>;
+  constexpr int WN = Cfg::WN;
+  constexpr int NR = WN / 2;                          // accumulator registers per thread (64 rows x WN / 128 threads)
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* patch = smem;                              // HALO: [2 buffers][hi, lo][18 rows x 2048 B]
+  uint8_t* stages = smem + 2 * Cfg::PATCH_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stages + STAGES * Cfg::STAGE_BYTES);
+  uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* patch_full_bar = empty_bar + STAGES;      // [2]
+  uint64_t* patch_empty_bar = patch_full_bar + 2;     // [2]
+
+  // PAIR: rank in the cluster; the scheduling unit is the pair, whose CTAs take M tiles 2 m and 2 m + 1 of one N tile
+  const int rank = PAIR ? (int)cluster_ctarank() : 0;
   const int sched_id = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
   const int sched_n = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  extern __shared__ uint8_t smem_raw[];
-  // 1024 B alignment by OFFSET (not by integer round-trip) so the compiler keeps the shared address space
-  // and emits LDS/STS for the staging buffers instead of generic LD/ST
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* patch = smem;                                      // HALO: [2 buffers][hi, lo][(th+2) x 10 pixels x 128 B]
-  uint8_t* stages = smem + 2 * Cfg::PATCH_BYTES;              // operand ring
-  uint8_t* out_stage = stages + STAGES * Cfg::STAGE_BYTES;    // [2 halves][hi, lo][128 rows x 64 B], 64 B swizzle
-  uint8_t* res_stage = out_stage + Cfg::OUT_STAGE_BYTES;      // [BN/32 slabs][hi, lo][128 rows x 64 B] (RES only)
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(res_stage + Cfg::RES_STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* acc_full_bar = empty_bar + STAGES;       // [2]  D1[buf] chunk complete (tcgen05.commit)
-  uint64_t* acc_empty_bar = acc_full_bar + 2;        // [2]  D1[buf] drained by the 8 epilogue warps
-  uint64_t* d2_empty_bar = acc_empty_bar + 2;        // [2]  D2[tbuf] drained
-  uint64_t* res_full_bar = d2_empty_bar + 2;         // [4]  residual slab landed (TMA)
-  uint64_t* res_empty_bar = res_full_bar + 4;        // [4]  residual slab consumed by its 4 epilogue warps
-  uint64_t* patch_full_bar = res_empty_bar + 4;      // [2]  HALO: patch buffer landed (TMA)
-  uint64_t* patch_empty_bar = patch_full_bar + 2;    // [2]  HALO: every MMA reading the patch buffer has retired
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(patch_empty_bar + 2);
-
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int m_tiles = a.tiles_w * a.tiles_h * a.tiles_n;
   const int total_tiles = (PAIR ? (m_tiles + 1) / 2 : m_tiles) * a.n_tiles;
   const int rows_valid = a.nb * a.th * a.tw;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) {       // pair: the leader's "drained" barriers collect the epilogue warps of BOTH CTAs
-      mbar_init(&acc_full_bar[s], 1);
-      mbar_init(&acc_empty_bar[s], PAIR ? 2 * EPI_WARPS : EPI_WARPS);
-      mbar_init(&d2_empty_bar[s], PAIR ? 2 * EPI_WARPS : EPI_WARPS);
-    }
-    // res_empty: the slab's four epilogue warps (separate residual staging) or the part's store leader (in place)
-    for (int s = 0; s < 4; ++s) { mbar_init(&res_full_bar[s], 1); mbar_init(&res_empty_bar[s], INPLACE ? 1 : 4); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&patch_full_bar[s], 1); mbar_init(&patch_empty_bar[s], 1); }
-    fence_mbar_init();
-  }
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&a.tm_a_hi); tma_prefetch_desc(&a.tm_a_lo);
-    tma_prefetch_desc(&a.tm_b_hi); tma_prefetch_desc(&a.tm_b_lo);
-    if (!a.out_f32) { tma_prefetch_desc(&a.tm_o_hi); tma_prefetch_desc(&a.tm_o_lo); }
-    if (RES) { tma_prefetch_desc(&a.tm_r_hi); tma_prefetch_desc(&a.tm_r_lo); }
-  }
-  if (PAIR) cluster_sync_all();          // both CTAs' barriers exist before anything is signalled across the pair
-  if (warp == 1) {
-    if (PAIR) { tmem_alloc_2sm(tmem_slot, Cfg::TMEM_COLS); tmem_relinquish_2sm(); }
-    else { tmem_alloc(tmem_slot, Cfg::TMEM_COLS); tmem_relinquish(); }
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
-
   const int cchunks = a.cin >> 6;
   const int n_iters = a.kh * a.kw * cchunks;
 
-  if (warp == 0) {
-    {
-      // ---------------- TMA producer: one (tap, 64-channel) slice per stage.  The whole warp walks the schedule and
-      // waits on the barriers (every value stays warp-uniform); lane 0 issues the copies.
+  if (threadIdx.x == 0) {
+    // empty: one arrival per consumer warpgroup of every CTA whose shared memory the stage's copies write
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], (PAIR ? 2 : 1) * NCWG); }
+    for (int s = 0; s < 2; ++s) { mbar_init(&patch_full_bar[s], 1); mbar_init(&patch_empty_bar[s], NCWG); }
+    fence_mbar_init();
+    tma_prefetch_desc(&a.tm_a_hi); tma_prefetch_desc(&a.tm_a_lo);
+    tma_prefetch_desc(&a.tm_b_hi); tma_prefetch_desc(&a.tm_b_lo);
+  }
+  if (PAIR) cluster_sync_all();        // both CTAs' barriers exist before either multicasts into the other
+  else __syncthreads();
+
+  if (wg == 0) {
+    setmaxnreg_dec<Cfg::PRODUCER_REGS>();
+    if (threadIdx.x == 0) {
+      // ---------------- TMA producer: one (tap, 64-channel) slice per stage
       const uint32_t stage_tx = (HALO ? 0u : 2u * (uint32_t)rows_valid * 128u) + 2u * (uint32_t)Cfg::B_BYTES;
-      const uint32_t patch_tx = 2u * (uint32_t)(a.th + 2) * (uint32_t)TC_HALO_PITCH;
+      const uint32_t patch_tx = 2u * (uint32_t)(a.th + 2) * (uint32_t)((TC_HALO_TW + 2) * 128);
       uint32_t git = 0, gpatch = 0;
       TcSched sched(a.sk_mode, total_tiles, n_iters, sched_id, sched_n);
       TcItem item;
       while (sched.next(item)) {
         const int t = item.tile;
-        const int nt = t % a.n_tiles, mt = PAIR ? 2 * (t / a.n_tiles) + pair_rank : t / a.n_tiles;
+        const int nt = t % a.n_tiles, mt = PAIR ? 2 * (t / a.n_tiles) + rank : t / a.n_tiles;
         const int x0 = (mt % a.tiles_w) * a.tw, y0 = ((mt / a.tiles_w) % a.tiles_h) * a.th;
         const int img0 = (mt / (a.tiles_w * a.tiles_h)) * a.nb, n0 = nt * BN;
         int patch_cc = -1;
@@ -430,17 +361,12 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
             const uint32_t pb = gpatch & 1u;
             mbar_wait(&patch_empty_bar[pb], ((gpatch >> 1) & 1u) ^ 1u);
             uint8_t* pbase = patch + pb * Cfg::PATCH_BYTES;
-            if (!elect_one()) {
-            } else if (PAIR) {
-              if (pair_rank == 0) mbar_arrive_expect_tx(&patch_full_bar[pb], 2u * patch_tx);
-              tma_load_4d_2sm(pbase, &a.tm_a_hi, &patch_full_bar[pb], cc * 64, x0 - a.pad_l, y0 - a.pad_t, img0);
-              tma_load_4d_2sm(pbase + TC_HALO_PLANE_BYTES, &a.tm_a_lo, &patch_full_bar[pb], cc * 64, x0 - a.pad_l,
-                              y0 - a.pad_t, img0);
-            } else {
-              mbar_arrive_expect_tx(&patch_full_bar[pb], patch_tx);
-              tma_load_4d(pbase, &a.tm_a_hi, &patch_full_bar[pb], cc * 64, x0 - a.pad_l, y0 - a.pad_t, img0);
-              tma_load_4d(pbase + TC_HALO_PLANE_BYTES, &a.tm_a_lo, &patch_full_bar[pb], cc * 64, x0 - a.pad_l,
-                          y0 - a.pad_t, img0);
+            mbar_arrive_expect_tx(&patch_full_bar[pb], patch_tx);
+            for (int i = 0; i < a.th + 2; ++i) {
+              tma_load_4d(pbase + i * TC_HALO_PITCH, &a.tm_a_hi, &patch_full_bar[pb], cc * 64, x0 - a.pad_l,
+                          y0 - a.pad_t + i, img0);
+              tma_load_4d(pbase + TC_HALO_PLANE_BYTES + i * TC_HALO_PITCH, &a.tm_a_lo, &patch_full_bar[pb], cc * 64,
+                          x0 - a.pad_l, y0 - a.pad_t + i, img0);
             }
             ++gpatch;
           }
@@ -448,394 +374,204 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
           mbar_wait(&empty_bar[st], ph ^ 1u);
           uint8_t* sbase = stages + st * Cfg::STAGE_BYTES;
           const int kcol = tap * a.cin + cc * 64;
-          if ((a.dbg & 1) && git >= (uint32_t)STAGES) {         // (experiment) stale operands: just flip the barrier
-            if (lane == 0 && pair_rank == 0) mbar_arrive(&full_bar[st]);
-          } else if (!elect_one()) {
-          } else if (HALO) {
-            if (PAIR) {
-              if (pair_rank == 0) mbar_arrive_expect_tx(&full_bar[st], 2u * stage_tx);
-              tma_load_2d_2sm(sbase, &a.tm_b_hi, &full_bar[st], kcol, n0 + pair_rank * (BN / 2));
-              tma_load_2d_2sm(sbase + Cfg::B_BYTES, &a.tm_b_lo, &full_bar[st], kcol, n0 + pair_rank * (BN / 2));
-            } else {
-              mbar_arrive_expect_tx(&full_bar[st], stage_tx);
-              tma_load_2d(sbase, &a.tm_b_hi, &full_bar[st], kcol, n0);
-              tma_load_2d(sbase + Cfg::B_BYTES, &a.tm_b_lo, &full_bar[st], kcol, n0);
-            }
-          } else if (PAIR) {
-            // the leader arms its barrier for the bytes of BOTH CTAs; either CTA's loads complete on that barrier
-            // (a tile of the odd CTA past the last M tile lies outside the tensor: zero-filled, same byte count)
-            if (pair_rank == 0) mbar_arrive_expect_tx(&full_bar[st], 2u * stage_tx);
-            tma_load_4d_2sm(sbase, &a.tm_a_hi, &full_bar[st], cc * 64, ix, iy, img0);
-            tma_load_4d_2sm(sbase + TC_A_BYTES, &a.tm_a_lo, &full_bar[st], cc * 64, ix, iy, img0);
-            tma_load_2d_2sm(sbase + 2 * TC_A_BYTES, &a.tm_b_hi, &full_bar[st], kcol, n0 + pair_rank * (BN / 2));
-            tma_load_2d_2sm(sbase + 2 * TC_A_BYTES + Cfg::B_BYTES, &a.tm_b_lo, &full_bar[st], kcol, n0 + pair_rank * (BN / 2));
-          } else {
-            mbar_arrive_expect_tx(&full_bar[st], stage_tx);
+          mbar_arrive_expect_tx(&full_bar[st], stage_tx);
+          if (!HALO) {
             tma_load_4d(sbase, &a.tm_a_hi, &full_bar[st], cc * 64, ix, iy, img0);
             tma_load_4d(sbase + TC_A_BYTES, &a.tm_a_lo, &full_bar[st], cc * 64, ix, iy, img0);
-            tma_load_2d(sbase + 2 * TC_A_BYTES, &a.tm_b_hi, &full_bar[st], kcol, n0);
-            tma_load_2d(sbase + 2 * TC_A_BYTES + Cfg::B_BYTES, &a.tm_b_lo, &full_bar[st], kcol, n0);
           }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (pair_rank == 0) {
-      // ---------------- MMA issuer: per K=16 slice  D1 += Ahi*Bhi ;  D2 += Ahi*Blo + Alo*Bhi
-      // (pair: only the leader issues; M = 256 spans both CTAs' A rows and accumulators).  Whole warp walks and
-      // waits, lane 0 issues: descriptors and TMEM addresses live in uniform registers.
-      constexpr uint32_t idesc = make_idesc_f16(PAIR ? 256 : 128, BN);
-      uint32_t git = 0, gchunk = 0, tile_iter = 0, gpatch = 0;
-      TcSched sched(a.sk_mode, total_tiles, n_iters, sched_id, sched_n);
-      TcItem item;
-      for (; sched.next(item); ++tile_iter) {
-        const uint32_t tbuf = tile_iter & 1u;
-        mbar_wait(&d2_empty_bar[tbuf], ((tile_iter >> 1) & 1u) ^ 1u);     // previous user of D2[tbuf] drained
-        tc_fence_after();
-        const uint32_t d2 = tmem_base + (2u + tbuf) * BN;
-        uint32_t d1 = 0, buf = 0;
-        const int n_rel = item.k1 - item.k0;
-        int chunk_begin = 0, chunk_stop = 0;           // current chunk = stages [chunk_begin, chunk_stop) of this item
-        int patch_cc = -1;
-        uint32_t pb = 0;
-        for (int it = item.k0; it < item.k1; ++it, ++git) {
-          const int rel = it - item.k0;
-          if (rel == chunk_stop) {
-            chunk_begin = rel;
-            chunk_stop = tc_chunk_end(rel, n_rel, a.chunk_head, a.chunk_tail);
-            buf = gchunk & 1u;
-            mbar_wait(&acc_empty_bar[buf], ((gchunk >> 1) & 1u) ^ 1u);    // D1[buf] drained
-            tc_fence_after();
-            d1 = tmem_base + buf * BN;
-          }
-          const bool first_of_chunk = rel == chunk_begin;
-          const uint32_t st = git % STAGES, ph = (git / STAGES) & 1u;
-          // (probing the NEXT stage's barrier before this stage's MMAs are issued, so that the satisfied wait costs
-          //  nothing between two stages, was measured: no gain -- conv 3.265 vs 3.281 ms)
-          mbar_wait(&full_bar[st], ph);
-          if (!(a.dbg & 16)) tc_fence_after();
-          const uint32_t sa = smem_u32(stages + st * Cfg::STAGE_BYTES);
-          uint64_t d_ahi, d_alo;
-          if (HALO) {
-            const int cc = it / 9, tap = it - cc * 9;
-            if (cc != patch_cc) {
-              patch_cc = cc;
-              pb = gpatch & 1u;
-              mbar_wait(&patch_full_bar[pb], (gpatch >> 1) & 1u);
-              tc_fence_after();
-              ++gpatch;
-            }
-            // view of the patch shifted by tap (r, s): row 8 g + j of the operand = patch pixel (g + r, j + s)
-            const uint32_t pa = smem_u32(patch + pb * Cfg::PATCH_BYTES) + (uint32_t)((tap / 3) * TC_HALO_PITCH + (tap % 3) * 128);
-            const uint32_t boff = a.halo_baseoff ? (pa >> 7) & 7u : 0u;
-            d_ahi = make_sw128_kmajor_desc_sbo(pa, TC_HALO_PITCH, boff);
-            d_alo = make_sw128_kmajor_desc_sbo(pa + TC_HALO_PLANE_BYTES, TC_HALO_PITCH, boff);
+          uint8_t* bbase = sbase + Cfg::A_STAGE_BYTES;
+          if (PAIR) {          // this CTA's half of the weight rows, into the same offset of both CTAs
+            const int off = rank * (BN / 2);
+            tma_load_2d_mc(bbase + off * 128, &a.tm_b_hi, &full_bar[st], kcol, n0 + off, 0x3);
+            tma_load_2d_mc(bbase + Cfg::B_BYTES + off * 128, &a.tm_b_lo, &full_bar[st], kcol, n0 + off, 0x3);
           } else {
-            d_ahi = make_sw128_kmajor_desc(sa);
-            d_alo = make_sw128_kmajor_desc(sa + TC_A_BYTES);
-          }
-          const uint64_t d_bhi = make_sw128_kmajor_desc(sa + Cfg::A_STAGE_BYTES);
-          const uint64_t d_blo = make_sw128_kmajor_desc(sa + Cfg::A_STAGE_BYTES + Cfg::B_BYTES);
-          if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t ko = (uint64_t)(k * 2);      // 16 fp16 = 32 B = 2 x 16 B units
-            if (PAIR) {
-              umma_f16_2sm(d1, d_ahi + ko, d_bhi + ko, idesc, (!first_of_chunk || k > 0) ? 1u : 0u);
-              if (a.dbg & 4) continue;
-              umma_f16_2sm(d2, d_ahi + ko, d_blo + ko, idesc, (it > item.k0 || k > 0) ? 1u : 0u);
-              umma_f16_2sm(d2, d_alo + ko, d_bhi + ko, idesc, 1u);
-            } else {
-              umma_f16(d1, d_ahi + ko, d_bhi + ko, idesc, (!first_of_chunk || k > 0) ? 1u : 0u);
-              if (a.dbg & 4) continue;
-              umma_f16(d2, d_ahi + ko, d_blo + ko, idesc, (it > item.k0 || k > 0) ? 1u : 0u);
-              umma_f16(d2, d_alo + ko, d_bhi + ko, idesc, 1u);
-            }
-          }
-          // frees the smem slot once these MMAs retire (pair: in both CTAs)
-          if (PAIR) umma_commit_2sm(&empty_bar[st], 0x3); else umma_commit(&empty_bar[st]);
-          if (HALO && (it + 1 == item.k1 || (it + 1) % 9 == 0)) {     // last tap of this item on the current patch
-            if (PAIR) umma_commit_2sm(&patch_empty_bar[pb], 0x3); else umma_commit(&patch_empty_bar[pb]);
-          }
-          if (rel + 1 == chunk_stop) {
-            // D1[buf] (and, on the last chunk, D2[tbuf]) complete -- published to the epilogue warps of both CTAs
-            if (PAIR) umma_commit_2sm(&acc_full_bar[buf], 0x3); else umma_commit(&acc_full_bar[buf]);
-          }
-          }
-          __syncwarp();
-          if (rel + 1 == chunk_stop) ++gchunk;
-        }
-      }
-    }
-  } else if (RES && warp == Cfg::RES_WARP) {
-    // ONE lane walks this role (unlike the producer / issuer warps).  The whole-warp form -- 32 lanes polling the slab
-    // barriers, one elected lane issuing -- made the results of the two-stream pipeline differ from run to run at
-    // production size (scripts/determinism_diag.py; elect.sync or `lane == 0` alike; single stream never), which the
-    // single-lane form does not.  Not understood; the eight copies per tile are not worth the risk.
-    if (lane == 0) {
-      // ---------------- residual producer: the shortcut tile of each output tile, one 32-channel slab (hi + lo
-      // plane) per barrier pair, refilled as soon as its four epilogue warps have read the previous tile's slab.
-      // It runs on its own warp so that it never holds back the operand loads of the next tile.
-      const uint32_t slab_tx = 2u * (uint32_t)rows_valid * 64u;
-      uint32_t tile_iter = 0;                       // counts the tiles whose epilogue runs in this CTA
-      TcSched sched(a.sk_mode, total_tiles, n_iters, sched_id, sched_n);
-      TcItem item;
-      while (sched.next(item)) {
-        if (item.k0 != 0) continue;                 // partial contribution: no epilogue here
-        const int t = item.tile;
-        const int nt = t % a.n_tiles, mt = t / a.n_tiles;
-        const int x0 = (mt % a.tiles_w) * a.tw, y0 = ((mt / a.tiles_w) % a.tiles_h) * a.th;
-        const int img0 = (mt / (a.tiles_w * a.tiles_h)) * a.nb, n0 = nt * BN;
-        // in place: slab sl lands in part sl's output staging (same {hi, lo} x 8 KB layout, same 64 B swizzle)
-        uint8_t* res_base = INPLACE ? out_stage : res_stage;
-#pragma unroll
-        for (int i = 0; i < BN / 32; ++i) {
-          // consumption order: every column part works on its first slab, then on its second, ...
-          const int sl = (i % NSPLIT) * (BN / 32 / NSPLIT) + (i / NSPLIT);
-          mbar_wait(&res_empty_bar[sl], (tile_iter & 1u) ^ 1u);
-          {
-            mbar_arrive_expect_tx(&res_full_bar[sl], slab_tx);
-            tma_load_4d(res_base + (sl * 2 + 0) * 8192, &a.tm_r_hi, &res_full_bar[sl], n0 + sl * 32,
-                        x0 * a.res_stride, y0 * a.res_stride, img0);
-            tma_load_4d(res_base + (sl * 2 + 1) * 8192, &a.tm_r_lo, &res_full_bar[sl], n0 + sl * 32,
-                        x0 * a.res_stride, y0 * a.res_stride, img0);
+            tma_load_2d(bbase, &a.tm_b_hi, &full_bar[st], kcol, n0);
+            tma_load_2d(bbase + Cfg::B_BYTES, &a.tm_b_lo, &full_bar[st], kcol, n0);
           }
         }
-        ++tile_iter;
       }
     }
   } else {
-    // ---------------- epilogue warps 2..: TMEM lane quadrant = warp % 4, column part = (warp-2)/4
-    constexpr int HC = BN / NSPLIT;                     // columns owned by this warp
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;                   // column part 0..NSPLIT-1 (named `half` since the 2-part kernel)
-    const int row = q * 32 + lane;
-    const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16);
-    uint32_t gchunk = 0, tile_iter = 0, epi_iter = 0;
+    // ---------------- consumer warpgroups: rows wrow .. wrow + 63, columns wcol .. wcol + WN - 1 of the tile
+    setmaxnreg_inc<Cfg::CONSUMER_REGS>();
+    const int c = wg - 1;
+    const int ctid = threadIdx.x - 128;               // 0 .. 128 NCWG - 1 over the consumer warpgroups
+    const int wrow = (c & 1) * 64, wcol = (c >> 1) * WN;
+    const int lrow = ((threadIdx.x & 127) >> 5) * 16 + ((threadIdx.x & 31) >> 2);   // + 8 for the odd register pairs
+    const int lcol = 2 * (threadIdx.x & 3);
+    uint32_t git = 0, gpatch = 0;
     TcSched sched(a.sk_mode, total_tiles, n_iters, sched_id, sched_n);
     TcItem item;
-    for (; sched.next(item); ++tile_iter) {
+    while (sched.next(item)) {
       const int t = item.tile;
-      const int n_rel = item.k1 - item.k0;
-      const int nt = t % a.n_tiles, mt = PAIR ? 2 * (t / a.n_tiles) + pair_rank : t / a.n_tiles;
+      const int nt = t % a.n_tiles, mt = PAIR ? 2 * (t / a.n_tiles) + rank : t / a.n_tiles;
       const int x0 = (mt % a.tiles_w) * a.tw, y0 = ((mt / a.tiles_w) % a.tiles_h) * a.th;
       const int img0 = (mt / (a.tiles_w * a.tiles_h)) * a.nb;
-      const int n0 = nt * BN + half * HC;               // first channel of this warp's columns
-      const uint32_t tbuf = tile_iter & 1u;
-      bool valid = row < rows_valid;
-      int n_img = 0, oy = 0, ox = 0;
-      if (valid) {
-        const int nl = row / (a.th * a.tw);
-        const int rem = row % (a.th * a.tw);
-        n_img = img0 + nl; oy = y0 + rem / a.tw; ox = x0 + rem % a.tw;
-        valid = n_img < a.n && oy < a.ho && ox < a.wo;
-      }
-      const size_t opix = ((size_t)n_img * a.ho + oy) * a.wo + ox;
-      size_t rpix = 0;
-      if (a.res_hi)
-        rpix = ((size_t)n_img * a.res_h + (size_t)oy * a.res_stride) * a.res_w + (size_t)ox * a.res_stride;
+      const int n0 = nt * BN + wcol;
 
-      // ---- drain D1 chunks into fp32 registers (round-to-nearest adds)
-      float racc[HC];
+      float racc[NR];
 #pragma unroll
-      for (int j = 0; j < HC; ++j) racc[j] = 0.f;
-      for (int rel = 0; rel < n_rel; ++gchunk) {
-        rel = tc_chunk_end(rel, n_rel, a.chunk_head, a.chunk_tail);
-        const bool last_chunk = rel >= n_rel;
-        const uint32_t buf = gchunk & 1u;
-        mbar_wait(&acc_full_bar[buf], (gchunk >> 1) & 1u);
-        tc_fence_after();
+      for (int j = 0; j < NR; ++j) racc[j] = 0.f;
+      int patch_cc = -1;
+      uint32_t pb = 0;
+      for (int k = item.k0; k < item.k1; ++k, ++git) {
+        const uint32_t st = git % STAGES, ph = (git / STAGES) & 1u;
+        uint64_t d_ahi, d_alo;
+        if (HALO) {
+          const int cc = k / 9, tap = k - cc * 9;
+          if (cc != patch_cc) {
+            patch_cc = cc;
+            pb = gpatch & 1u;
+            mbar_wait(&patch_full_bar[pb], (gpatch >> 1) & 1u);
+            ++gpatch;
+          }
+          // view of the patch shifted by tap (r, s): row 8 g + j of the operand = patch pixel (g + r, j + s)
+          const int r = tap / 3, s = tap - r * 3;
+          const uint32_t pa = smem_u32(patch + pb * Cfg::PATCH_BYTES) + (uint32_t)(((wrow >> 3) + r) * TC_HALO_PITCH + s * 128);
+          d_ahi = make_sw128_kmajor_desc(pa, TC_HALO_PITCH);
+          d_alo = make_sw128_kmajor_desc(pa + TC_HALO_PLANE_BYTES, TC_HALO_PITCH);
+        }
+        mbar_wait(&full_bar[st], ph);
+        const uint32_t sa = smem_u32(stages + st * Cfg::STAGE_BYTES);
+        if (!HALO) {
+          d_ahi = make_sw128_kmajor_desc(sa + wrow * 128);
+          d_alo = make_sw128_kmajor_desc(sa + TC_A_BYTES + wrow * 128);
+        }
+        const uint64_t d_bhi = make_sw128_kmajor_desc(sa + Cfg::A_STAGE_BYTES + wcol * 128);
+        const uint64_t d_blo = make_sw128_kmajor_desc(sa + Cfg::A_STAGE_BYTES + Cfg::B_BYTES + wcol * 128);
+        float d[NR];
+        wgmma_fence();
+        // the 2^-11-times-smaller cross terms first, the hi*hi products last: each MMA's addition into the chain can
+        // cost up to one ulp of the value held, so only the last four additions act on the full-size partial sum
 #pragma unroll
-        for (int ch = 0; ch < HC / 32; ++ch) {
-          if (n0 + ch * 32 < a.cout && !(a.dbg & 2)) {   // warp-uniform
-            uint32_t r[32];
-            tmem_ld_32x32b_x32(lane_base + (uint32_t)(buf * BN + half * HC + ch * 32), r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) racc[ch * 32 + j] = __fadd_rn(racc[ch * 32 + j], __uint_as_float(r[j]));
+        for (int kk = 0; kk < 4; ++kk) {
+          const uint64_t ko = (uint64_t)(kk * 2);       // 16 fp16 = 32 B = 2 x 16 B descriptor units
+          if constexpr (WN == 128) {
+            wgmma_m64n128k16_f16(d, d_ahi + ko, d_blo + ko, kk > 0 ? 1u : 0u);
+            wgmma_m64n128k16_f16(d, d_alo + ko, d_bhi + ko, 1u);
+          } else {
+            wgmma_m64n64k16_f16(d, d_ahi + ko, d_blo + ko, kk > 0 ? 1u : 0u);
+            wgmma_m64n64k16_f16(d, d_alo + ko, d_bhi + ko, 1u);
           }
         }
-        if (last_chunk) {                                // the last commit also covers every D2 MMA of the tile
 #pragma unroll
-          for (int ch = 0; ch < HC / 32; ++ch) {
-            if (n0 + ch * 32 < a.cout) {
-              uint32_t r[32];
-              tmem_ld_32x32b_x32(lane_base + (uint32_t)((2 + tbuf) * BN + half * HC + ch * 32), r);
-              tmem_ld_wait();
-#pragma unroll
-              for (int j = 0; j < 32; ++j) racc[ch * 32 + j] = __fadd_rn(racc[ch * 32 + j], __uint_as_float(r[j]));
-            }
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) { if (PAIR) mbar_arrive_leader(&d2_empty_bar[tbuf]); else mbar_arrive(&d2_empty_bar[tbuf]); }
+        for (int kk = 0; kk < 4; ++kk) {
+          const uint64_t ko = (uint64_t)(kk * 2);
+          if constexpr (WN == 128) wgmma_m64n128k16_f16(d, d_ahi + ko, d_bhi + ko, 1u);
+          else wgmma_m64n64k16_f16(d, d_ahi + ko, d_bhi + ko, 1u);
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) { if (PAIR) mbar_arrive_leader(&acc_empty_bar[buf]); else mbar_arrive(&acc_empty_bar[buf]); }
+        wgmma_commit();
+        wgmma_wait0();
+        if ((threadIdx.x & 127) == 0) {               // this warpgroup is done with the slot (pair: in both CTAs)
+          mbar_arrive(&empty_bar[st]);
+          if (PAIR) mbar_arrive_cluster(&empty_bar[st], (uint32_t)(rank ^ 1));
+          if (HALO && (k + 1 == item.k1 || (k + 1) % 9 == 0)) mbar_arrive(&patch_empty_bar[pb]);
+        }
+#pragma unroll
+        for (int j = 0; j < NR; ++j) racc[j] = __fadd_rn(racc[j], d[j]);
       }
 
-      // ---- stream-K fix-up
+      // ---- stream-K fix-up.  Partial-sum layout [column][row] of the 128 x BN tile, one slot per CTA.
       if (item.k0 != 0) {
-        // this CTA continued a tile somebody else started: publish the partial sums, no epilogue.  Layout
-        // [column][row] so that a warp (32 consecutive rows) writes 128 contiguous bytes per column.
-        float* wsp = a.sk_partials + (size_t)blockIdx.x * (128 * BN) + (size_t)(half * HC) * 128 + row;
+        // this CTA continued a tile somebody else started: publish the partial sums, no epilogue
+        float* wsp = a.sk_partials + (size_t)blockIdx.x * (128 * BN);
 #pragma unroll
-        for (int j = 0; j < HC; ++j) wsp[j * 128] = racc[j];
+        for (int j = 0; j < NR; ++j) {
+          const int row = wrow + lrow + ((j & 2) ? 8 : 0), col = wcol + (j >> 2) * 8 + lcol + (j & 1);
+          wsp[col * 128 + row] = racc[j];
+        }
         __threadfence();
-        named_bar_sync(7, 32 * EPI_WARPS);               // all epilogue warps have written and fenced
-        if (warp == 2 && lane == 0)
+        named_bar_sync(1, 128 * NCWG);                 // all consumer threads have written and fenced
+        if (ctid == 0)
           asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(a.sk_flags + blockIdx.x), "r"(a.sk_epoch) : "memory");
         continue;
       }
       if (item.k1 != n_iters) {
-        // this CTA holds the head of the tile: the following CTAs hold the rest (they computed it first thing)
+        // this CTA holds the head of the tile: the following units hold the rest (they computed it first thing); in a
+        // pair the partner in unit u is the CTA of the same rank, slot 2 u + rank
         const long long tile_end = (long long)(item.tile + 1) * n_iters;
-        // scheduling units after this one hold the rest of the tile; in a CTA pair every unit is a pair and this CTA's
-        // partner in unit u is the CTA of the same rank: its partial slot / flag index is 2 u + rank
         int last_unit = sched_id;
         for (int unit = sched_id + 1;; ++unit) {
-          const int cta = PAIR ? 2 * unit + pair_rank : unit;
+          const int cta = PAIR ? 2 * unit + rank : unit;
           int seen;
           do {
             asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(seen) : "l"(a.sk_flags + cta) : "memory");
           } while (seen != a.sk_epoch);
-          const float* wsp = a.sk_partials + (size_t)cta * (128 * BN) + (size_t)(half * HC) * 128 + row;
+          const float* wsp = a.sk_partials + (size_t)cta * (128 * BN);
 #pragma unroll
-          for (int j = 0; j < HC; ++j) racc[j] = __fadd_rn(racc[j], __ldcg(wsp + j * 128));
+          for (int j = 0; j < NR; ++j) {
+            const int row = wrow + lrow + ((j & 2) ? 8 : 0), col = wcol + (j >> 2) * 8 + lcol + (j & 1);
+            racc[j] = __fadd_rn(racc[j], __ldcg(wsp + col * 128 + row));
+          }
           last_unit = unit;
           if (TcSched::range_end(unit, total_tiles, n_iters, sched_n) >= tile_end) break;
         }
         // every flag is consumed by exactly one CTA (the one holding the tile's head): clear it once all
-        // epilogue warps are past their polls, so a REPLAY of this launch with the same epoch (CUDA graph) starts clean
-        named_bar_sync(7, 32 * EPI_WARPS);
-        if (warp == 2 && lane == 0)
+        // consumer threads are past their polls, so a REPLAY of this launch with the same epoch (CUDA graph) starts clean
+        named_bar_sync(1, 128 * NCWG);
+        if (ctid == 0)
           for (int unit = sched_id + 1; unit <= last_unit; ++unit)
-            asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(a.sk_flags + (PAIR ? 2 * unit + pair_rank : unit)), "r"(0) : "memory");
+            asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(a.sk_flags + (PAIR ? 2 * unit + rank : unit)), "r"(0) : "memory");
       }
 
-      // ---- scale/bias (folded BN) -> +residual -> activation -> store (overlaps the next tile's MMAs)
-      // split outputs: each column half (4 warps) stages a 128 x 32-channel slab per plane in shared
-      // memory (64 B swizzle) and one thread issues the two bulk tensor stores -- fully coalesced, and
-      // TMA clips partial tiles; fp32 outputs (head layers) are written directly.
-      uint8_t* st_hi = out_stage + half * (2 * 128 * 64);
-      uint8_t* st_lo = st_hi + 128 * 64;
-      const bool store_leader = ((warp - 2) & 3) == 0 && lane == 0;     // one issuing thread per column half
+      // ---- scale/bias (folded BN) -> +residual -> activation -> store; two rows per thread, column pairs
 #pragma unroll
-      for (int ch = 0; ch < HC / 32; ++ch) {
-        const int c0 = n0 + ch * 32;
-        if (c0 < a.cout) {                               // uniform over the 4 warps of this column half
-          float v[32];
-          const bool full = (c0 + 32 <= a.cout);
-          // scale / bias vectors are padded to cout_pad: 16 B loads are always in bounds
+      for (int hrow = 0; hrow < 2; ++hrow) {
+        const int row = wrow + lrow + hrow * 8;
+        bool valid = row < rows_valid;
+        int n_img = 0, oy = 0, ox = 0;
+        if (valid) {
+          const int nl = row / (a.th * a.tw);
+          const int rem = row % (a.th * a.tw);
+          n_img = img0 + nl; oy = y0 + rem / a.tw; ox = x0 + rem % a.tw;
+          valid = n_img < a.n && oy < a.ho && ox < a.wo;
+        }
+        const size_t opix = ((size_t)n_img * a.ho + oy) * a.wo + ox;
+        size_t rpix = 0;
+        if (a.res_hi)
+          rpix = ((size_t)n_img * a.res_h + (size_t)oy * a.res_stride) * a.res_w + (size_t)ox * a.res_stride;
+        bool ovf = false;
 #pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            const float4 sc = __ldg(reinterpret_cast<const float4*>(a.scale + c0) + g);
-            const float4 bi = __ldg(reinterpret_cast<const float4*>(a.bias + c0) + g);
-            v[g * 4 + 0] = fmaf(racc[ch * 32 + g * 4 + 0], sc.x, bi.x);
-            v[g * 4 + 1] = fmaf(racc[ch * 32 + g * 4 + 1], sc.y, bi.y);
-            v[g * 4 + 2] = fmaf(racc[ch * 32 + g * 4 + 2], sc.z, bi.z);
-            v[g * 4 + 3] = fmaf(racc[ch * 32 + g * 4 + 3], sc.w, bi.w);
+        for (int jb = 0; jb < WN / 8; ++jb) {
+          const int c0 = n0 + jb * 8 + lcol;
+          if (!valid || c0 >= a.cout) continue;
+          // scale / bias vectors are padded to cout_pad (even): 8 B loads are always in bounds
+          const float2 sc = __ldg(reinterpret_cast<const float2*>(a.scale + c0));
+          const float2 bi = __ldg(reinterpret_cast<const float2*>(a.bias + c0));
+          float v0 = fmaf(racc[jb * 4 + hrow * 2 + 0], sc.x, bi.x);
+          float v1 = fmaf(racc[jb * 4 + hrow * 2 + 1], sc.y, bi.y);
+          if (a.res_hi) {              // residual tensors always have cout % 32 == 0 channels
+            const __half2 h2 = *reinterpret_cast<const __half2*>(a.res_hi + rpix * a.cout + c0);
+            const __half2 l2 = *reinterpret_cast<const __half2*>(a.res_lo + rpix * a.cout + c0);
+            v0 = add_f16_pair(v0, __low2half(h2), __low2half(l2));
+            v1 = add_f16_pair(v1, __high2half(h2), __high2half(l2));
           }
-          if (RES) {                   // residual slab was TMA-prefetched into shared memory (64 B swizzle)
-            const int sl = half * (HC / 32) + ch;
-            mbar_wait(&res_full_bar[sl], epi_iter & 1u);
-            const int rsw = (row >> 1) & 3;
-            const uint8_t* rbase = INPLACE ? out_stage : res_stage;     // in place: this part's own staging slab
-            const uint8_t* rh = rbase + (sl * 2 + 0) * 8192 + row * 64;
-            const uint8_t* rl = rbase + (sl * 2 + 1) * 8192 + row * 64;
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              const uint4 h4 = *reinterpret_cast<const uint4*>(rh + ((g ^ rsw) << 4));
-              const uint4 l4 = *reinterpret_cast<const uint4*>(rl + ((g ^ rsw) << 4));
-              const __half* ph = reinterpret_cast<const __half*>(&h4);
-              const __half* pl = reinterpret_cast<const __half*>(&l4);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) v[g * 8 + j] = add_f16_pair(v[g * 8 + j], ph[j], pl[j]);
-            }
-            if (!INPLACE) {            // (in place the slab is released by the store leader once the store has read it)
-              __syncwarp();            // this warp is done with the slab
-              if (lane == 0) mbar_arrive(&res_empty_bar[sl]);
-            }
-          } else if (a.res_hi && valid) {     // residual tensors always have cout % 32 == 0 channels
-            const uint4* rh = reinterpret_cast<const uint4*>(a.res_hi + rpix * a.cout + c0);
-            const uint4* rl = reinterpret_cast<const uint4*>(a.res_lo + rpix * a.cout + c0);
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              uint4 h4 = __ldg(rh + g), l4 = __ldg(rl + g);
-              const __half* ph = reinterpret_cast<const __half*>(&h4);
-              const __half* pl = reinterpret_cast<const __half*>(&l4);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) v[g * 8 + j] = add_f16_pair(v[g * 8 + j], ph[j], pl[j]);
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = apply_act(v[j], a.act);
+          v0 = apply_act(v0, a.act);
+          v1 = apply_act(v1, a.act);
           if (a.out_f32) {
-            if (valid) {
-              float* op = a.out_f32 + opix * a.cout + c0;
-              if (full && (a.cout % 4) == 0) {
-#pragma unroll
-                for (int g = 0; g < 8; ++g)
-                  reinterpret_cast<float4*>(op)[g] = make_float4(v[g * 4], v[g * 4 + 1], v[g * 4 + 2], v[g * 4 + 3]);
-              } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                  if (c0 + j < a.cout) op[j] = v[j];
-              }
+            float* op = a.out_f32 + opix * a.cout + c0;
+            if ((a.cout & 1) == 0) {
+              *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
+            } else {
+              op[0] = v0;
+              if (c0 + 1 < a.cout) op[1] = v1;
             }
-          } else {            // split outputs always have cout % 32 == 0
-            // packed split: hi = rn16(v), lo = rn16(v - hi), two channels per cvt.rn.f16x2.f32; an fp16
-            // overflow shows up as inf/nan in the hi plane (tracked as a running |max| with NaN propagation)
-            uint4 hv[4], lv[4];
-            __half2* ph = reinterpret_cast<__half2*>(hv);
-            __half2* pl = reinterpret_cast<__half2*>(lv);
-            __half2 amax = __float2half2_rn(0.f);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              split2_f32(v[2 * j], v[2 * j + 1], ph[j], pl[j]);
-              amax = __hmax2_nan(amax, __habs2(ph[j]));
-            }
-            const uint32_t ab = *reinterpret_cast<const uint32_t*>(&amax);
-            const bool ovf = ((ab & 0x7C00u) == 0x7C00u) || ((ab & 0x7C000000u) == 0x7C000000u);
-            if (ovf && valid && a.overflow) atomicOr(a.overflow, 1);
-            if (!INPLACE) {            // (in place: res_full already implies that the previous store has read the slab)
-              if (store_leader) bulk_wait_group_read0();   // the previous slab's stores have drained the staging
-              named_bar_sync(1 + half, 128);
-            }
-            const int sw = (row >> 1) & 3;               // SWIZZLE_64B: 16 B chunk index ^= address bits [7:8]
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              *reinterpret_cast<uint4*>(st_hi + row * 64 + ((g ^ sw) << 4)) = hv[g];
-              *reinterpret_cast<uint4*>(st_lo + row * 64 + ((g ^ sw) << 4)) = lv[g];
-            }
-            fence_proxy_async();
-            named_bar_sync(1 + half, 128);
-            if (store_leader) {
-              if ((!PAIR || mt < m_tiles) && !(a.dbg & 8)) {       // (the odd CTA's tile past the last M tile has nothing to store)
-                tma_store_4d(&a.tm_o_hi, st_hi, c0, x0, y0, img0);
-                tma_store_4d(&a.tm_o_lo, st_lo, c0, x0, y0, img0);
-              }
-              bulk_commit_group();
-              if (INPLACE) {           // hand the slab back to the residual producer once the store has read it
-                bulk_wait_group_read0();
-                mbar_arrive(&res_empty_bar[half]);
-              }
-            }
+          } else {                     // split outputs always have cout % 32 == 0
+            // packed split: hi = rn16(v), lo = rn16(v - hi); an fp16 overflow shows up as inf/nan in the hi plane
+            __half2 h2, l2;
+            split2_f32(v0, v1, h2, l2);
+            const uint32_t ab = *reinterpret_cast<const uint32_t*>(&h2);
+            ovf |= ((ab & 0x7C00u) == 0x7C00u) || ((ab & 0x7C000000u) == 0x7C000000u);
+            *reinterpret_cast<__half2*>(a.out_hi + opix * a.cout + c0) = h2;
+            *reinterpret_cast<__half2*>(a.out_lo + opix * a.cout + c0) = l2;
           }
         }
+        if (ovf && a.overflow) atomicOr(a.overflow, 1);
       }
-      ++epi_iter;
     }
-    if (((warp - 2) & 3) == 0 && lane == 0) bulk_wait_group0();   // all output stores complete before exit
   }
-  tc_fence_before();
-  __syncthreads();
-  if (PAIR) cluster_sync_all();          // the peer's shared memory / TMEM / barriers stay alive until both CTAs are done
-  if (warp == 1) {
-    __syncwarp();
-    if (PAIR) tmem_dealloc_2sm(tmem_base, Cfg::TMEM_COLS); else tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
+  // PAIR: the peer's shared memory and barriers must stay alive until both CTAs are done with them
+  if (PAIR) cluster_sync_all();
 }
 
 // ---------------------------------------------------------------- host: TMA descriptors
@@ -875,21 +611,6 @@ static CUtensorMap make_map_act(const __half* base, int n, int h, int w, int c, 
   return m;
 }
 
-// output / residual plane: box {32 ch, tw, th, nb} (x traversal stride rs for subsampled residuals),
-// 64 B swizzle (matches the epilogue's staging layout)
-static CUtensorMap make_map_out(const __half* base, int n, int h, int w, int c, int nb, int th, int tw, int rs = 1) {
-  CUtensorMap m;
-  cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
-  cuuint64_t strides[3] = {(cuuint64_t)c * 2, (cuuint64_t)w * c * 2, (cuuint64_t)h * w * c * 2};
-  cuuint32_t box[4] = {32, (cuuint32_t)(tw * rs), (cuuint32_t)(th * rs), (cuuint32_t)nb};
-  cuuint32_t es[4] = {1, (cuuint32_t)rs, (cuuint32_t)rs, 1};
-  CUresult r = get_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)base, dims, strides, box, es,
-                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
-                               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) throw Error(-2, "cuTensorMapEncodeTiled(output) failed: " + std::to_string((int)r));
-  return m;
-}
-
 static CUtensorMap make_map_wgt(const __half* base, int rows, int kdim, int bn) {
   CUtensorMap m;
   cuuint64_t dims[2] = {(cuuint64_t)kdim, (cuuint64_t)rows};
@@ -921,15 +642,6 @@ static CUtensorMap cached_act_map(const __half* base, int n, int h, int w, int c
   if (it != g_map_cache.end()) return it->second;
   if (g_map_cache.size() > 4096) g_map_cache.clear();
   CUtensorMap m = make_map_act(base, n, h, w, c, nb, th, tw, stride, pix_pitch, row_pitch, img_pitch);
-  g_map_cache[k] = m;
-  return m;
-}
-static CUtensorMap cached_out_map(const __half* base, int n, int h, int w, int c, int nb, int th, int tw, int rs = 1) {
-  std::lock_guard<std::mutex> lk(g_map_mutex);
-  MapKey k{base, n, h, w, -c, nb, th * 16 + rs, tw};       // negative c: output-map key space
-  auto it = g_map_cache.find(k);
-  if (it != g_map_cache.end()) return it->second;
-  CUtensorMap m = make_map_out(base, n, h, w, c, nb, th, tw, rs);
   g_map_cache[k] = m;
   return m;
 }
@@ -973,7 +685,7 @@ bool conv_tc_supported(const ConvLayer& L, const ConvIO& io) {
 
 // SMs a persistent conv launch may occupy.  While the engine runs its two-stream pipeline it leaves
 // io.sm_reserve SMs free so the few-CTA latency-bound kernels (sort, NMS scan) of the other half-batch
-// run concurrently instead of waiting behind a 148-CTA persistent grid (measured +1.7 % images/s at 8-16).
+// run concurrently instead of waiting behind a persistent grid that fills every SM.
 // The count is cached per DEVICE (an engine may live on any device of the process).
 int device_sm_count() {
   static int n[LUMI_MAX_DEVICES] = {0};
@@ -1011,31 +723,50 @@ void conv_workspace_free(ConvWorkspace& w) {
   w.partials = nullptr; w.flags = nullptr; w.ctas = 0;
 }
 
-template <int BN, int STAGES, bool RES, int NSPLIT = 2, bool INPLACE = false, bool PAIR = false, bool HALO = false>
+template <int BN, int STAGES, int NCWG = 2, bool PAIR = false, bool HALO = false>
 static void launch_tc_cfg(const TcArgs& a, ConvWorkspace* sk, int streamk, int sm_reserve, cudaStream_t st) {
-  using Cfg = TcCfg<BN, STAGES, RES, NSPLIT, INPLACE, PAIR, HALO>;
+  using Cfg = TcCfg<BN, STAGES, NCWG, PAIR, HALO>;
+  auto kernel = conv_tc_kernel<BN, STAGES, NCWG, PAIR, HALO>;
   // cudaFuncSetAttribute is per device: one flag per (kernel instance, device)
   static bool attr_set[LUMI_MAX_DEVICES] = {false};
   int dev = 0;
   LUMI_CUDA_CHECK(cudaGetDevice(&dev));
   if (dev < 0 || dev >= LUMI_MAX_DEVICES || !__atomic_load_n(&attr_set[dev], __ATOMIC_ACQUIRE)) {
-    LUMI_CUDA_CHECK(cudaFuncSetAttribute(conv_tc_kernel<BN, STAGES, RES, NSPLIT, INPLACE, PAIR, HALO>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    LUMI_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     if (dev >= 0 && dev < LUMI_MAX_DEVICES) __atomic_store_n(&attr_set[dev], true, __ATOMIC_RELEASE);
   }
   const long m_tiles = (long)a.tiles_w * a.tiles_h * a.tiles_n;
   const long total = (PAIR ? (m_tiles + 1) / 2 : m_tiles) * a.n_tiles;      // scheduling units (tiles or tile pairs)
   const int sms = sm_budget(sm_reserve);
+  int units_max = PAIR ? sms / 2 : sms;
+  if (PAIR) {
+    // stream-K needs every cluster of the grid resident at once: never launch more pairs than can be co-scheduled
+    static int max_clusters[LUMI_MAX_DEVICES] = {0};
+    int mc = (dev >= 0 && dev < LUMI_MAX_DEVICES) ? __atomic_load_n(&max_clusters[dev], __ATOMIC_RELAXED) : 0;
+    if (!mc) {
+      cudaLaunchConfig_t cfg;
+      std::memset(&cfg, 0, sizeof(cfg));
+      cfg.gridDim = dim3(2 * units_max, 1, 1);
+      cfg.blockDim = dim3(Cfg::THREADS, 1, 1);
+      cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
+      cudaLaunchAttribute at[1];
+      at[0].id = cudaLaunchAttributeClusterDimension;
+      at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+      cfg.attrs = at;
+      cfg.numAttrs = 1;
+      LUMI_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&mc, kernel, &cfg));
+      LUMI_REQUIRE(mc > 0, "conv_tc: the 2-CTA cluster kernel cannot be scheduled on this device");
+      if (dev >= 0 && dev < LUMI_MAX_DEVICES) __atomic_store_n(&max_clusters[dev], mc, __ATOMIC_RELAXED);
+    }
+    if (units_max > mc) units_max = mc;
+  }
   TcArgs args = a;
   args.sk_mode = 0;
-  // scheduling units: CTAs, or 2-CTA clusters for the pair kernel
-  const int units_max = PAIR ? sms / 2 : sms;
   int units = (int)(total < units_max ? total : units_max);             // persistent: one CTA (pair) per SM (pair)
   if (sk && sk->partials && streamk > 0 && sms <= sk->ctas) {
     // stream-K when whole-tile scheduling would leave SMs idle in the last wave (or has fewer tiles than SMs).
-    // It balances K iterations, not epilogues, and every CTA pays one partial-tile write and one read: measured
-    // (profiles/r1_streamk_per_layer.txt) it wins 13-26 % on the long-K layers (3x3 with C_in >= 128,
-    // 1x1 with C_in >= 1024, the RPN conv) and loses 5-35 % on short-K, epilogue-bound ones -- hence the K floor.
+    // It balances K iterations, not epilogues, and every CTA pays one partial-tile write and one read, so it is
+    // kept to the long-K layers (3x3 with C_in >= 128, 1x1 with C_in >= 1024, the RPN conv).
     const long n_iters = (long)a.kh * a.kw * (a.cin >> 6);
     const double waves = (double)total / units_max;
     const double eff = waves / std::ceil(waves);
@@ -1061,12 +792,10 @@ static void launch_tc_cfg(const TcArgs& a, ConvWorkspace* sk, int streamk, int s
     at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     cfg.attrs = at;
     cfg.numAttrs = 1;
-    LUMI_CUDA_CHECK(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, STAGES, RES, NSPLIT, INPLACE, PAIR, HALO>, args));
-    count_launch();
-    return;
+    LUMI_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, args));
+  } else {
+    kernel<<<units, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(args);
   }
-  const int grid = units;
-  conv_tc_kernel<BN, STAGES, RES, NSPLIT, INPLACE, PAIR, HALO><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(args);
   count_launch();
   LUMI_CUDA_CHECK(cudaGetLastError());
 }
@@ -1082,7 +811,8 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
   const int bn = (L.cout_pad % 128 == 0) ? 128 : 64;
   // halo-patch kernels (3x3, stride 1, rate 1, SAME): tiles of th x 8 pixels of one image, th <= 16 chosen so that the
   // rows of the map split evenly.  They trade M-tile occupancy (th * 8 <= 128 rows, and the weights stream once per
-  // tile) for ~6x less activation traffic, so they are used while the tile count stays within io.halo_tiles_pct of the generic one.
+  // tile) for ~6x less activation traffic, so they are used while the tile count stays within io.halo_tiles_pct of the
+  // generic one.
   bool halo = false;
   if (io.halo && L.kh == 3 && L.kw == 3 && L.stride == 1 && L.rate == 1 && io.pad_t == 1 && io.pad_l == 1 &&
       !io.res.hi && !io.out_f32 && !io.in_pix_pitch && !io.in_row_pitch && !io.in_img_pitch) {
@@ -1091,22 +821,21 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
     const long halo_tiles = (long)io.in.n * h_tiles * cdiv(io.wo, TC_HALO_TW);
     if (halo_tiles * 100 <= std_tiles * io.halo_tiles_pct) { halo = true; nb = 1; th = h_th; tw = TC_HALO_TW; }
   }
-  if (halo) {            // the activation maps describe the PATCH box {64 ch, 10, th + 2, 1}
-    a.tm_a_hi = cached_act_map(io.in.hi, io.in.n, io.in.h, io.in.w, io.in.c, 1, th + 2, tw + 2, 1, 0, 0, 0);
-    a.tm_a_lo = cached_act_map(io.in.lo, io.in.n, io.in.h, io.in.w, io.in.c, 1, th + 2, tw + 2, 1, 0, 0, 0);
+  if (halo) {            // the activation maps describe one patch row: box {64 ch, 10, 1, 1}
+    a.tm_a_hi = cached_act_map(io.in.hi, io.in.n, io.in.h, io.in.w, io.in.c, 1, 1, TC_HALO_TW + 2, 1, 0, 0, 0);
+    a.tm_a_lo = cached_act_map(io.in.lo, io.in.n, io.in.h, io.in.w, io.in.c, 1, 1, TC_HALO_TW + 2, 1, 0, 0, 0);
   } else {
-  a.tm_a_hi = cached_act_map(io.in.hi, io.in.n, io.in.h, io.in.w, io.in.c, nb, th, tw, L.stride, io.in_pix_pitch,
-                             io.in_row_pitch, io.in_img_pitch);
-  a.tm_a_lo = cached_act_map(io.in.lo, io.in.n, io.in.h, io.in.w, io.in.c, nb, th, tw, L.stride, io.in_pix_pitch,
-                             io.in_row_pitch, io.in_img_pitch);
+    a.tm_a_hi = cached_act_map(io.in.hi, io.in.n, io.in.h, io.in.w, io.in.c, nb, th, tw, L.stride, io.in_pix_pitch,
+                               io.in_row_pitch, io.in_img_pitch);
+    a.tm_a_lo = cached_act_map(io.in.lo, io.in.n, io.in.h, io.in.w, io.in.c, nb, th, tw, L.stride, io.in_pix_pitch,
+                               io.in_row_pitch, io.in_img_pitch);
   }
+  // CTA pairs on the long-K layers: each CTA of a pair loads (and multicasts) 64 of the 128 weight rows
+  const long n_iters_all = (long)L.kh * L.kw * (L.cin >> 6);
+  const bool pair = io.cta2 && bn == 128 && !io.out_f32 && n_iters_all >= io.cta2;
   const int kdim = L.kh * L.kw * L.cin;
-  a.tm_b_hi = cached_wgt_map(L.w_hi, L.cout_pad, kdim, bn);
-  a.tm_b_lo = cached_wgt_map(L.w_lo, L.cout_pad, kdim, bn);
-  if (!io.out_f32) {
-    a.tm_o_hi = cached_out_map(io.out.hi, io.in.n, io.ho, io.wo, L.cout, nb, th, tw);
-    a.tm_o_lo = cached_out_map(io.out.lo, io.in.n, io.ho, io.wo, L.cout, nb, th, tw);
-  }
+  a.tm_b_hi = cached_wgt_map(L.w_hi, L.cout_pad, kdim, pair ? bn / 2 : bn);
+  a.tm_b_lo = cached_wgt_map(L.w_lo, L.cout_pad, kdim, pair ? bn / 2 : bn);
   a.scale = L.scale_tc; a.bias = L.bias;
   a.out_hi = io.out.hi; a.out_lo = io.out.lo; a.out_f32 = io.out_f32;
   a.res_hi = io.res.hi; a.res_lo = io.res.lo; a.res_h = io.res.h; a.res_w = io.res.w; a.res_stride = io.res_stride;
@@ -1116,58 +845,20 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
   a.tiles_w = cdiv(io.wo, tw); a.tiles_h = cdiv(io.ho, th); a.tiles_n = cdiv(io.in.n, nb);
   a.n_tiles = L.cout_pad / bn;
   a.stride = L.stride;
-  a.chunk_head = 2 * TC_CHUNK_STAGES;
-  a.chunk_tail = (io.chunk_tail >= 1 && io.chunk_tail <= TC_CHUNK_STAGES) ? io.chunk_tail : TC_CHUNK_STAGES;
   a.overflow = io.overflow_flag;
-  a.halo_baseoff = io.halo_baseoff;
-  {
-    // bits 1-8 produce WRONG results (they remove work to time the rest): honoured only together with
-    // LUMI_ALLOW_WRONG_RESULTS=1, which bench.py / the tests never set
-    static const int dbg = [] {
-      const char* e = std::getenv("LUMI_CONV_DBG");
-      int v = e ? std::atoi(e) : 0;
-      const char* ok = std::getenv("LUMI_ALLOW_WRONG_RESULTS");
-      if ((v & 15) && !(ok && std::atoi(ok) == 1)) v &= ~15;
-      return v;
-    }();
-    a.dbg = dbg;
-  }
+  // operands per stage: 64 KB (BN = 128) or 48 KB (BN = 64), B only for HALO (next to two 72 KB patch buffers)
   if (halo) {
-    if (bn == 128 && io.halo >= 2) {           // CTA pair: each CTA its own patch, half of the weight tile
-      a.tm_b_hi = cached_wgt_map(L.w_hi, L.cout_pad, kdim, 64);
-      a.tm_b_lo = cached_wgt_map(L.w_lo, L.cout_pad, kdim, 64);
-      launch_tc_cfg<128, 6, false, 2, false, true, true>(a, io.sk, io.streamk, io.sm_reserve, st);
-    } else if (bn == 128) {
-      launch_tc_cfg<128, 3, false, 2, false, false, true>(a, io.sk, io.streamk, io.sm_reserve, st);
-    } else {
-      launch_tc_cfg<64, 6, false, 2, false, false, true>(a, io.sk, io.streamk, io.sm_reserve, st);
-    }
+    if (pair) launch_tc_cfg<128, 2, 2, true, true>(a, io.sk, io.streamk, io.sm_reserve, st);
+    else if (bn == 128) launch_tc_cfg<128, 2, 2, false, true>(a, io.sk, io.streamk, io.sm_reserve, st);
+    else launch_tc_cfg<64, 4, 2, false, true>(a, io.sk, io.streamk, io.sm_reserve, st);
     return;
   }
-  const bool res_tma = io.res.hi != nullptr && bn == 128 && L.cout % 128 == 0 && !io.out_f32;
-  // CTA pairs (cta_group::2) for the long-K layers without residual: 48 KB of operands per CTA and stage, four stages
-  const long n_iters_all = (long)L.kh * L.kw * (L.cin >> 6);
-  if (io.cta2 && bn == 128 && !io.res.hi && !io.out_f32 && n_iters_all >= io.cta2) {
-    a.tm_b_hi = cached_wgt_map(L.w_hi, L.cout_pad, kdim, 64);       // each CTA of a pair loads 64 of the 128 B rows
-    a.tm_b_lo = cached_wgt_map(L.w_lo, L.cout_pad, kdim, 64);
-    launch_tc_cfg<128, 4, false, 2, false, true>(a, io.sk, io.streamk, io.sm_reserve, st);
-    return;
-  }
-  // 16 epilogue warps for the shortest-K layers (io.epi16 = largest K-stage count that uses them; measured per layer,
-  // profiles/r2_conv_variants.txt: they win on one-stage tiles (C_in = 64) and lose from four stages up, where their
-  // two operand stages cost more than the faster epilogue gains)
-  const bool epi16 = io.epi16 && bn == 128 && !io.out_f32 && (long)L.kh * L.kw * (L.cin >> 6) <= io.epi16;
-  if (res_tma) {          // residual tile prefetched by TMA (box over the unit's input, subsampled by res_stride)
-    a.tm_r_hi = cached_out_map(io.res.hi, io.res.n, io.res.h, io.res.w, io.res.c, nb, th, tw, io.res_stride);
-    a.tm_r_lo = cached_out_map(io.res.lo, io.res.n, io.res.h, io.res.w, io.res.c, nb, th, tw, io.res_stride);
-    if (epi16) launch_tc_cfg<128, 2, true, 4, true>(a, io.sk, io.streamk, io.sm_reserve, st);
-    else launch_tc_cfg<128, 2, true>(a, io.sk, io.streamk, io.sm_reserve, st);
-  } else if (bn == 128) {
-    if (epi16 && !io.res.hi) launch_tc_cfg<128, 2, false, 4, false>(a, io.sk, io.streamk, io.sm_reserve, st);
-    else launch_tc_cfg<128, 3, false>(a, io.sk, io.streamk, io.sm_reserve, st);
-  } else {
-    launch_tc_cfg<64, 4, false>(a, io.sk, io.streamk, io.sm_reserve, st);
-  }
+  // four consumer warpgroups (sixteen epilogue warps) for the shortest-K layers (io.epi16 = largest K-slice count)
+  const bool epi16 = io.epi16 && bn == 128 && !io.out_f32 && n_iters_all <= io.epi16;
+  if (pair) launch_tc_cfg<128, 3, 2, true>(a, io.sk, io.streamk, io.sm_reserve, st);
+  else if (epi16) launch_tc_cfg<128, 3, 4>(a, io.sk, io.streamk, io.sm_reserve, st);
+  else if (bn == 128) launch_tc_cfg<128, 3>(a, io.sk, io.streamk, io.sm_reserve, st);
+  else launch_tc_cfg<64, 4>(a, io.sk, io.streamk, io.sm_reserve, st);
 }
 
 // ---------------------------------------------------------------- host: weight packing
@@ -1176,7 +867,7 @@ void conv_layer_upload(ConvLayer& L, const float* w, const float* scale, const f
   const size_t nw = kdim * L.cout;
   LUMI_CUDA_CHECK(cudaMalloc(&L.w_f32, nw * sizeof(float)));
   LUMI_CUDA_CHECK(cudaMemcpy(L.w_f32, w, nw * sizeof(float), cudaMemcpyHostToDevice));
-  const int cpad = cdiv(L.cout, 128) * 128;        // vectors padded so the tcgen05 epilogue can use 16 B loads
+  const int cpad = cdiv(L.cout, 128) * 128;        // vectors padded so the tensor-core epilogue can use vector loads
   std::vector<float> sc(cpad, 1.f), bi(cpad, 0.f);
   if (scale) std::memcpy(sc.data(), scale, L.cout * sizeof(float));
   if (bias) std::memcpy(bi.data(), bias, L.cout * sizeof(float));

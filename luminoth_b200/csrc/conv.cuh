@@ -14,7 +14,7 @@ struct ConvLayer {
   float* w_f32 = nullptr;
   float* scale = nullptr;   // [cout]  (BN gamma*rsqrt(var+eps), or 1)
   float* bias = nullptr;    // [cout]  (BN beta - mean*scale, or conv bias)
-  // tcgen05 form: [cout_pad][kh*kw*cin] fp16 hi/lo planes of w * 2^e[c]; scale_tc = scale * 2^-e[c]
+  // tensor-core form: [cout_pad][kh*kw*cin] fp16 hi/lo planes of w * 2^e[c]; scale_tc = scale * 2^-e[c]
   __half* w_hi = nullptr;
   __half* w_lo = nullptr;
   float* scale_tc = nullptr;
@@ -46,16 +46,14 @@ struct ConvIO {
   int pad_t = 0, pad_l = 0;
   int ho = 0, wo = 0;
   int* overflow_flag = nullptr;
-  ConvWorkspace* sk = nullptr;  // enables stream-K scheduling on the tcgen05 path (nullptr: whole tiles only)
+  ConvWorkspace* sk = nullptr;  // enables stream-K scheduling on the tensor-core path (nullptr: whole tiles only)
   int streamk = 1;              // stream-K policy of THIS launch: 0 off, 1 auto (wave-quantisation heuristic), 2 whenever possible
-  int chunk_tail = 2;           // stages per D1 chunk after the first eight stages of a tile (1, 2 or 4; see tc_chunk_end)
-  int cta2 = 0;                 // CTA-pair (cta_group::2) kernel on residual-free layers with at least this many K stages per tile (0 = never)
-  int halo = 0;                 // halo-patch kernels on 3x3 stride-1 layers: 0 never, 1 single CTA, 2 CTA pairs where C_out % 128 == 0
+  int cta2 = 0;                 // 2-CTA cluster kernel (weight tile multicast) on layers with at least this many K slices per tile (0 = never)
+  int halo = 0;                 // halo-patch kernels on 3x3 stride-1 SAME layers without residual or fp32 output (0 never; on CTA pairs with cta2)
   int halo_tiles_pct = 150;     // ... while their M-tile count stays within this percentage of the generic kernel's
-  int halo_baseoff = 0;         // (bring-up switch) write the patch views' swizzle phase into the matrix descriptors
-  int epi16 = 0;                // 16-epilogue-warp kernels on layers with at most this many K stages per tile (0 = never)
+  int epi16 = 0;                // four-consumer-warpgroup (16 epilogue warps) kernel on layers with at most this many K slices per tile (0 = never)
   int sm_reserve = 0;           // SMs a persistent launch leaves free (the engine's two-stream pipeline sets 8)
-  // Optional strided ("Toeplitz") view of the input for the tcgen05 path: element pitches between
+  // Optional strided ("Toeplitz") view of the input for the tensor-core path: element pitches between
   // consecutive pixels / rows / images (0 = dense NHWC).  Used by the space-to-depth stem, where each
   // A row is the 64 contiguous fp16 of four horizontally adjacent 16-channel pixels.
   long in_pix_pitch = 0, in_row_pitch = 0, in_img_pitch = 0;

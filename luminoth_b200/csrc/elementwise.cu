@@ -70,7 +70,7 @@ void launch_resize_bilinear(const void* src, bool src_f32, int h0, int w0, float
 
 // Space-to-depth staging of the 7x7/2 stem (slim conv2d_same: zero pad 3/3 AFTER mean subtraction):
 // X2[n][Y][X][dy*6 + dx*3 + c] = xp[2Y+dy][2X+dx][c], xp = padded (image - mean); channels 12..15 = 0.
-// The stem then is a 4x4/1 VALID conv over X2 that the tcgen05 kernel runs as 4 taps of K = 64.
+// The stem then is a 4x4/1 VALID conv over X2 that the tensor-core kernel runs as 4 taps of K = 64.
 template <typename PIX>
 __global__ void stem_s2d_kernel(const PIX* __restrict__ img, __half* __restrict__ hi, __half* __restrict__ lo, int n,
                                 int h, int w, int h2, int w2, float m0, float m1, float m2) {

@@ -116,14 +116,11 @@ struct lumi_engine {
   int* d_overflow = nullptr;
   ConvWorkspace sk_ws[2];       // stream-K scratch, one per stream
   int conv_streamk = 1;         // 0 off, 1 auto, 2 whenever possible
-  int conv_chunk_tail = 2;      // env LUMI_CONV_CHUNK_TAIL: D1 chunk length (stages) past the first eight stages of a tile
-  int conv_cta2 = 9;            // env LUMI_CONV_2CTA: minimum K stages per tile for the CTA-pair kernel (0 = off).  Measured per
-                                // layer (profiles/r2_conv_variants.txt): with the elect.sync issue path pairs win from 9 stages
-                                // (3x3x128: 66 -> 60 us, 3x3x256: 64 -> 57, RPN 3x3x1024: 461 -> 377); one leader issues for two SMs
-  int conv_halo = 0;            // env LUMI_CONV_HALO: halo-patch kernels on the 3x3 stride-1 layers (0 off, 1 single CTA, 2 CTA pairs)
+  // conv kernel variants, all off by default (not timed on H100 yet; see DESIGN 7.2):
+  int conv_cta2 = 0;            // env LUMI_CONV_2CTA: 2-CTA cluster kernel on layers with at least this many K slices per tile
+  int conv_halo = 0;            // env LUMI_CONV_HALO: 1 = halo-patch kernels on the 3x3 stride-1 layers
   int conv_halo_pct = 150;      // env LUMI_CONV_HALO_PCT: ... while the M-tile count stays within this percentage of the generic kernel's
-  int conv_halo_baseoff = 0;    // env LUMI_HALO_BASEOFF (bring-up)
-  int conv_epi16 = 1;           // env LUMI_CONV_EPI16: 16-epilogue-warp kernels for tiles of at most this many K stages
+  int conv_epi16 = 0;           // env LUMI_CONV_EPI16: four-warpgroup kernel on layers with at most this many K slices per tile
   uint8_t* d_images = nullptr; size_t images_cap = 0;
   float* d_boxes = nullptr; float* d_scores = nullptr; int* d_labels = nullptr; int* d_counts = nullptr;
   int* d_prop_counts = nullptr;
@@ -435,7 +432,7 @@ void build_layers(lumi_engine* e) {
     const std::string root = "truncated_base_network/" + e->arch;
     const int* units = e->arch == "resnet_v1_50" ? RESNET_UNITS_50 : RESNET_UNITS_101;
     make_conv_bn(e, root + "/conv1", 2, 1, ACT_RELU);
-    {   // tcgen05 form of the stem: 7x7/2 over 3 channels == 4x4/1 over the 12(+4 pad)-channel
+    {   // tensor-core form of the stem: 7x7/2 over 3 channels == 4x4/1 over the 12(+4 pad)-channel
         // space-to-depth input; one filter row r' = 4 taps x 16 ch = one K=64 slice  (kh=4, kw=1, cin=64)
       const HostTensor& w = W(e, root + "/conv1/weights");
       const ConvLayer& base = e->layers.at(root + "/conv1");
@@ -498,7 +495,7 @@ void build_layers(lumi_engine* e) {
         const std::string p = s + "/vgg_16/" + VGG_NAMES[b] + "/" + VGG_NAMES[b] + "_" + std::to_string(r + 1);
         make_conv_bias(e, p, {p + "/weights"}, {p + "/biases"}, 1, 1, ACT_RELU);
       }
-    {   // tcgen05 form of conv1_1 (3x3 over 3 channels): one filter row = 4 pixels x 16 ch = one K=64 slice
+    {   // tensor-core form of conv1_1 (3x3 over 3 channels): one filter row = 4 pixels x 16 ch = one K=64 slice
         // (kh=3, kw=1, cin=64) over the padded 16-channel staging written by launch_pack_c3
       const std::string p = s + "/vgg_16/conv1/conv1_1";
       const HostTensor& w = W(e, p + "/weights");
@@ -656,17 +653,15 @@ Act run_conv(Ctx& cx, const std::string& key, Act in, int padding, const Act* re
   io.sk = cx.sk;
   io.streamk = cx.e->conv_streamk;
   io.sm_reserve = cx.sm_reserve;
-  io.epi16 = cx.e->conv_epi16;
   io.cta2 = cx.e->conv_cta2;
   io.halo = cx.e->conv_halo;
   io.halo_tiles_pct = cx.e->conv_halo_pct;
-  io.halo_baseoff = cx.e->conv_halo_baseoff;
-  io.chunk_tail = cx.e->conv_chunk_tail;
+  io.epi16 = cx.e->conv_epi16;
   if (!cx.dry) {
     const bool tc = cx.e->conv_impl == 1 && conv_tc_supported(L, io);
     const double flops = algorithmic_flops >= 0 ? algorithmic_flops
                                                 : 2.0 * (double)in.n * ho * wo * (double)L.kh * L.kw * L.cin * L.cout;
-    LUMI_REQUIRE(tc || !view_pitch, "strided input views exist only on the tcgen05 path (internal)");
+    LUMI_REQUIRE(tc || !view_pitch, "strided input views exist only on the tensor-core path (internal)");
     ProfScope ps(cx.e, cx.dry, tc ? PC_CONV_TC : PC_CONV_SIMT, flops, key);
     if (tc) launch_conv_tc(L, io, cx.st);
     else launch_conv_simt(L, io, cx.st);
@@ -816,9 +811,6 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
     const double bytes = 4.0 * fmap.numel() + 16.0 * n * post + 4.0 * (double)(need_pooled ? pooled.numel() : 0) +
                          4.0 * (double)(fuse_mean ? feat.numel() : 0);
     ProfScope ps(cx.e, cx.dry, PC_ROI, bytes);
-    // (writing this fp32 copy from the last block3 conv's epilogue was tried in round 2: direct global stores from the
-    //  epilogue warps of the residual-slab kernel made that kernel's results flaky at production size -- plain delays in
-    //  the same place did not -- profiles/r2_conv_variants.txt; the separate 60 us pass stays)
     launch_act_to_f32(fmap, fmap_f32, cx.st);
     launch_roi_pool(fmap_f32, fmap.n, fmap.h, fmap.w, fmap.c, proposals, prop_counts, post, (float)h, (float)w,
                     e->pooled_h, e->pooled_w, pooled, fuse_mean ? feat : Act(), cx.st);
@@ -1066,7 +1058,7 @@ int fail(lumi_engine* e, int code, const std::string& msg) {
 // ======================================================================================
 extern "C" {
 
-const char* lumi_version(void) { return "luminoth_b200 0.1 (sm_100a)"; }
+const char* lumi_version(void) { return "luminoth_b200 0.1 (sm_90a)"; }
 
 int lumi_device_count(void) {
   int n = 0;
@@ -1170,13 +1162,11 @@ int lumi_finalize(lumi_engine* e) {
   }
   conv_workspace_create(e->sk_ws[0]);
   if (const char* v = std::getenv("LUMI_CONV_STREAMK")) e->conv_streamk = std::max(0, std::min(2, std::atoi(v)));
-  if (const char* v = std::getenv("LUMI_GRAPHS")) e->use_graphs = std::atoi(v) != 0;
-  if (const char* v = std::getenv("LUMI_CONV_EPI16")) e->conv_epi16 = std::max(0, std::min(8, std::atoi(v)));
   if (const char* v = std::getenv("LUMI_CONV_2CTA")) e->conv_cta2 = std::max(0, std::atoi(v));
-  if (const char* v = std::getenv("LUMI_CONV_HALO")) e->conv_halo = std::max(0, std::min(2, std::atoi(v)));
+  if (const char* v = std::getenv("LUMI_CONV_HALO")) e->conv_halo = std::max(0, std::min(1, std::atoi(v)));
   if (const char* v = std::getenv("LUMI_CONV_HALO_PCT")) e->conv_halo_pct = std::max(0, std::atoi(v));
-  if (const char* v = std::getenv("LUMI_HALO_BASEOFF")) e->conv_halo_baseoff = std::atoi(v);
-  if (const char* v = std::getenv("LUMI_CONV_CHUNK_TAIL")) e->conv_chunk_tail = std::max(1, std::min(4, std::atoi(v)));
+  if (const char* v = std::getenv("LUMI_CONV_EPI16")) e->conv_epi16 = std::max(0, std::atoi(v));
+  if (const char* v = std::getenv("LUMI_GRAPHS")) e->use_graphs = std::atoi(v) != 0;
   if (e->max_batch >= 2) {
     conv_workspace_create(e->sk_ws[1]);
     LUMI_CUDA_CHECK(cudaStreamCreateWithFlags(&e->stream2, cudaStreamNonBlocking));

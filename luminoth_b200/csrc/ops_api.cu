@@ -84,8 +84,9 @@ int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wg
   }
   if (impl >= 1 && impl <= 11) {
     // 1 whole tiles, 2 stream-K forced (fp32 outputs written by the epilogue);
-    // 3 / 4 / 5: the engine's inter-layer form -- fp16x2 split planes through the staged TMA-store epilogue (and the
-    // TMA-prefetched residual) -- with the 8-warp epilogue (3), the 16-warp short-K kernels allowed (4), and 4 + stream-K (5)
+    // 3 / 4 / 5: the engine's inter-layer form -- fp16x2 split planes -- with two consumer warpgroups (3), the
+    // four-warpgroup short-K kernel allowed (4), and 4 + stream-K (5); 6 / 7: the 2-CTA cluster kernel wherever it
+    // applies (7: + stream-K); 8-11: the halo-patch kernels (10, 11 on cluster pairs; 9, 11: + stream-K)
     std::unique_ptr<ActBuf> split_out;
     if (impl >= 3) {
       LUMI_REQUIRE(cout % 32 == 0, "conv2d: split outputs need cout % 32 == 0");
@@ -93,10 +94,9 @@ int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wg
       io.out = split_out->a;
       io.out_f32 = nullptr;
       io.epi16 = (impl == 4 || impl == 5) ? 8 : 0;
-      io.cta2 = (impl == 6 || impl == 7) ? 1 : 0;   // 6 / 7: CTA-pair kernel wherever it applies (7: + stream-K forced)
-      io.halo = (impl == 8 || impl == 9) ? 1 : ((impl == 10 || impl == 11) ? 2 : 0);   // 8-11: halo-patch kernels (9, 11: + stream-K)
+      io.cta2 = (impl == 6 || impl == 7 || impl == 10 || impl == 11) ? 1 : 0;
+      io.halo = (impl >= 8) ? 1 : 0;
       io.halo_tiles_pct = 1000000;                  // test hook: whenever the shape allows
-      if (const char* e = std::getenv("LUMI_HALO_BASEOFF")) io.halo_baseoff = std::atoi(e);
     }
     LUMI_REQUIRE(conv_tc_supported(L, io), "conv2d: this layer shape is not handled by the tensor-core kernel");
     ConvWorkspace sk;

@@ -11,6 +11,7 @@
 // round-to-nearest intrinsics (no FMA contraction): discrete decisions
 // (>=, >, iou > thr) must agree with the fp32 reference bit for bit on equal inputs.
 #include "ops.cuh"
+#include "conv.cuh"
 #include <cstdlib>
 
 namespace lumi {
@@ -636,10 +637,10 @@ static dim3 mask_grid(const NmsWorkspace& ws, int problems, int n_max) {
   // blocks walk their problem's (row block, column block) pairs with a grid stride; the x extent is sized so that
   // the whole launch is ~64 resident blocks per SM -- with hundreds of (image, class) problems whose candidate
   // lists are short (SSD: 640 problems, most rows filtered by min_prob) a fixed 2048-wide grid was 1.3 M blocks
-  // that exit at once: 0.68 ms of block-launch overhead per step (ncu, profiles/r2_ncu_step_summary.json)
+  // that exit at once, and their block-launch overhead dominated the step
   const long nw = (n_max + 63) / 64;
   long maxpairs = nw * (nw + 1) / 2;
-  long gx = (148L * 64 + problems - 1) / problems;
+  long gx = ((long)device_sm_count() * 64 + problems - 1) / problems;
   if (gx > 2048) gx = 2048;
   if (gx > maxpairs) gx = maxpairs;
   if (gx < 1) gx = 1;
@@ -651,9 +652,8 @@ static void run_nms(NmsWorkspace& ws, int problems, float thr, int max_out, cuda
   if (!problems) return;
   const size_t staged_smem = ((size_t)ws.words + 2 * 64 * (size_t)ws.words) * sizeof(unsigned long long);
   const bool staged = staged_smem <= 200 * 1024;
-  // two-phase when the mask kernel is a full-GPU kernel (several long lists at once): measured (call C,
-  // profiles/r2_nms_variants.txt) 0.93 -> 0.75 ms per step at batch 8, but its longer kernel chain costs +0.1 ms of
-  // latency when one or two images are in flight.  LUMI_NMS_LAZY=0 / 1 forces it off / on.
+  // two-phase when the mask kernel is a full-GPU kernel (several long lists at once): it shortens the step at
+  // batch 8, but its longer kernel chain adds latency when one or two images are in flight.  LUMI_NMS_LAZY=0 / 1 forces it off / on.
   static const int lazy_env = [] { const char* e = getenv("LUMI_NMS_LAZY"); return e ? (atoi(e) != 0 ? 1 : 0) : -1; }();
   const bool lazy_ok = staged && ws.sboxes2 && ws.ncap >= NMS_LAZY_MIN && thr > 0.f && thr < INFINITY;
   const bool lazy = lazy_ok && (lazy_env == 1 || (lazy_env < 0 && problems >= 3));

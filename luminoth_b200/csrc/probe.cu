@@ -1,10 +1,5 @@
-// Measurement hook (not on the product path): issue-rate probe of tcgen05.mma kind::f16 in the shapes conv_tc_kernel
-// uses.  One CTA per SM; operands sit still in shared memory (zeros), one thread issues `iters` stages of twelve
-// 128 x N x 16 MMAs in a chosen accumulator pattern and the elapsed SM clocks are reported per CTA.  Answers, without
-// the rest of the conv pipeline around it: what does an MMA of this shape cost when (a) every MMA accumulates into the
-// same TMEM tile, (b) in the D1 / D2 / D2 pattern of the split-operand conv, (c) round-robin over 3 or 4 tiles, (d) with
-// N = 256, (e) with a shifted (not 1024 B aligned) A view as in the halo kernels, and (f) while bulk copies stream into
-// the same shared memory at the rate the TMA producer does.
+// Measurement hook (not on the product path): whether the lanes of one warp see different answers from a single
+// mbarrier.try_wait instruction.
 #include "../../include/luminoth_b200.h"
 #include "common.cuh"
 
@@ -14,172 +9,9 @@
 
 namespace lumi {
 
-struct ProbeArgs {
-  int mode;          // accumulator pattern, see lumi_op_mma_probe
-  int n;             // MMA N (128 or 256)
-  int iters;         // stages of 12 MMAs
-  int shifted_a;     // 1: A descriptors start 128 B past the 1024 B boundary with a 1280 B group stride
-  int fill_bytes;    // > 0: a second thread keeps bulk-copying this many bytes per stage-equivalent into shared memory
-  int ldtm_warps;    // > 0: this many further warps keep reading a TMEM tile with tcgen05.ld (32x32b.x32) meanwhile
-  int ldtm_gap;      // ... with this many clocks of pause between two reads of a warp
-  int sync;          // per-stage synchronisation around the MMAs: 1 tcgen05.commit to a barrier nobody waits on; 2 the conv
-                     // kernel's ring: commit -> empty[s], a helper warp answers full[s], the issuer waits full[s] (depth `ring`)
-  int ring;          // ring depth for sync = 2 (2..8)
-  int mmas;          // MMAs per stage: 12 (all), 4 (hi*hi only)
-  int flags;         // 1: no tcgen05.fence after the ring wait; 2: spin on mbarrier.test_wait instead of try_wait;
-                     // 4: TWO issuing warps -- warp 1 the four hi*hi MMAs of a stage, warp 2 the eight cross-term MMAs
-  const uint8_t* fill_src;
-  long long* clocks; // [gridDim.x]
-};
-
-constexpr int PROBE_STAGE_BYTES = 2 * 16384 + 2 * 32768;   // A hi, A lo (128 rows) + B hi, B lo (up to 256 rows)
-constexpr int PROBE_STAGES = 2;
-constexpr int PROBE_FILL_BYTES = 32768;
-constexpr int PROBE_SMEM = PROBE_STAGES * PROBE_STAGE_BYTES + PROBE_FILL_BYTES + 1024 + 64 + 128;
-
-__global__ void __launch_bounds__(96 + 8 * 32, 1) mma_probe_kernel(const ProbeArgs a) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* fill = smem + PROBE_STAGES * PROBE_STAGE_BYTES;
-  uint64_t* done_bar = reinterpret_cast<uint64_t*>(fill + PROBE_FILL_BYTES);
-  uint64_t* fill_bar = done_bar + 1;                 // [4]
-  volatile uint32_t* stop_flag = reinterpret_cast<volatile uint32_t*>(fill_bar + 4);
-  uint32_t* tmem_slot = const_cast<uint32_t*>(stop_flag) + 1;
-  uint64_t* ring_full = reinterpret_cast<uint64_t*>(smem + PROBE_STAGES * PROBE_STAGE_BYTES + PROBE_FILL_BYTES + 64);   // [8]
-  uint64_t* ring_empty = ring_full + 8;                                                                              // [8]
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
-  for (int i = threadIdx.x; i < (PROBE_STAGES * PROBE_STAGE_BYTES + PROBE_FILL_BYTES) / 16; i += blockDim.x)
-    reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 4; ++i) mbar_init(&fill_bar[i], 1);
-    for (int i = 0; i < 8; ++i) { mbar_init(&ring_full[i], 1); mbar_init(&ring_empty[i], (a.flags & 4) ? 2 : 1); }
-    mbar_init(done_bar, (a.flags & 4) ? 2 : 1);
-    *stop_flag = 0;
-    fence_mbar_init();
-  }
-  fence_proxy_async();
-  __syncthreads();
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
-
-  if (warp == 1 || (warp == 2 && (a.flags & 4))) {
-    const int part = (a.flags & 4) ? warp : 0;        // 0 everything, 1 the hi*hi MMAs, 2 the cross terms
-    const uint32_t idesc = make_idesc_f16(128, a.n);
-    const uint32_t acc_cols = (uint32_t)a.n;
-    long long t0 = 0;
-    if (lane == 0) t0 = clock64();
-    for (int it = 0; it < a.iters; ++it) {
-      const uint32_t sa = smem_u32(smem + (it % PROBE_STAGES) * PROBE_STAGE_BYTES);
-      uint64_t d_ahi, d_alo;
-      if (a.shifted_a) {
-        d_ahi = make_sw128_kmajor_desc_sbo(sa + 128, 1280, 0);
-        d_alo = make_sw128_kmajor_desc_sbo(sa + 128 + 2048, 1280, 0);   // (overlaps the hi plane: contents are irrelevant)
-      } else {
-        d_ahi = make_sw128_kmajor_desc(sa);
-        d_alo = make_sw128_kmajor_desc(sa + 16384);
-      }
-      const uint64_t d_bhi = make_sw128_kmajor_desc(sa + 32768);
-      const uint64_t d_blo = make_sw128_kmajor_desc(sa + 32768 + 32768);
-      const uint32_t rs = (uint32_t)it % (uint32_t)a.ring, rph = ((uint32_t)it / (uint32_t)a.ring) & 1u;
-      if (a.sync == 2) {
-        if (a.flags & 2) {
-          uint32_t ok = 0;
-          do {
-            asm volatile("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                         : "=r"(ok) : "r"(smem_u32(&ring_full[rs])), "r"(rph) : "memory");
-          } while (!ok);
-        } else {
-          mbar_wait(&ring_full[rs], rph);
-        }
-        if (!(a.flags & 1)) tc_fence_after();
-      }
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t ko = (uint64_t)(k * 2);
-          const int m = k * 3;          // running MMA index inside the stage
-          uint32_t t[3];
-          if (a.mode == 0) { t[0] = t[1] = t[2] = 0; }
-          else if (a.mode == 1) { t[0] = 0; t[1] = t[2] = 1; }
-          else if (a.mode == 2) { t[0] = 0; t[1] = 1; t[2] = 2; }
-          else { t[0] = (uint32_t)(m & 3); t[1] = (uint32_t)((m + 1) & 3); t[2] = (uint32_t)((m + 2) & 3); }
-          // (always accumulating: the accumulators start with whatever TMEM held, which is irrelevant for the timing)
-          if (part != 2) umma_f16(tmem_base + (t[0] * acc_cols) % 512u, d_ahi + ko, d_bhi + ko, idesc, 1u);
-          if (a.mmas == 4 || part == 1) continue;
-          umma_f16(tmem_base + (t[1] * acc_cols) % 512u, d_ahi + ko, d_blo + ko, idesc, 1u);
-          umma_f16(tmem_base + (t[2] * acc_cols) % 512u, d_alo + ko, d_bhi + ko, idesc, 1u);
-        }
-        if (a.sync == 1) umma_commit(&ring_empty[0]);
-        if (a.sync == 2) umma_commit(&ring_empty[rs]);
-      }
-      __syncwarp();
-    }
-    if (lane == 0) {
-      umma_commit(done_bar);
-      mbar_wait(done_bar, 0);
-      const long long t1 = clock64();
-      if (warp == 1) { a.clocks[blockIdx.x] = t1 - t0; *stop_flag = 1; }
-    }
-    __syncwarp();
-  } else if (warp == 0 && a.sync == 2) {
-    // the conv kernel's producer without the copies: stage s is handed back as soon as its MMAs have retired
-    for (int it = 0; it < a.iters; ++it) {
-      const uint32_t rs = (uint32_t)it % (uint32_t)a.ring, rph = ((uint32_t)it / (uint32_t)a.ring) & 1u;
-      mbar_wait(&ring_empty[rs], rph ^ 1u);
-      if (lane == 0) mbar_arrive(&ring_full[rs]);
-      __syncwarp();
-    }
-  } else if (warp == 0 && a.fill_bytes > 0) {
-    // bulk copies global -> shared at full tilt until the MMA thread is done (the rate is reported by the host from the
-    // copy count); they land in their own 32 KB window, i.e. they compete for the shared-memory port only
-    if (lane == 0) {
-      // four 8 KB copies in flight (ring of four windows, one barrier each)
-      uint32_t n = 0;
-      while (!*stop_flag) {
-        const uint32_t slot = n & 3u;
-        if (n >= 4) mbar_wait(&fill_bar[slot], ((n >> 2) - 1u) & 1u);
-        mbar_arrive_expect_tx(&fill_bar[slot], (uint32_t)(PROBE_FILL_BYTES / 4));
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     ::"r"(smem_u32(fill + slot * (PROBE_FILL_BYTES / 4))),
-                       "l"(a.fill_src + (size_t)((blockIdx.x * 7 + n) % 256) * (PROBE_FILL_BYTES / 4)),
-                       "r"((uint32_t)(PROBE_FILL_BYTES / 4)), "r"(smem_u32(&fill_bar[slot]))
-                     : "memory");
-        ++n;
-      }
-      for (uint32_t m = (n >= 4 ? n - 4 : 0); m < n; ++m) mbar_wait(&fill_bar[m & 3u], (m >> 2) & 1u);   // drain
-      a.clocks[gridDim.x + blockIdx.x] = (long long)n;
-    }
-  }
-  else if (warp >= 3 && warp - 3 < a.ldtm_warps) {
-    // epilogue-style readers: warp w reads lanes 32 (w % 4) .. +31, 32 columns of the LAST accumulator tile (columns
-    // 384..511: never written in modes 0-2 with N = 128), as conv_tc_kernel's D1 drain does
-    const uint32_t taddr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + 384u + (uint32_t)(((warp - 3) >> 2) * 32);
-    uint32_t n = 0;
-    float sink = 0.f;
-    while (!*stop_flag) {
-      uint32_t r[32];
-      tmem_ld_32x32b_x32(taddr, r);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 32; ++j) sink += __uint_as_float(r[j]);
-      ++n;
-      if (a.ldtm_gap > 0) { const long long t = clock64(); while (clock64() - t < a.ldtm_gap) {} }
-    }
-    if (lane == 0) a.clocks[2 * gridDim.x + blockIdx.x * 8 + (warp - 3)] = (long long)n;
-    if (sink == 123.456f) a.clocks[0] = 0;      // keep the loads alive
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { __syncwarp(); tmem_dealloc(tmem_base, 512); }
-}
-
-
 // ---------------------------------------------------------------------------------------------------------------
-// Second probe: can the 32 lanes of ONE warp instruction `mbarrier.try_wait` see different answers?  Warp 0 spins on a
-// barrier with all lanes (the whole-warp role pattern of conv_tc_kernel), counting its attempts per lane; warp 1 arrives
+// Probe: can the 32 lanes of ONE warp instruction `mbarrier.try_wait` see different answers?  Warp 0 spins on a
+// barrier with all lanes (a whole-warp barrier-polling role), counting its attempts per lane; warp 1 arrives
 // after a pseudo-random pause.  Lanes that run in lockstep make the same number of attempts unless the instruction
 // answered them differently.  Reports the number of rounds in which the per-lane attempt counts differed.
 __global__ void __launch_bounds__(64, 1) trywait_probe_kernel(int rounds, unsigned* out) {
@@ -224,47 +56,6 @@ __global__ void __launch_bounds__(64, 1) trywait_probe_kernel(int rounds, unsign
 }
 
 }  // namespace lumi
-
-extern "C" int lumi_op_mma_probe(int mode, int n, int iters, int shifted_a, int fill, int ldtm_warps, int ldtm_gap,
-                                 int sync, int ring, int mmas_per_stage, int flags, double* clk_per_mma,
-                                 double* fill_bytes_per_clk, double* ldtm_bytes_per_clk) {
-  using namespace lumi;
-  try {
-    LUMI_REQUIRE((n == 128 || n == 256) && iters > 0 && mode >= 0 && mode <= 3, "mma_probe: bad arguments");
-    LUMI_REQUIRE(n == 128 || mode <= 1, "mma_probe: N = 256 has two accumulator tiles");
-    LUMI_REQUIRE(ldtm_warps >= 0 && ldtm_warps <= 8 && ldtm_gap >= 0, "mma_probe: at most 8 reader warps");
-    LUMI_REQUIRE(sync >= 0 && sync <= 2 && ring >= 2 && ring <= 8 && (mmas_per_stage == 12 || mmas_per_stage == 4) &&
-                 !(sync == 2 && fill) && !((flags & 4) && (mmas_per_stage != 12 || mode != 1)),
-                 "mma_probe: bad synchronisation arguments");
-    int dev = 0, sms = 0;
-    LUMI_CUDA_CHECK(cudaGetDevice(&dev));
-    LUMI_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    LUMI_CUDA_CHECK(cudaFuncSetAttribute(mma_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PROBE_SMEM));
-    long long* d_clk = nullptr;
-    uint8_t* d_src = nullptr;
-    LUMI_CUDA_CHECK(cudaMalloc(&d_clk, 10 * sms * sizeof(long long)));
-    LUMI_CUDA_CHECK(cudaMemset(d_clk, 0, 10 * sms * sizeof(long long)));
-    LUMI_CUDA_CHECK(cudaMalloc(&d_src, (size_t)64 * PROBE_FILL_BYTES));
-    LUMI_CUDA_CHECK(cudaMemset(d_src, 0, (size_t)64 * PROBE_FILL_BYTES));
-    ProbeArgs a{mode, n, iters, shifted_a, fill ? PROBE_FILL_BYTES : 0, ldtm_warps, ldtm_gap, sync, ring, mmas_per_stage, flags, d_src, d_clk};
-    mma_probe_kernel<<<sms, 96 + 8 * 32, PROBE_SMEM>>>(a);
-    cudaError_t e = cudaDeviceSynchronize();
-    std::vector<long long> h(10 * sms);
-    if (e == cudaSuccess) e = cudaMemcpy(h.data(), d_clk, h.size() * sizeof(long long), cudaMemcpyDeviceToHost);
-    cudaFree(d_clk); cudaFree(d_src);
-    LUMI_CUDA_CHECK(e);
-    double clk = 0, copies = 0;
-    for (int i = 0; i < sms; ++i) { clk += (double)h[i]; copies += (double)h[sms + i]; }
-    if (clk_per_mma) *clk_per_mma = clk / sms / ((double)iters * mmas_per_stage);
-    double reads = 0;
-    for (int i = 2 * sms; i < 10 * sms; ++i) reads += (double)h[i];
-    if (ldtm_bytes_per_clk) *ldtm_bytes_per_clk = clk > 0 ? reads * 4096.0 / clk : 0.0;     // per SM
-    if (fill_bytes_per_clk) *fill_bytes_per_clk = clk > 0 ? copies * (PROBE_FILL_BYTES / 4) / clk : 0.0;
-    return LUMI_OK;
-  } catch (const std::exception& ex) {
-    return LUMI_EINVAL;
-  }
-}
 
 extern "C" int lumi_op_trywait_probe(int rounds, unsigned* diverged_rounds, unsigned* max_spread, unsigned* mean_attempts) {
   using namespace lumi;

@@ -229,9 +229,7 @@ __global__ void __launch_bounds__(32 * NW, (CPL == 8 ? 2 : 3) * (8 / NW)) roi_po
 // the horizontally interpolated values of the last two feature rows it touched in registers (H0 / H1, tagged with
 // their row index): vertically adjacent samples -- inside a cell AND across cells -- reuse them, so each feature row
 // is fetched once per pooled column instead of once per sample row (round-1 kernel: sharing inside one 2x2 cell only).
-// The sample tables live in the lanes of the warp (lane t = sample t) and are broadcast with shuffles; the lerps run
-// on the packed fp32 pipe (FADD2 / FFMA2: two IEEE fp32 results per instruction, each rounded exactly like the scalar
-// op, so parity is unaffected).  Instruction count per ROI and channel: ~3.0 k (round 1) -> ~0.9 k.
+// The sample tables live in the lanes of the warp (lane t = sample t) and are broadcast with shuffles.
 // =====================================================================================================================
 template <int CPL> struct RoiVec { float2 p[CPL / 2]; };
 
@@ -251,10 +249,10 @@ __device__ __forceinline__ RoiVec<CPL> roi_load(const float* f, int off) {
 template <int CPL>
 __device__ __forceinline__ RoiVec<CPL> roi_lerp(const RoiVec<CPL>& l, const RoiVec<CPL>& r, float t) {
   RoiVec<CPL> h;
-  const float2 tt = make_float2(t, t);
 #pragma unroll
   for (int j = 0; j < CPL / 2; ++j)
-    h.p[j] = __ffma2_rn(__fadd2_rn(r.p[j], make_float2(-l.p[j].x, -l.p[j].y)), tt, l.p[j]);
+    h.p[j] = make_float2(__fmaf_rn(__fsub_rn(r.p[j].x, l.p[j].x), t, l.p[j].x),
+                         __fmaf_rn(__fsub_rn(r.p[j].y, l.p[j].y), t, l.p[j].y));
   return h;
 }
 struct RoiX { int lo, hi; float t; int ok; };   // lo / hi: ELEMENT offsets of the two feature columns (x * C)
@@ -441,7 +439,7 @@ __global__ void __launch_bounds__(32 * WARPS) roi_pool_cols_kernel(const RoiArgs
 
 
 // =====================================================================================================================
-// Row-walk kernel (round 2, second pass over the design).  ncu on the column-walk kernel above (profiles/r2_*): only
+// Row-walk kernel (round 2, second pass over the design).  A profile of the column-walk kernel above: only
 // 28 % of its 1.12 G warp instructions were lerps / maxima / loads -- the rest was the warp-uniform bookkeeping of tap
 // sharing (compares, branches, register moves) -- and its L1 hit rate was 6 %: every tap is an L2 hit, so sharing
 // taps across samples does not save memory traffic that L1 would not merge anyway.  This kernel drops all

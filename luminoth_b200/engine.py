@@ -62,7 +62,6 @@ SIGNATURES = {
                                         ctypes.c_int, _c_int_p, _c_int_p]),
     'lumi_jpeg_last_error': (ctypes.c_char_p, []),
     'lumi_op_last_error': (ctypes.c_char_p, []),
-    'lumi_op_mma_probe': (ctypes.c_int, [ctypes.c_int] * 11 + [ctypes.POINTER(ctypes.c_double)] * 3),
     'lumi_op_trywait_probe': (ctypes.c_int, [ctypes.c_int] + [ctypes.POINTER(ctypes.c_uint)] * 3),
     'lumi_op_conv2d': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] + [ctypes.c_int] * 6 +
                        [ctypes.c_void_p] * 3 + [ctypes.c_int] * 2 + [ctypes.c_void_p, _c_int_p, _c_int_p,
@@ -205,7 +204,7 @@ class Engine(object):
             raise ValueError('conv impl must be "simt" or "tc"')
 
     def set_conv_streamk(self, mode):
-        """tcgen05 conv scheduling: 'off' (whole tiles), 'auto' (default), 'always' (stream-K wherever applicable)."""
+        """Tensor-core conv scheduling: 'off' (whole tiles), 'auto' (default), 'always' (stream-K wherever applicable)."""
         rc = self._lib.lumi_set_conv_streamk(self._h, {'off': 0, 'auto': 1, 'always': 2}.get(mode, mode))
         if rc != LUMI_OK:
             raise ValueError('stream-K mode must be "off", "auto" or "always"')

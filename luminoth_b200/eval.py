@@ -1,4 +1,4 @@
-"""``lumi eval`` on the B200 engine (SURVEY.md section 8f-3).
+"""``lumi eval`` on the H100 engine (SURVEY.md section 8f-3).
 
 Mirrors ``luminoth/eval.py``: the caller-side config mutations (:61-76), the walk over the checkpoints of
 ``<job_dir>/<run_name>`` (:222-275 ``get_checkpoints``), one pass over ``<dataset.dir>/<split>.tfrecords`` with the

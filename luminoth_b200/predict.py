@@ -1,4 +1,4 @@
-"""``lumi predict`` on the B200 engine -- mirrors ``luminoth/predict.py`` (SURVEY.md section 8f-2 / 8f-4).
+"""``lumi predict`` on the H100 engine -- mirrors ``luminoth/predict.py`` (SURVEY.md section 8f-2 / 8f-4).
 
 Same command line, same JSON lines (``{"file": ..., "objects": [{"bbox", "label", "prob"}]}``), same caller-side
 config mutations (``--min-prob`` / ``--max-detections`` written into the config before the network is built,

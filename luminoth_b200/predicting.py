@@ -6,7 +6,7 @@ rounded to 4 decimals).  ``predict_batch(images)`` is the batched extension
 (the reference is hard-wired to batch 1, ``fasterrcnn.py:101-103``).
 
 What changed underneath: graph build + ``session.run`` is one call into the
-sm_100a engine (``lumi_predict`` / ``lumi_predict_f32``).  The aspect-preserving
+sm_90a engine (``lumi_predict`` / ``lumi_predict_f32``).  The aspect-preserving
 resize of ``datasets/object_detection_dataset.py:71-83`` / ``utils/image.py:38-147``
 runs on the GPU (``lumi_op_resize_bilinear``, bit-identical to the TF1 legacy
 bilinear kernel); only its size arithmetic (float32, like the reference) stays on

@@ -1,4 +1,4 @@
-"""``lumi server web`` on the B200 engine -- mirrors ``luminoth/tools/server/web.py`` (SURVEY.md section 8f-4).
+"""``lumi server web`` on the H100 engine -- mirrors ``luminoth/tools/server/web.py`` (SURVEY.md section 8f-4).
 
 Same HTTP surface: ``POST /api/<model_name>/predict/`` with a multipart ``image`` field (optional ``?total=N``)
 answers ``{"objects": [{"bbox", "label", "prob"}, ...]}``; ``GET`` on it answers 400 ``Use POST method to send

@@ -3,7 +3,7 @@
 TEST INFRASTRUCTURE ONLY.  Nothing under ``luminoth_b200/`` imports this
 package; only ``tests/``, ``__graft_entry__.smoke()`` and the ``cpu_baseline``
 / ``--impl reference`` legs of ``bench.py`` may.  It is the checker, never the
-product: the product path is the sm_100a CUDA library and fails loudly when
+product: the product path is the sm_90a CUDA library and fails loudly when
 that library is missing.
 
 What it restates (reference = tryolabs/luminoth @ 9109d8b, paths relative to

@@ -56,7 +56,7 @@ def test_two_engines_two_threads_bit_identical():
 
 
 def test_second_device_engine_matches_first():
-    """cudaFuncSetAttribute / SM count are per device: an engine on device 1 needs its own opt-in for the 225 KB
+    """cudaFuncSetAttribute / SM count are per device: an engine on device 1 needs its own opt-in for the large
     dynamic shared memory of the conv kernel.  Skipped on a single-GPU box."""
     if load_library().lumi_device_count() < 2:
         pytest.skip('needs two visible GPUs')

@@ -1,5 +1,5 @@
 """Per-kernel parity: every CUDA stage, called through the C ABI, against the CPU
-oracle on the same seeded inputs (`-m gpu`, needs a B200).
+oracle on the same seeded inputs (`-m gpu`, needs an H100).
 
 Tolerances: integer / index outputs bit-exact; floating point within the
 north-star's 1e-3 on box coordinates (px) and fp32-class (<= 2e-5 of the output
@@ -68,7 +68,7 @@ CONV_CASES = [
     # enough tiles that a stream-K range holds whole tiles plus a head and a tail piece
     ('sk_many_tiles', 2, 64, 96, 128, 256, 3, 1, 1, 'SAME', True, 1),
     ('sk_1x1_512_128', 3, 40, 64, 512, 128, 1, 1, 1, 'SAME', False, 1),
-    # short-K 1x1 layers of the bottlenecks (the 16-epilogue-warp kernels): residual in place / no residual / subsampled
+    # short-K 1x1 layers of the bottlenecks (the 16-epilogue-warp kernels): residual / no residual / subsampled
     ('b1_conv3_64_256_res', 2, 38, 64, 64, 256, 1, 1, 1, 'SAME', True, 1),
     ('b1_shortcut_64_256', 2, 38, 64, 64, 256, 1, 1, 1, 'SAME', False, 0),
     ('b2_conv3_128_512_res', 3, 19, 32, 128, 512, 1, 1, 1, 'SAME', True, 1),

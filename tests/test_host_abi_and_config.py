@@ -30,9 +30,9 @@ def test_library_exports_every_declared_symbol():
     assert lib.lumi_version().startswith(b'luminoth_b200')
 
 
-def test_library_is_blackwell_native_sass():
-    """The built library carries the sm_100a instructions the design claims (DESIGN 4.1) and no legacy tensor path:
-    tcgen05.mma (UTCHMMA, and .2CTA for the CTA-pair kernels), TMA tensor loads / stores, tcgen05.ld / commit."""
+def test_library_is_hopper_native_sass():
+    """The built library carries the sm_90a instructions the design claims (DESIGN 4.1) and no legacy tensor path:
+    wgmma (HGMMA, both tile widths of the conv kernel), TMA tensor loads, mbarrier transaction counts."""
     import shutil
     import subprocess
     from luminoth_b200 import build as B
@@ -40,10 +40,10 @@ def test_library_is_blackwell_native_sass():
     if not os.path.exists(exe) or not os.path.exists(B.LIB):
         pytest.skip('cuobjdump or the built library is not available')
     sass = subprocess.run([exe, '-sass', B.LIB], capture_output=True, text=True).stdout
-    assert 'sm_100a' in sass
-    for mnemonic in ('UTCHMMA ', 'UTCHMMA.2CTA', 'UTMALDG.4D', 'UTMASTG.4D', 'LDTM', 'UTCBAR', 'ELECT'):
+    assert 'sm_90a' in sass and 'sm_100' not in sass
+    for mnemonic in ('HGMMA.64x128x16.F32', 'HGMMA.64x64x16.F32', 'UTMALDG.4D', 'UTMALDG.2D', 'SYNCS.ARRIVE.TRANS'):
         assert mnemonic in sass, mnemonic
-    assert not re.search(r'\bHMMA\b|\bHGMMA\b', sass), 'legacy tensor-core instructions in the library'
+    assert not re.search(r'\bHMMA\b', sass), 'legacy (mma.sync) tensor-core instructions in the library'
 
 
 def test_engine_has_no_cpu_fallback():
