@@ -194,6 +194,13 @@ template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+// pins an accumulator tile at this point of the instruction stream: placed after a wait_group, reads of the tile
+// cannot be scheduled above the wait (the compiler does not know the wgmma writes the registers asynchronously)
+template <int N> __device__ __forceinline__ void wgmma_fence_operand(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 // D(64 x N, fp32 registers of the warpgroup) (+)= A(64 x 16, smem desc) * B(16 x N, smem desc), both K-major fp16;
 // scale_d = 0 overwrites D.  Fragment: thread t holds rows 16 (t / 32) + (t % 32) / 4 (+ 8), columns 8 j + 2 (t % 4) (+ 1).
 __device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {

@@ -291,15 +291,48 @@ struct TcCfg {
   static_assert(128 * (PRODUCER_REGS + NCWG * CONSUMER_REGS) <= THREADS * LAUNCH_REGS, "register budget of the CTA");
 };
 
+// Operand descriptors of one K slice, with the ring stage and (HALO) patch buffer it occupies.
+struct TcSlice { uint64_t ahi, alo, bhi, blo; uint32_t st, pb; };
+
+// The 12 wgmma of one 64-deep K slice into a fresh accumulator tile d, committed as one group.  The 2^-11-times-smaller
+// cross terms come first, the hi*hi products last: each MMA's addition into the chain can cost up to one ulp of the
+// value held, so only the last four additions act on the full-size partial sum.
+template <int WN>
+__device__ __forceinline__ void tc_slice_mma(float (&d)[WN / 2], const TcSlice& s) {
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    const uint64_t ko = (uint64_t)(kk * 2);           // 16 fp16 = 32 B = 2 x 16 B descriptor units
+    if constexpr (WN == 128) {
+      wgmma_m64n128k16_f16(d, s.ahi + ko, s.blo + ko, kk > 0 ? 1u : 0u);
+      wgmma_m64n128k16_f16(d, s.alo + ko, s.bhi + ko, 1u);
+    } else {
+      wgmma_m64n64k16_f16(d, s.ahi + ko, s.blo + ko, kk > 0 ? 1u : 0u);
+      wgmma_m64n64k16_f16(d, s.alo + ko, s.bhi + ko, 1u);
+    }
+  }
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    const uint64_t ko = (uint64_t)(kk * 2);
+    if constexpr (WN == 128) wgmma_m64n128k16_f16(d, s.ahi + ko, s.bhi + ko, 1u);
+    else wgmma_m64n64k16_f16(d, s.ahi + ko, s.bhi + ko, 1u);
+  }
+  wgmma_commit();
+}
+
 // Persistent: grid = min(#tiles, #SMs) (or #SMs for stream-K); every CTA (or CTA pair) walks its schedule.  One
 // producer thread keeps a ring of STAGES (tap, 64-channel) K slices in flight with TMA: im2col is fused -- one 4-D box
 // {64 ch, tw, th, nb} per filter tap at shifted (possibly negative) coordinates, zero-filled outside the map, which IS
 // the TF SAME zero padding.  Per K slice each consumer warpgroup issues, for each K = 16 step, the three products
-// Ahi*Blo + Alo*Bhi + Ahi*Bhi  into a fresh fp32 register tile (the lo*lo term is below fp32 resolution), waits for
-// them and adds the tile into the running fp32 sum with round-to-nearest adds: the tensor core's own accumulation
-// chain never spans more than one 64-deep slice, which keeps fp32-class accuracy at K = 9216 (DESIGN section 3).
+// Ahi*Blo + Alo*Bhi + Ahi*Bhi  into a fresh fp32 register tile (the lo*lo term is below fp32 resolution) and adds the
+// tile into the running fp32 sum with round-to-nearest adds once the tensor core is done with it: the tensor core's
+// own accumulation chain never spans more than one 64-deep slice, which keeps fp32-class accuracy at K = 9216
+// (DESIGN section 3).
+// PIPE: two slice tiles d0 / d1 alternate, so slice k + 1's wgmma run while slice k is waited for, released and
+// folded; without it every slice drains the warpgroup's wgmma queue before the fold.  Both orders fold the same tiles
+// in ascending k, so the results are bit-identical.
 // Epilogue: scale/bias (folded BN) -> +residual -> relu/relu6 -> fp32 or hi/lo split.
-template <int BN, int STAGES, int NCWG, bool PAIR, bool HALO>
+template <int BN, int STAGES, int NCWG, bool PAIR, bool HALO, bool PIPE>
 __global__ void __launch_bounds__(TcCfg<BN, STAGES, NCWG, PAIR, HALO>::THREADS, 1)
 conv_tc_kernel(const __grid_constant__ TcArgs a) {
   using Cfg = TcCfg<BN, STAGES, NCWG, PAIR, HALO>;
@@ -414,9 +447,10 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
       for (int j = 0; j < NR; ++j) racc[j] = 0.f;
       int patch_cc = -1;
       uint32_t pb = 0;
-      for (int k = item.k0; k < item.k1; ++k, ++git) {
-        const uint32_t st = git % STAGES, ph = (git / STAGES) & 1u;
-        uint64_t d_ahi, d_alo;
+      // waits until slice k (ring position g) has landed and returns its operand descriptors
+      auto acquire = [&](int k, uint32_t g) {
+        TcSlice s;
+        s.st = g % STAGES;
         if (HALO) {
           const int cc = k / 9, tap = k - cc * 9;
           if (cc != patch_cc) {
@@ -426,49 +460,81 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
             ++gpatch;
           }
           // view of the patch shifted by tap (r, s): row 8 g + j of the operand = patch pixel (g + r, j + s)
-          const int r = tap / 3, s = tap - r * 3;
-          const uint32_t pa = smem_u32(patch + pb * Cfg::PATCH_BYTES) + (uint32_t)(((wrow >> 3) + r) * TC_HALO_PITCH + s * 128);
-          d_ahi = make_sw128_kmajor_desc(pa, TC_HALO_PITCH);
-          d_alo = make_sw128_kmajor_desc(pa + TC_HALO_PLANE_BYTES, TC_HALO_PITCH);
+          const int r = tap / 3, c3 = tap - r * 3;
+          const uint32_t pa = smem_u32(patch + pb * Cfg::PATCH_BYTES) + (uint32_t)(((wrow >> 3) + r) * TC_HALO_PITCH + c3 * 128);
+          s.ahi = make_sw128_kmajor_desc(pa, TC_HALO_PITCH);
+          s.alo = make_sw128_kmajor_desc(pa + TC_HALO_PLANE_BYTES, TC_HALO_PITCH);
         }
-        mbar_wait(&full_bar[st], ph);
-        const uint32_t sa = smem_u32(stages + st * Cfg::STAGE_BYTES);
+        s.pb = pb;
+        mbar_wait(&full_bar[s.st], (g / STAGES) & 1u);
+        const uint32_t sa = smem_u32(stages + s.st * Cfg::STAGE_BYTES);
         if (!HALO) {
-          d_ahi = make_sw128_kmajor_desc(sa + wrow * 128);
-          d_alo = make_sw128_kmajor_desc(sa + TC_A_BYTES + wrow * 128);
+          s.ahi = make_sw128_kmajor_desc(sa + wrow * 128);
+          s.alo = make_sw128_kmajor_desc(sa + TC_A_BYTES + wrow * 128);
         }
-        const uint64_t d_bhi = make_sw128_kmajor_desc(sa + Cfg::A_STAGE_BYTES + wcol * 128);
-        const uint64_t d_blo = make_sw128_kmajor_desc(sa + Cfg::A_STAGE_BYTES + Cfg::B_BYTES + wcol * 128);
-        float d[NR];
-        wgmma_fence();
-        // the 2^-11-times-smaller cross terms first, the hi*hi products last: each MMA's addition into the chain can
-        // cost up to one ulp of the value held, so only the last four additions act on the full-size partial sum
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const uint64_t ko = (uint64_t)(kk * 2);       // 16 fp16 = 32 B = 2 x 16 B descriptor units
-          if constexpr (WN == 128) {
-            wgmma_m64n128k16_f16(d, d_ahi + ko, d_blo + ko, kk > 0 ? 1u : 0u);
-            wgmma_m64n128k16_f16(d, d_alo + ko, d_bhi + ko, 1u);
-          } else {
-            wgmma_m64n64k16_f16(d, d_ahi + ko, d_blo + ko, kk > 0 ? 1u : 0u);
-            wgmma_m64n64k16_f16(d, d_alo + ko, d_bhi + ko, 1u);
-          }
+        s.bhi = make_sw128_kmajor_desc(sa + Cfg::A_STAGE_BYTES + wcol * 128);
+        s.blo = make_sw128_kmajor_desc(sa + Cfg::A_STAGE_BYTES + Cfg::B_BYTES + wcol * 128);
+        return s;
+      };
+      // the wgmma of slice k have completed: free its stage (pair: in both CTAs) and, after the last tap of a channel
+      // slice, its patch buffer -- the buffer of the slice retired, not of one issued since
+      auto release = [&](int k, const TcSlice& s) {
+        if ((threadIdx.x & 127) == 0) {
+          mbar_arrive(&empty_bar[s.st]);
+          if (PAIR) mbar_arrive_cluster(&empty_bar[s.st], (uint32_t)(rank ^ 1));
+          if (HALO && (k + 1 == item.k1 || (k + 1) % 9 == 0)) mbar_arrive(&patch_empty_bar[s.pb]);
         }
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const uint64_t ko = (uint64_t)(kk * 2);
-          if constexpr (WN == 128) wgmma_m64n128k16_f16(d, d_ahi + ko, d_bhi + ko, 1u);
-          else wgmma_m64n64k16_f16(d, d_ahi + ko, d_bhi + ko, 1u);
-        }
-        wgmma_commit();
-        wgmma_wait0();
-        if ((threadIdx.x & 127) == 0) {               // this warpgroup is done with the slot (pair: in both CTAs)
-          mbar_arrive(&empty_bar[st]);
-          if (PAIR) mbar_arrive_cluster(&empty_bar[st], (uint32_t)(rank ^ 1));
-          if (HALO && (k + 1 == item.k1 || (k + 1) % 9 == 0)) mbar_arrive(&patch_empty_bar[pb]);
-        }
+      };
+      auto fold = [&](float (&d)[NR]) {
+        wgmma_fence_operand(d);
 #pragma unroll
         for (int j = 0; j < NR; ++j) racc[j] = __fadd_rn(racc[j], d[j]);
+      };
+      if constexpr (PIPE) {
+        // slices alternate between d0 and d1 at compile-time-known places (a run-time choice of the tile serialises
+        // the wgmma); the loop runs two slices per trip, the tail finishes one or two
+        const int k1 = item.k1;
+        int k = item.k0;
+        float d0[NR], d1[NR];
+        TcSlice s0 = acquire(k, git), s1;
+        tc_slice_mma<WN>(d0, s0);
+        for (; k + 2 < k1; k += 2, git += 2) {
+          s1 = acquire(k + 1, git + 1);
+          tc_slice_mma<WN>(d1, s1);
+          wgmma_wait1();                              // slice k done, k + 1 in flight
+          release(k, s0);
+          fold(d0);
+          s0 = acquire(k + 2, git + 2);
+          tc_slice_mma<WN>(d0, s0);
+          wgmma_wait1();
+          release(k + 1, s1);
+          fold(d1);
+        }
+        if (k + 1 < k1) {
+          s1 = acquire(k + 1, git + 1);
+          tc_slice_mma<WN>(d1, s1);
+          wgmma_wait1();
+          release(k, s0);
+          fold(d0);
+          wgmma_wait0();
+          release(k + 1, s1);
+          fold(d1);
+          git += 2;
+        } else {
+          wgmma_wait0();
+          release(k, s0);
+          fold(d0);
+          git += 1;
+        }
+      } else {
+        for (int k = item.k0; k < item.k1; ++k, ++git) {
+          const TcSlice s = acquire(k, git);
+          float d[NR];
+          tc_slice_mma<WN>(d, s);
+          wgmma_wait0();
+          release(k, s);
+          fold(d);
+        }
       }
 
       // ---- stream-K fix-up.  Partial-sum layout [column][row] of the 128 x BN tile, one slot per CTA.
@@ -723,10 +789,10 @@ void conv_workspace_free(ConvWorkspace& w) {
   w.partials = nullptr; w.flags = nullptr; w.ctas = 0;
 }
 
-template <int BN, int STAGES, int NCWG = 2, bool PAIR = false, bool HALO = false>
+template <int BN, int STAGES, int NCWG, bool PAIR, bool HALO, bool PIPE>
 static void launch_tc_cfg(const TcArgs& a, ConvWorkspace* sk, int streamk, int sm_reserve, cudaStream_t st) {
   using Cfg = TcCfg<BN, STAGES, NCWG, PAIR, HALO>;
-  auto kernel = conv_tc_kernel<BN, STAGES, NCWG, PAIR, HALO>;
+  auto kernel = conv_tc_kernel<BN, STAGES, NCWG, PAIR, HALO, PIPE>;
   // cudaFuncSetAttribute is per device: one flag per (kernel instance, device)
   static bool attr_set[LUMI_MAX_DEVICES] = {false};
   int dev = 0;
@@ -800,6 +866,13 @@ static void launch_tc_cfg(const TcArgs& a, ConvWorkspace* sk, int streamk, int s
   LUMI_CUDA_CHECK(cudaGetLastError());
 }
 
+// io.pipe selects the double-buffered slice accumulators (the single-buffered loop is kept for A/B runs)
+template <int BN, int STAGES, int NCWG = 2, bool PAIR = false, bool HALO = false>
+static void launch_tc(const TcArgs& a, const ConvIO& io, cudaStream_t st) {
+  if (io.pipe) launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, true>(a, io.sk, io.streamk, io.sm_reserve, st);
+  else launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, false>(a, io.sk, io.streamk, io.sm_reserve, st);
+}
+
 void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
   LUMI_REQUIRE(conv_tc_supported(L, io), "conv_tc: layer not supported by the tensor-core kernel");
   LUMI_REQUIRE(io.in.c == L.cin, "conv_tc: channel mismatch");
@@ -848,17 +921,17 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
   a.overflow = io.overflow_flag;
   // operands per stage: 64 KB (BN = 128) or 48 KB (BN = 64), B only for HALO (next to two 72 KB patch buffers)
   if (halo) {
-    if (pair) launch_tc_cfg<128, 2, 2, true, true>(a, io.sk, io.streamk, io.sm_reserve, st);
-    else if (bn == 128) launch_tc_cfg<128, 2, 2, false, true>(a, io.sk, io.streamk, io.sm_reserve, st);
-    else launch_tc_cfg<64, 4, 2, false, true>(a, io.sk, io.streamk, io.sm_reserve, st);
+    if (pair) launch_tc<128, 2, 2, true, true>(a, io, st);
+    else if (bn == 128) launch_tc<128, 2, 2, false, true>(a, io, st);
+    else launch_tc<64, 4, 2, false, true>(a, io, st);
     return;
   }
   // four consumer warpgroups (sixteen epilogue warps) for the shortest-K layers (io.epi16 = largest K-slice count)
   const bool epi16 = io.epi16 && bn == 128 && !io.out_f32 && n_iters_all <= io.epi16;
-  if (pair) launch_tc_cfg<128, 3, 2, true>(a, io.sk, io.streamk, io.sm_reserve, st);
-  else if (epi16) launch_tc_cfg<128, 3, 4>(a, io.sk, io.streamk, io.sm_reserve, st);
-  else if (bn == 128) launch_tc_cfg<128, 3>(a, io.sk, io.streamk, io.sm_reserve, st);
-  else launch_tc_cfg<64, 4>(a, io.sk, io.streamk, io.sm_reserve, st);
+  if (pair) launch_tc<128, 3, 2, true>(a, io, st);
+  else if (epi16) launch_tc<128, 3, 4>(a, io, st);
+  else if (bn == 128) launch_tc<128, 3>(a, io, st);
+  else launch_tc<64, 4>(a, io, st);
 }
 
 // ---------------------------------------------------------------- host: weight packing

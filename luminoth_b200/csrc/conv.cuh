@@ -51,6 +51,7 @@ struct ConvIO {
   int cta2 = 0;                 // 2-CTA cluster kernel (weight tile multicast) on layers with at least this many K slices per tile (0 = never)
   int halo = 0;                 // halo-patch kernels on 3x3 stride-1 SAME layers without residual or fp32 output (0 never; on CTA pairs with cta2)
   int halo_tiles_pct = 150;     // ... while their M-tile count stays within this percentage of the generic kernel's
+  int pipe = 1;                 // 1: double-buffered slice accumulators (slice k + 1's MMAs overlap slice k's fold); 0: single (the engine's default, LUMI_CONV_PIPE)
   int epi16 = 0;                // four-consumer-warpgroup (16 epilogue warps) kernel on layers with at most this many K slices per tile (0 = never)
   int sm_reserve = 0;           // SMs a persistent launch leaves free (the engine's two-stream pipeline sets 8)
   // Optional strided ("Toeplitz") view of the input for the tensor-core path: element pitches between

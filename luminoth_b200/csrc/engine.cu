@@ -116,11 +116,12 @@ struct lumi_engine {
   int* d_overflow = nullptr;
   ConvWorkspace sk_ws[2];       // stream-K scratch, one per stream
   int conv_streamk = 1;         // 0 off, 1 auto, 2 whenever possible
-  // conv kernel variants, all off by default (not timed on H100 yet; see DESIGN 7.2):
+  // conv kernel variants; the defaults are the fastest setting measured on the Faster R-CNN R50 workload (DESIGN 7.2):
   int conv_cta2 = 0;            // env LUMI_CONV_2CTA: 2-CTA cluster kernel on layers with at least this many K slices per tile
   int conv_halo = 0;            // env LUMI_CONV_HALO: 1 = halo-patch kernels on the 3x3 stride-1 layers
   int conv_halo_pct = 150;      // env LUMI_CONV_HALO_PCT: ... while the M-tile count stays within this percentage of the generic kernel's
-  int conv_epi16 = 0;           // env LUMI_CONV_EPI16: four-warpgroup kernel on layers with at most this many K slices per tile
+  int conv_epi16 = 16;          // env LUMI_CONV_EPI16: four-warpgroup kernel on layers with at most this many K slices per tile
+  int conv_pipe = 0;            // env LUMI_CONV_PIPE: 1 = double-buffered slice accumulators in the conv mainloop (slower on R50, DESIGN 7.1)
   uint8_t* d_images = nullptr; size_t images_cap = 0;
   float* d_boxes = nullptr; float* d_scores = nullptr; int* d_labels = nullptr; int* d_counts = nullptr;
   int* d_prop_counts = nullptr;
@@ -657,6 +658,7 @@ Act run_conv(Ctx& cx, const std::string& key, Act in, int padding, const Act* re
   io.halo = cx.e->conv_halo;
   io.halo_tiles_pct = cx.e->conv_halo_pct;
   io.epi16 = cx.e->conv_epi16;
+  io.pipe = cx.e->conv_pipe;
   if (!cx.dry) {
     const bool tc = cx.e->conv_impl == 1 && conv_tc_supported(L, io);
     const double flops = algorithmic_flops >= 0 ? algorithmic_flops
@@ -1166,6 +1168,7 @@ int lumi_finalize(lumi_engine* e) {
   if (const char* v = std::getenv("LUMI_CONV_HALO")) e->conv_halo = std::max(0, std::min(1, std::atoi(v)));
   if (const char* v = std::getenv("LUMI_CONV_HALO_PCT")) e->conv_halo_pct = std::max(0, std::atoi(v));
   if (const char* v = std::getenv("LUMI_CONV_EPI16")) e->conv_epi16 = std::max(0, std::atoi(v));
+  if (const char* v = std::getenv("LUMI_CONV_PIPE")) e->conv_pipe = std::atoi(v) != 0;
   if (const char* v = std::getenv("LUMI_GRAPHS")) e->use_graphs = std::atoi(v) != 0;
   if (e->max_batch >= 2) {
     conv_workspace_create(e->sk_ws[1]);
