@@ -12,7 +12,8 @@
 //    shifted (possibly negative) coordinates; out-of-bounds elements are
 //    zero-filled by TMA, which IS the TF SAME zero padding.  Persistent CTAs
 //    (whole tiles or stream-K) of one producer and two or four consumer
-//    warpgroups, mbarrier operand ring.  Variants: 2-CTA clusters that
+//    warpgroups, mbarrier operand ring; split-plane outputs leave through shared-memory
+//    epilogue slots (TMA residual prefetch, TMA stores).  Variants: 2-CTA clusters that
 //    multicast the weight tile, and halo-patch kernels for 3x3 layers.
 //
 // Replaces slim conv2d+batch_norm+relu (luminoth/models/base/base_network.py:143-151),
@@ -200,6 +201,9 @@ void launch_conv_simt(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
 // =====================================================================================
 struct TcArgs {
   CUtensorMap tm_a_hi, tm_a_lo, tm_b_hi, tm_b_lo;
+  // slot epilogue (SLOTS > 0): output and residual planes as boxes {64 ch, tw, th, nb} (residual with the traversal
+  // stride res_stride)
+  CUtensorMap tm_o_hi, tm_o_lo, tm_r_hi, tm_r_lo;
   const float* scale; const float* bias;
   __half* out_hi; __half* out_lo; float* out_f32;
   const __half* res_hi; const __half* res_lo;
@@ -270,16 +274,25 @@ constexpr int TC_HALO_PLANE_BYTES = TC_HALO_ROWS * TC_HALO_PITCH;
 // with half the accumulator registers each, for the short-K layers whose time is mostly epilogue).
 // PAIR: a 2-CTA cluster shares one N tile between two M tiles; each CTA loads HALF of the weight tile and multicasts
 // it into both CTAs' shared memory, halving the weight traffic from L2.
-template <int BN, int STAGES, int NCWG = 2, bool PAIR = false, bool HALO = false>
+// SLOTS > 0: split-plane outputs leave through a ring of SLOTS epilogue slots (one 64-column group of the tile, hi and
+// lo plane, in the SWIZZLE_128B layout of a box {64 ch, tw, th, nb}): the producer prefetches the residual into the
+// slot, the consumers overwrite it with the result in place and one thread TMA-stores it.  0: register epilogue.
+template <int BN, int STAGES, int NCWG = 2, bool PAIR = false, bool HALO = false, int SLOTS = 0>
 struct TcCfg {
   static_assert(NCWG == 2 || NCWG == 4, "two or four consumer warpgroups");
   static_assert(!PAIR || BN == 128, "the cluster pair exists for BN = 128");
   static constexpr int WN = BN * 2 / NCWG;                         // columns per consumer warpgroup
+  static_assert(SLOTS == 0 || (!PAIR && !HALO && WN % 64 == 0), "slot epilogue: generic kernel, whole column groups");
+  // four warpgroups: each column group's pair waits only on its own groups' slot phases, so every slot must carry
+  // the same column group (a waiter two phases behind would read the other parity as complete)
+  static_assert(NCWG == 2 || SLOTS % 2 == 0, "four warpgroups: an even slot count");
   static constexpr int B_BYTES = BN * 128;                         // BN weight rows x 64 fp16
   static constexpr int A_STAGE_BYTES = HALO ? 0 : 2 * TC_A_BYTES;  // HALO: A lives in the patch buffers
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + 2 * B_BYTES;  // A hi, A lo, B hi, B lo
   static constexpr int PATCH_BYTES = HALO ? 2 * TC_HALO_PLANE_BYTES : 0;   // one patch buffer: hi + lo plane
-  static constexpr int SMEM_BYTES = 2 * PATCH_BYTES + STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int SLOT_BYTES = 2 * TC_A_BYTES;                // 128 rows x 64 fp16, hi + lo plane
+  static constexpr int SMEM_BYTES = 2 * PATCH_BYTES + STAGES * STAGE_BYTES + SLOTS * SLOT_BYTES + 1024 /*align slack*/ +
+                                    256 /*barriers*/;
   static_assert(SMEM_BYTES <= 232448, "shared memory per CTA");
   static constexpr int THREADS = (1 + NCWG) * 128;   // warpgroup 0: TMA producer (one thread), then the consumers
   // register split: the producer warpgroup keeps the minimum and hands the rest to the consumers.  setmaxnreg.inc
@@ -332,20 +345,30 @@ __device__ __forceinline__ void tc_slice_mma(float (&d)[WN / 2], const TcSlice& 
 // folded; without it every slice drains the warpgroup's wgmma queue before the fold.  Both orders fold the same tiles
 // in ascending k, so the results are bit-identical.
 // Epilogue: scale/bias (folded BN) -> +residual -> relu/relu6 -> fp32 or hi/lo split.
-template <int BN, int STAGES, int NCWG, bool PAIR, bool HALO, bool PIPE>
-__global__ void __launch_bounds__(TcCfg<BN, STAGES, NCWG, PAIR, HALO>::THREADS, 1)
+// SLOTS > 0 (split outputs): per 64-column group of a tile, in order, the slot ring carries
+//   producer: wait slot empty -> TMA-load the residual boxes (hi, lo) into it, or arrive without bytes;
+//   consumers of those columns: wait slot full -> read the residual -> the same arithmetic as the register epilogue ->
+//     write hi / lo over it in place -> fence.proxy.async -> named barrier -> one thread TMA-stores both boxes;
+//   that thread frees the slot once cp.async.bulk.wait_group.read shows the store has read it.
+// TMA zero-fills the out-of-range part of a residual box and clips it on the store, so edge tiles need no masking.
+template <int BN, int STAGES, int NCWG, bool PAIR, bool HALO, bool PIPE, int SLOTS>
+__global__ void __launch_bounds__(TcCfg<BN, STAGES, NCWG, PAIR, HALO, SLOTS>::THREADS, 1)
 conv_tc_kernel(const __grid_constant__ TcArgs a) {
-  using Cfg = TcCfg<BN, STAGES, NCWG, PAIR, HALO>;
+  using Cfg = TcCfg<BN, STAGES, NCWG, PAIR, HALO, SLOTS>;
   constexpr int WN = Cfg::WN;
   constexpr int NR = WN / 2;                          // accumulator registers per thread (64 rows x WN / 128 threads)
+  constexpr int NGT = BN / 64;                        // 64-column groups (slots) per tile
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* patch = smem;                              // HALO: [2 buffers][hi, lo][18 rows x 2048 B]
   uint8_t* stages = smem + 2 * Cfg::PATCH_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stages + STAGES * Cfg::STAGE_BYTES);
+  uint8_t* slots = stages + STAGES * Cfg::STAGE_BYTES;   // [SLOTS][hi, lo][128 rows x 128 B]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(slots + SLOTS * Cfg::SLOT_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* patch_full_bar = empty_bar + STAGES;      // [2]
   uint64_t* patch_empty_bar = patch_full_bar + 2;     // [2]
+  uint64_t* slot_full_bar = patch_empty_bar + 2;      // [SLOTS]
+  uint64_t* slot_empty_bar = slot_full_bar + SLOTS;   // [SLOTS]
 
   // PAIR: rank in the cluster; the scheduling unit is the pair, whose CTAs take M tiles 2 m and 2 m + 1 of one N tile
   const int rank = PAIR ? (int)cluster_ctarank() : 0;
@@ -362,9 +385,14 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
     // empty: one arrival per consumer warpgroup of every CTA whose shared memory the stage's copies write
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], (PAIR ? 2 : 1) * NCWG); }
     for (int s = 0; s < 2; ++s) { mbar_init(&patch_full_bar[s], 1); mbar_init(&patch_empty_bar[s], NCWG); }
+    for (int s = 0; s < SLOTS; ++s) { mbar_init(&slot_full_bar[s], 1); mbar_init(&slot_empty_bar[s], 1); }
     fence_mbar_init();
     tma_prefetch_desc(&a.tm_a_hi); tma_prefetch_desc(&a.tm_a_lo);
     tma_prefetch_desc(&a.tm_b_hi); tma_prefetch_desc(&a.tm_b_lo);
+    if (SLOTS) {
+      tma_prefetch_desc(&a.tm_o_hi); tma_prefetch_desc(&a.tm_o_lo);
+      if (a.res_hi) { tma_prefetch_desc(&a.tm_r_hi); tma_prefetch_desc(&a.tm_r_lo); }
+    }
   }
   if (PAIR) cluster_sync_all();        // both CTAs' barriers exist before either multicasts into the other
   else __syncthreads();
@@ -375,7 +403,8 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
       // ---------------- TMA producer: one (tap, 64-channel) slice per stage
       const uint32_t stage_tx = (HALO ? 0u : 2u * (uint32_t)rows_valid * 128u) + 2u * (uint32_t)Cfg::B_BYTES;
       const uint32_t patch_tx = 2u * (uint32_t)(a.th + 2) * (uint32_t)((TC_HALO_TW + 2) * 128);
-      uint32_t git = 0, gpatch = 0;
+      const uint32_t res_tx = 2u * (uint32_t)rows_valid * 128u;
+      uint32_t git = 0, gpatch = 0, gslot = 0;
       TcSched sched(a.sk_mode, total_tiles, n_iters, sched_id, sched_n);
       TcItem item;
       while (sched.next(item)) {
@@ -422,6 +451,23 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
             tma_load_2d(bbase + Cfg::B_BYTES, &a.tm_b_lo, &full_bar[st], kcol, n0);
           }
         }
+        // the tile's slots, after its K slices (which need no slot): the CTA holding the head of the tile runs the
+        // epilogue.  The residual lands while the consumers work through those slices.
+        if constexpr (SLOTS > 0) {
+          for (int g = 0; g < NGT && item.k0 == 0; ++g, ++gslot) {
+            const uint32_t sl = gslot % SLOTS;
+            mbar_wait(&slot_empty_bar[sl], ((gslot / SLOTS) & 1u) ^ 1u);
+            if (a.res_hi) {
+              uint8_t* sb = slots + sl * Cfg::SLOT_BYTES;
+              mbar_arrive_expect_tx(&slot_full_bar[sl], res_tx);
+              tma_load_4d(sb, &a.tm_r_hi, &slot_full_bar[sl], n0 + g * 64, x0 * a.res_stride, y0 * a.res_stride, img0);
+              tma_load_4d(sb + TC_A_BYTES, &a.tm_r_lo, &slot_full_bar[sl], n0 + g * 64, x0 * a.res_stride,
+                          y0 * a.res_stride, img0);
+            } else {
+              mbar_arrive(&slot_full_bar[sl]);
+            }
+          }
+        }
       }
     }
   } else {
@@ -433,6 +479,10 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
     const int lrow = ((threadIdx.x & 127) >> 5) * 16 + ((threadIdx.x & 31) >> 2);   // + 8 for the odd register pairs
     const int lcol = 2 * (threadIdx.x & 3);
     uint32_t git = 0, gpatch = 0;
+    // slot epilogue: the slot sequence of the producer, and the stores of this warpgroup pair's columns are issued
+    // (and their slots freed, in order from `rel`) by thread 0 of the row-0 warpgroup
+    uint32_t gslot = 0, rel = 0;
+    const bool slot_issuer = (threadIdx.x & 127) == 0 && (c & 1) == 0;
     TcSched sched(a.sk_mode, total_tiles, n_iters, sched_id, sched_n);
     TcItem item;
     while (sched.next(item)) {
@@ -580,61 +630,139 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
             asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(a.sk_flags + (PAIR ? 2 * unit + rank : unit)), "r"(0) : "memory");
       }
 
-      // ---- scale/bias (folded BN) -> +residual -> activation -> store; two rows per thread, column pairs
+      if constexpr (SLOTS > 0) {
+        // ---- slot epilogue, one 64-column group at a time (the arithmetic of the register epilogue below)
+        bool row_ok[2];                                 // the overflow flag counts real output elements only
 #pragma unroll
-      for (int hrow = 0; hrow < 2; ++hrow) {
-        const int row = wrow + lrow + hrow * 8;
-        bool valid = row < rows_valid;
-        int n_img = 0, oy = 0, ox = 0;
-        if (valid) {
-          const int nl = row / (a.th * a.tw);
-          const int rem = row % (a.th * a.tw);
-          n_img = img0 + nl; oy = y0 + rem / a.tw; ox = x0 + rem % a.tw;
-          valid = n_img < a.n && oy < a.ho && ox < a.wo;
+        for (int hrow = 0; hrow < 2; ++hrow) {
+          const int row = wrow + lrow + hrow * 8;
+          bool valid = row < rows_valid;
+          if (valid) {
+            const int nl = row / (a.th * a.tw), rem = row % (a.th * a.tw);
+            valid = img0 + nl < a.n && y0 + rem / a.tw < a.ho && x0 + rem % a.tw < a.wo;
+          }
+          row_ok[hrow] = valid;
         }
-        const size_t opix = ((size_t)n_img * a.ho + oy) * a.wo + ox;
-        size_t rpix = 0;
-        if (a.res_hi)
-          rpix = ((size_t)n_img * a.res_h + (size_t)oy * a.res_stride) * a.res_w + (size_t)ox * a.res_stride;
         bool ovf = false;
 #pragma unroll
-        for (int jb = 0; jb < WN / 8; ++jb) {
-          const int c0 = n0 + jb * 8 + lcol;
-          if (!valid || c0 >= a.cout) continue;
-          // scale / bias vectors are padded to cout_pad (even): 8 B loads are always in bounds
-          const float2 sc = __ldg(reinterpret_cast<const float2*>(a.scale + c0));
-          const float2 bi = __ldg(reinterpret_cast<const float2*>(a.bias + c0));
-          float v0 = fmaf(racc[jb * 4 + hrow * 2 + 0], sc.x, bi.x);
-          float v1 = fmaf(racc[jb * 4 + hrow * 2 + 1], sc.y, bi.y);
-          if (a.res_hi) {              // residual tensors always have cout % 32 == 0 channels
-            const __half2 h2 = *reinterpret_cast<const __half2*>(a.res_hi + rpix * a.cout + c0);
-            const __half2 l2 = *reinterpret_cast<const __half2*>(a.res_lo + rpix * a.cout + c0);
-            v0 = add_f16_pair(v0, __low2half(h2), __low2half(l2));
-            v1 = add_f16_pair(v1, __high2half(h2), __high2half(l2));
-          }
-          v0 = apply_act(v0, a.act);
-          v1 = apply_act(v1, a.act);
-          if (a.out_f32) {
-            float* op = a.out_f32 + opix * a.cout + c0;
-            if ((a.cout & 1) == 0) {
-              *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
-            } else {
-              op[0] = v0;
-              if (c0 + 1 < a.cout) op[1] = v1;
+        for (int i = 0; i < WN / 64; ++i) {
+          const int cg = wcol / 64 + i;
+          const uint32_t gs = gslot + cg, sl = gs % SLOTS;
+          uint8_t* sb = slots + sl * Cfg::SLOT_BYTES;
+          mbar_wait(&slot_full_bar[sl], (gs / SLOTS) & 1u);
+#pragma unroll
+          for (int jl = 0; jl < 8; ++jl) {
+            const int jb = i * 8 + jl;
+            const int c0 = n0 + jb * 8 + lcol;
+            const float2 sc = __ldg(reinterpret_cast<const float2*>(a.scale + c0));
+            const float2 bi = __ldg(reinterpret_cast<const float2*>(a.bias + c0));
+#pragma unroll
+            for (int hrow = 0; hrow < 2; ++hrow) {
+              // row r of the box, 16 B chunk (column / 8) ^ (r % 8): a warp's 8 rows x 16 B hit all 32 banks once
+              const int row = wrow + lrow + hrow * 8;
+              const int off = row * 128 + ((jl ^ (row & 7)) << 4) + lcol * 2;
+              __half2* ph = reinterpret_cast<__half2*>(sb + off);
+              __half2* pl = reinterpret_cast<__half2*>(sb + TC_A_BYTES + off);
+              float v0 = fmaf(racc[jb * 4 + hrow * 2 + 0], sc.x, bi.x);
+              float v1 = fmaf(racc[jb * 4 + hrow * 2 + 1], sc.y, bi.y);
+              if (a.res_hi) {
+                const __half2 h2 = *ph, l2 = *pl;
+                v0 = add_f16_pair(v0, __low2half(h2), __low2half(l2));
+                v1 = add_f16_pair(v1, __high2half(h2), __high2half(l2));
+              }
+              v0 = apply_act(v0, a.act);
+              v1 = apply_act(v1, a.act);
+              __half2 h2, l2;
+              split2_f32(v0, v1, h2, l2);
+              const uint32_t ab = *reinterpret_cast<const uint32_t*>(&h2);
+              ovf |= row_ok[hrow] && c0 < a.cout &&
+                     (((ab & 0x7C00u) == 0x7C00u) || ((ab & 0x7C000000u) == 0x7C000000u));
+              *ph = h2;                                 // in place: each thread rewrites only what it read
+              *pl = l2;
             }
-          } else {                     // split outputs always have cout % 32 == 0
-            // packed split: hi = rn16(v), lo = rn16(v - hi); an fp16 overflow shows up as inf/nan in the hi plane
-            __half2 h2, l2;
-            split2_f32(v0, v1, h2, l2);
-            const uint32_t ab = *reinterpret_cast<const uint32_t*>(&h2);
-            ovf |= ((ab & 0x7C00u) == 0x7C00u) || ((ab & 0x7C000000u) == 0x7C000000u);
-            *reinterpret_cast<__half2*>(a.out_hi + opix * a.cout + c0) = h2;
-            *reinterpret_cast<__half2*>(a.out_lo + opix * a.cout + c0) = l2;
+          }
+          fence_proxy_async();                          // the generic-proxy writes, before the TMA store reads them
+          named_bar_sync(2 + cg, 256);                  // the two warpgroups that own rows 0-63 / 64-127 of these columns
+          if (slot_issuer) {
+            const int oc = n0 - wcol + cg * 64;
+            tma_store_4d(&a.tm_o_hi, sb, oc, x0, y0, img0);
+            tma_store_4d(&a.tm_o_lo, sb + TC_A_BYTES, oc, x0, y0, img0);
+            bulk_commit_group();
+            if constexpr (NCWG == 4) {                  // one issuer per column group, one slot each (SLOTS == 2)
+              bulk_wait_group_read<0>();
+              mbar_arrive(&slot_empty_bar[sl]);
+            } else if (i + 1 == NGT || SLOTS < NGT) {
+              // free the slots whose stores have read them: before the tile's next group when it needs this slot,
+              // else at the end of the tile; with a spare slot in the ring the newest store stays in flight
+              constexpr int KEEP = SLOTS > NGT ? 1 : 0;
+              const bool last = i + 1 == NGT;
+              if (last) bulk_wait_group_read<KEEP>();
+              else bulk_wait_group_read<0>();
+              for (const uint32_t upto = gs + 1 - (last ? KEEP : 0); rel < upto; ++rel)
+                mbar_arrive(&slot_empty_bar[rel % SLOTS]);
+            }
           }
         }
+        gslot += NGT;
         if (ovf && a.overflow) atomicOr(a.overflow, 1);
+      } else {
+        // ---- scale/bias (folded BN) -> +residual -> activation -> store; two rows per thread, column pairs
+#pragma unroll
+        for (int hrow = 0; hrow < 2; ++hrow) {
+          const int row = wrow + lrow + hrow * 8;
+          bool valid = row < rows_valid;
+          int n_img = 0, oy = 0, ox = 0;
+          if (valid) {
+            const int nl = row / (a.th * a.tw);
+            const int rem = row % (a.th * a.tw);
+            n_img = img0 + nl; oy = y0 + rem / a.tw; ox = x0 + rem % a.tw;
+            valid = n_img < a.n && oy < a.ho && ox < a.wo;
+          }
+          const size_t opix = ((size_t)n_img * a.ho + oy) * a.wo + ox;
+          size_t rpix = 0;
+          if (a.res_hi)
+            rpix = ((size_t)n_img * a.res_h + (size_t)oy * a.res_stride) * a.res_w + (size_t)ox * a.res_stride;
+          bool ovf = false;
+#pragma unroll
+          for (int jb = 0; jb < WN / 8; ++jb) {
+            const int c0 = n0 + jb * 8 + lcol;
+            if (!valid || c0 >= a.cout) continue;
+            // scale / bias vectors are padded to cout_pad (even): 8 B loads are always in bounds
+            const float2 sc = __ldg(reinterpret_cast<const float2*>(a.scale + c0));
+            const float2 bi = __ldg(reinterpret_cast<const float2*>(a.bias + c0));
+            float v0 = fmaf(racc[jb * 4 + hrow * 2 + 0], sc.x, bi.x);
+            float v1 = fmaf(racc[jb * 4 + hrow * 2 + 1], sc.y, bi.y);
+            if (a.res_hi) {              // residual tensors always have cout % 32 == 0 channels
+              const __half2 h2 = *reinterpret_cast<const __half2*>(a.res_hi + rpix * a.cout + c0);
+              const __half2 l2 = *reinterpret_cast<const __half2*>(a.res_lo + rpix * a.cout + c0);
+              v0 = add_f16_pair(v0, __low2half(h2), __low2half(l2));
+              v1 = add_f16_pair(v1, __high2half(h2), __high2half(l2));
+            }
+            v0 = apply_act(v0, a.act);
+            v1 = apply_act(v1, a.act);
+            if (a.out_f32) {
+              float* op = a.out_f32 + opix * a.cout + c0;
+              if ((a.cout & 1) == 0) {
+                *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
+              } else {
+                op[0] = v0;
+                if (c0 + 1 < a.cout) op[1] = v1;
+              }
+            } else {                     // split outputs always have cout % 32 == 0
+              // packed split: hi = rn16(v), lo = rn16(v - hi); an fp16 overflow shows up as inf/nan in the hi plane
+              __half2 h2, l2;
+              split2_f32(v0, v1, h2, l2);
+              const uint32_t ab = *reinterpret_cast<const uint32_t*>(&h2);
+              ovf |= ((ab & 0x7C00u) == 0x7C00u) || ((ab & 0x7C000000u) == 0x7C000000u);
+              *reinterpret_cast<__half2*>(a.out_hi + opix * a.cout + c0) = h2;
+              *reinterpret_cast<__half2*>(a.out_lo + opix * a.cout + c0) = l2;
+            }
+          }
+          if (ovf && a.overflow) atomicOr(a.overflow, 1);
+        }
       }
     }
+    if (SLOTS && slot_issuer) bulk_wait_group0();     // the stores are complete before the CTA (and its smem) ends
   }
   // PAIR: the peer's shared memory and barriers must stay alive until both CTAs are done with them
   if (PAIR) cluster_sync_all();
@@ -691,19 +819,21 @@ static CUtensorMap make_map_wgt(const __half* base, int rows, int kdim, int bn) 
 }
 
 // descriptor cache: engine buffers are static, so every (pointer, geometry) repeats each predict call.
+// `kind` keeps the maps of different uses of one pointer apart (an epilogue store map never stands in for a load map).
+enum MapKind { MAP_LOAD = 0, MAP_STORE = 1 };
 struct MapKey {
-  const void* p; int a, b, c, d, e, f, g;
+  const void* p; int a, b, c, d, e, f, g, kind;
   bool operator<(const MapKey& o) const {
-    return std::tie(p, a, b, c, d, e, f, g) < std::tie(o.p, o.a, o.b, o.c, o.d, o.e, o.f, o.g);
+    return std::tie(p, a, b, c, d, e, f, g, kind) < std::tie(o.p, o.a, o.b, o.c, o.d, o.e, o.f, o.g, o.kind);
   }
 };
 static std::map<MapKey, CUtensorMap> g_map_cache;
 static std::mutex g_map_mutex;
 
 static CUtensorMap cached_act_map(const __half* base, int n, int h, int w, int c, int nb, int th, int tw, int stride,
-                                  long pix_pitch, long row_pitch, long img_pitch) {
+                                  long pix_pitch, long row_pitch, long img_pitch, MapKind kind = MAP_LOAD) {
   std::lock_guard<std::mutex> lk(g_map_mutex);
-  MapKey k{base, n, h, w, c + (int)(pix_pitch << 12), nb, th * 16 + stride, tw};
+  MapKey k{base, n, h, w, c + (int)(pix_pitch << 12), nb, th * 16 + stride, tw, kind};
   auto it = g_map_cache.find(k);
   if (it != g_map_cache.end()) return it->second;
   if (g_map_cache.size() > 4096) g_map_cache.clear();
@@ -713,7 +843,7 @@ static CUtensorMap cached_act_map(const __half* base, int n, int h, int w, int c
 }
 static CUtensorMap cached_wgt_map(const __half* base, int rows, int kdim, int bn) {
   std::lock_guard<std::mutex> lk(g_map_mutex);
-  MapKey k{base, rows, kdim, bn, -1, -1, -1, -1};
+  MapKey k{base, rows, kdim, bn, -1, -1, -1, -1, MAP_LOAD};
   auto it = g_map_cache.find(k);
   if (it != g_map_cache.end()) return it->second;
   CUtensorMap m = make_map_wgt(base, rows, kdim, bn);
@@ -789,10 +919,10 @@ void conv_workspace_free(ConvWorkspace& w) {
   w.partials = nullptr; w.flags = nullptr; w.ctas = 0;
 }
 
-template <int BN, int STAGES, int NCWG, bool PAIR, bool HALO, bool PIPE>
+template <int BN, int STAGES, int NCWG, bool PAIR, bool HALO, bool PIPE, int SLOTS>
 static void launch_tc_cfg(const TcArgs& a, ConvWorkspace* sk, int streamk, int sm_reserve, cudaStream_t st) {
-  using Cfg = TcCfg<BN, STAGES, NCWG, PAIR, HALO>;
-  auto kernel = conv_tc_kernel<BN, STAGES, NCWG, PAIR, HALO, PIPE>;
+  using Cfg = TcCfg<BN, STAGES, NCWG, PAIR, HALO, SLOTS>;
+  auto kernel = conv_tc_kernel<BN, STAGES, NCWG, PAIR, HALO, PIPE, SLOTS>;
   // cudaFuncSetAttribute is per device: one flag per (kernel instance, device)
   static bool attr_set[LUMI_MAX_DEVICES] = {false};
   int dev = 0;
@@ -867,10 +997,10 @@ static void launch_tc_cfg(const TcArgs& a, ConvWorkspace* sk, int streamk, int s
 }
 
 // io.pipe selects the double-buffered slice accumulators (the single-buffered loop is kept for A/B runs)
-template <int BN, int STAGES, int NCWG = 2, bool PAIR = false, bool HALO = false>
+template <int BN, int STAGES, int NCWG = 2, bool PAIR = false, bool HALO = false, int SLOTS = 0>
 static void launch_tc(const TcArgs& a, const ConvIO& io, cudaStream_t st) {
-  if (io.pipe) launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, true>(a, io.sk, io.streamk, io.sm_reserve, st);
-  else launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, false>(a, io.sk, io.streamk, io.sm_reserve, st);
+  if (io.pipe) launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, true, SLOTS>(a, io.sk, io.streamk, io.sm_reserve, st);
+  else launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, false, SLOTS>(a, io.sk, io.streamk, io.sm_reserve, st);
 }
 
 void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
@@ -928,8 +1058,24 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
   }
   // four consumer warpgroups (sixteen epilogue warps) for the shortest-K layers (io.epi16 = largest K-slice count)
   const bool epi16 = io.epi16 && bn == 128 && !io.out_f32 && n_iters_all <= io.epi16;
-  if (pair) launch_tc<128, 3, 2, true>(a, io, st);
-  else if (epi16) launch_tc<128, 3, 4>(a, io, st);
+  if (pair) { launch_tc<128, 3, 2, true>(a, io, st); return; }
+  // split outputs leave through the slot epilogue: on an H100 it was faster on every split-output layer of the R50
+  // step, 1x1 and 3x3, short and long K (DESIGN 7.1).  Per instance, the slot count that measured best: two (one per
+  // column group) with four consumers, one next to three operand stages for BN = 128 (the 36-slice 3x3 layers want
+  // the third stage), two next to three stages for BN = 64.
+  if (!io.out_f32 && io.epi_tma) {
+    a.tm_o_hi = cached_act_map(io.out.hi, io.in.n, io.ho, io.wo, L.cout, nb, th, tw, 1, 0, 0, 0, MAP_STORE);
+    a.tm_o_lo = cached_act_map(io.out.lo, io.in.n, io.ho, io.wo, L.cout, nb, th, tw, 1, 0, 0, 0, MAP_STORE);
+    if (io.res.hi) {
+      a.tm_r_hi = cached_act_map(io.res.hi, io.res.n, io.res.h, io.res.w, io.res.c, nb, th, tw, io.res_stride, 0, 0, 0);
+      a.tm_r_lo = cached_act_map(io.res.lo, io.res.n, io.res.h, io.res.w, io.res.c, nb, th, tw, io.res_stride, 0, 0, 0);
+    }
+    if (epi16) launch_tc<128, 2, 4, false, false, 2>(a, io, st);
+    else if (bn == 128) launch_tc<128, 3, 2, false, false, 1>(a, io, st);
+    else launch_tc<64, 3, 2, false, false, 2>(a, io, st);
+    return;
+  }
+  if (epi16) launch_tc<128, 3, 4>(a, io, st);
   else if (bn == 128) launch_tc<128, 3>(a, io, st);
   else launch_tc<64, 4>(a, io, st);
 }

@@ -53,6 +53,7 @@ struct ConvIO {
   int halo_tiles_pct = 150;     // ... while their M-tile count stays within this percentage of the generic kernel's
   int pipe = 1;                 // 1: double-buffered slice accumulators (slice k + 1's MMAs overlap slice k's fold); 0: single (the engine's default, LUMI_CONV_PIPE)
   int epi16 = 0;                // four-consumer-warpgroup (16 epilogue warps) kernel on layers with at most this many K slices per tile (0 = never)
+  int epi_tma = 1;              // 1: split outputs of the generic kernel leave through the shared-memory slot epilogue (TMA); 0: register epilogue
   int sm_reserve = 0;           // SMs a persistent launch leaves free (the engine's two-stream pipeline sets 8)
   // Optional strided ("Toeplitz") view of the input for the tensor-core path: element pitches between
   // consecutive pixels / rows / images (0 = dense NHWC).  Used by the space-to-depth stem, where each

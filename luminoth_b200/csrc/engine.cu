@@ -122,6 +122,7 @@ struct lumi_engine {
   int conv_halo_pct = 150;      // env LUMI_CONV_HALO_PCT: ... while the M-tile count stays within this percentage of the generic kernel's
   int conv_epi16 = 16;          // env LUMI_CONV_EPI16: four-warpgroup kernel on layers with at most this many K slices per tile
   int conv_pipe = 0;            // env LUMI_CONV_PIPE: 1 = double-buffered slice accumulators in the conv mainloop (slower on R50, DESIGN 7.1)
+  int conv_epi_tma = 1;         // env LUMI_CONV_EPI_TMA: 1 = split outputs through the shared-memory slot epilogue, 0 = register epilogue
   uint8_t* d_images = nullptr; size_t images_cap = 0;
   float* d_boxes = nullptr; float* d_scores = nullptr; int* d_labels = nullptr; int* d_counts = nullptr;
   int* d_prop_counts = nullptr;
@@ -659,6 +660,7 @@ Act run_conv(Ctx& cx, const std::string& key, Act in, int padding, const Act* re
   io.halo_tiles_pct = cx.e->conv_halo_pct;
   io.epi16 = cx.e->conv_epi16;
   io.pipe = cx.e->conv_pipe;
+  io.epi_tma = cx.e->conv_epi_tma;
   if (!cx.dry) {
     const bool tc = cx.e->conv_impl == 1 && conv_tc_supported(L, io);
     const double flops = algorithmic_flops >= 0 ? algorithmic_flops
@@ -1169,6 +1171,7 @@ int lumi_finalize(lumi_engine* e) {
   if (const char* v = std::getenv("LUMI_CONV_HALO_PCT")) e->conv_halo_pct = std::max(0, std::atoi(v));
   if (const char* v = std::getenv("LUMI_CONV_EPI16")) e->conv_epi16 = std::max(0, std::atoi(v));
   if (const char* v = std::getenv("LUMI_CONV_PIPE")) e->conv_pipe = std::atoi(v) != 0;
+  if (const char* v = std::getenv("LUMI_CONV_EPI_TMA")) e->conv_epi_tma = std::atoi(v) != 0;
   if (const char* v = std::getenv("LUMI_GRAPHS")) e->use_graphs = std::atoi(v) != 0;
   if (e->max_batch >= 2) {
     conv_workspace_create(e->sk_ws[1]);

@@ -82,20 +82,22 @@ int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wg
     launch_f32_to_act(residual, res->a, st);
     io.res = res->a; io.res_stride = 1;
   }
-  if (impl >= 1 && impl <= 11) {
+  if (impl >= 1 && impl <= 12) {
     // 1 whole tiles, 2 stream-K forced (fp32 outputs written by the epilogue);
     // 3 / 4 / 5: the engine's inter-layer form -- fp16x2 split planes -- with two consumer warpgroups (3), the
-    // four-warpgroup short-K kernel allowed (4), and 4 + stream-K (5); 6 / 7: the 2-CTA cluster kernel wherever it
-    // applies (7: + stream-K); 8-11: the halo-patch kernels (10, 11 on cluster pairs; 9, 11: + stream-K)
+    // four-warpgroup short-K kernel allowed (4), and 4 + stream-K (5), all through the shared-memory slot epilogue;
+    // 6 / 7: the 2-CTA cluster kernel wherever it applies (7: + stream-K); 8-11: the halo-patch kernels (10, 11 on
+    // cluster pairs; 9, 11: + stream-K); 12: as 3 with the register epilogue
     std::unique_ptr<ActBuf> split_out;
     if (impl >= 3) {
       LUMI_REQUIRE(cout % 32 == 0, "conv2d: split outputs need cout % 32 == 0");
       split_out.reset(new ActBuf(n, ho, wo, cout));
       io.out = split_out->a;
       io.out_f32 = nullptr;
+      io.epi_tma = impl == 12 ? 0 : 1;
       io.epi16 = (impl == 4 || impl == 5) ? 8 : 0;
       io.cta2 = (impl == 6 || impl == 7 || impl == 10 || impl == 11) ? 1 : 0;
-      io.halo = (impl >= 8) ? 1 : 0;
+      io.halo = (impl >= 8 && impl <= 11) ? 1 : 0;
       io.halo_tiles_pct = 1000000;                  // test hook: whenever the shape allows
     }
     LUMI_REQUIRE(conv_tc_supported(L, io), "conv2d: this layer shape is not handled by the tensor-core kernel");
