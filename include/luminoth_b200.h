@@ -153,12 +153,27 @@ int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wg
                    int stride, int rate, int padding, const float* scale, const float* bias,
                    const float* residual, int act, int impl, float* y, int* ho, int* wo, void* stream);
 
+/* lumi_op_conv2d with the pre-activation output of a pre-activation ResNet unit, as the engine fuses it into the conv
+ * epilogue: p = relu(fmaf(x^, pre_scale[c], pre_bias[c])) where x^ is the output x as stored in its fp16x2 split
+ * planes.  pre_scale / pre_bias [cout] on DEVICE.  y (x) and p are NHWC fp32 read back from the split planes; y may be
+ * NULL to write p only; y and p both NULL is a shape query.  impl: 0 SIMT, or one of the split-output codes 3-7, 12
+ * (12: as 3 with the register epilogue).  Returns LUMI_EOVERFLOW when x or p exceeds the split range. */
+int lumi_op_conv2d_preact(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout,
+                          int stride, int rate, int padding, const float* scale, const float* bias,
+                          const float* residual, int act, int impl, const float* pre_scale, const float* pre_bias,
+                          float* y, float* p, int* ho, int* wo, void* stream);
+
 /* tf.image.resize_images(BILINEAR) of TF 1.x (legacy kernel, align_corners=False) on one HWC image with 3 channels,
  * utils/image.py:94-97,139-142.  src: DEVICE uint8 (src_is_f32 = 0) or float32 (1) [h0,w0,3]; dst DEVICE float32 [h,w,3]. */
 int lumi_op_resize_bilinear(const void* src, int src_is_f32, int h0, int w0, float* dst, int h, int w, void* stream);
 
 /* max_pool NHWC fp32. padding 0 VALID / 1 SAME. */
 int lumi_op_max_pool(const float* x, int n, int h, int w, int c, int k, int stride, int padding, float* y, void* stream);
+
+/* max_pool followed by the pre-activation of a pre-activation ResNet unit: y = relu(fmaf(m^, pre_scale[c],
+ * pre_bias[c])), m^ the max as stored in its split planes.  pre_scale / pre_bias [c] on DEVICE. */
+int lumi_op_max_pool_preact(const float* x, int n, int h, int w, int c, int k, int stride, int padding,
+                            const float* pre_scale, const float* pre_bias, float* y, void* stream);
 
 /* ROI crop (2ph x 2pw bilinear) + 2x2 max pool: roi_pool.py:68-95.
  * rois [r,4] (x1,y1,x2,y2) px of image 0..; roi_batch [r] image index; y [r,ph,pw,c]. */

@@ -42,10 +42,13 @@ struct SimtArgs {
   __half* out_hi; __half* out_lo; float* out_f32;
   const __half* res_hi; const __half* res_lo; int res_h, res_w, res_stride;
   int* overflow;
+  const float* pre_scale; const float* pre_bias; __half* pre_hi; __half* pre_lo;   // PRE: see ConvIO::pre
 };
 
 constexpr int SM_BM = 128, SM_BN = 64, SM_BK = 16;
 
+// PRE: the layer also writes the pre-activation output p (out_hi == nullptr: p only)
+template <bool PRE>
 __global__ void __launch_bounds__(256) conv_simt_kernel(const SimtArgs a) {
   __shared__ float As[SM_BK][SM_BM + 4];
   __shared__ float Bs[SM_BK][SM_BN + 4];
@@ -170,8 +173,17 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const SimtArgs a) {
         if (!(fabsf(v) <= LUMI_F16_MAX) && a.overflow) atomicOr(a.overflow, 1);
         __half hi, lo;
         split_f32(v, hi, lo);
-        a.out_hi[obase + c] = hi;
-        a.out_lo[obase + c] = lo;
+        if (!PRE || a.out_hi) {
+          a.out_hi[obase + c] = hi;
+          a.out_lo[obase + c] = lo;
+        }
+        if constexpr (PRE) {
+          const float p = fmaxf(fmaf(join_f16(hi, lo), a.pre_scale[c], a.pre_bias[c]), 0.f);
+          if (!(p <= LUMI_F16_MAX) && a.overflow) atomicOr(a.overflow, 1);
+          split_f32(p, hi, lo);
+          a.pre_hi[obase + c] = hi;
+          a.pre_lo[obase + c] = lo;
+        }
       }
     }
   }
@@ -188,10 +200,13 @@ void launch_conv_simt(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
   a.out_hi = io.out.hi; a.out_lo = io.out.lo; a.out_f32 = io.out_f32;
   a.res_hi = io.res.hi; a.res_lo = io.res.lo; a.res_h = io.res.h; a.res_w = io.res.w; a.res_stride = io.res_stride;
   a.overflow = io.overflow_flag;
+  a.pre_scale = io.pre_scale; a.pre_bias = io.pre_bias; a.pre_hi = io.pre.hi; a.pre_lo = io.pre.lo;
+  LUMI_REQUIRE(!io.pre.hi || (!io.out_f32 && io.pre_scale && io.pre_bias), "conv_simt: bad pre-activation output");
   long M = (long)a.n * a.ho * a.wo;
   if (M == 0) return;
   dim3 grid((unsigned)cdiv64(M, SM_BM), (unsigned)cdiv(L.cout, SM_BN));
-  conv_simt_kernel<<<grid, 256, 0, st>>>(a);
+  if (io.pre.hi) conv_simt_kernel<true><<<grid, 256, 0, st>>>(a);
+  else conv_simt_kernel<false><<<grid, 256, 0, st>>>(a);
   count_launch();
   LUMI_CUDA_CHECK(cudaGetLastError());
 }
@@ -204,6 +219,10 @@ struct TcArgs {
   // slot epilogue (SLOTS > 0): output and residual planes as boxes {64 ch, tw, th, nb} (residual with the traversal
   // stride res_stride)
   CUtensorMap tm_o_hi, tm_o_lo, tm_r_hi, tm_r_lo;
+  // PRE: the pre-activation planes (ConvIO::pre) as store boxes; with p only (out_hi == nullptr) tm_o_* describe them
+  CUtensorMap tm_p_hi, tm_p_lo;
+  const float* pre_scale; const float* pre_bias;
+  __half* pre_hi; __half* pre_lo;
   const float* scale; const float* bias;
   __half* out_hi; __half* out_lo; float* out_f32;
   const __half* res_hi; const __half* res_lo;
@@ -333,6 +352,18 @@ __device__ __forceinline__ void tc_slice_mma(float (&d)[WN / 2], const TcSlice& 
   wgmma_commit();
 }
 
+// The pre-activation output of a column pair, in place: (h2, l2) holding x as split become p = relu(fmaf(x^, s, b)) as
+// split.  Returns whether p overflows the fp16 hi plane.
+__device__ __forceinline__ bool tc_preact(__half2& h2, __half2& l2, const float* s, const float* b, int c0) {
+  const float2 sc = __ldg(reinterpret_cast<const float2*>(s + c0));
+  const float2 bi = __ldg(reinterpret_cast<const float2*>(b + c0));
+  const float p0 = fmaxf(fmaf(__low2float(h2) + __low2float(l2), sc.x, bi.x), 0.f);
+  const float p1 = fmaxf(fmaf(__high2float(h2) + __high2float(l2), sc.y, bi.y), 0.f);
+  split2_f32(p0, p1, h2, l2);
+  const uint32_t ab = *reinterpret_cast<const uint32_t*>(&h2);
+  return ((ab & 0x7C00u) == 0x7C00u) || ((ab & 0x7C000000u) == 0x7C000000u);
+}
+
 // Persistent: grid = min(#tiles, #SMs) (or #SMs for stream-K); every CTA (or CTA pair) walks its schedule.  One
 // producer thread keeps a ring of STAGES (tap, 64-channel) K slices in flight with TMA: im2col is fused -- one 4-D box
 // {64 ch, tw, th, nb} per filter tap at shifted (possibly negative) coordinates, zero-filled outside the map, which IS
@@ -351,10 +382,17 @@ __device__ __forceinline__ void tc_slice_mma(float (&d)[WN / 2], const TcSlice& 
 //     write hi / lo over it in place -> fence.proxy.async -> named barrier -> one thread TMA-stores both boxes;
 //   that thread frees the slot once cp.async.bulk.wait_group.read shows the store has read it.
 // TMA zero-fills the out-of-range part of a residual box and clips it on the store, so edge tiles need no masking.
-template <int BN, int STAGES, int NCWG, bool PAIR, bool HALO, bool PIPE, int SLOTS>
+// PRE (split outputs only): the layer also writes the pre-activation output p = relu(fmaf(x^, pre_scale, pre_bias)) of
+// ConvIO::pre.  The register epilogue writes its planes next to x's.  The slot epilogue has no room for a second slot
+// ring (four consumers: 2 x 64 KB stages + 2 x 32 KB slots already), so p reuses the slot: x is stored, the issuer
+// waits until that store has read the slot and releases the column group's warpgroups, each thread rewrites the
+// values it wrote with p and a second store follows; the slot is freed after the second store has read it.  With
+// p only (out_hi == nullptr) the slot carries p in the first place and one store (through tm_o_*) suffices.
+template <int BN, int STAGES, int NCWG, bool PAIR, bool HALO, bool PIPE, int SLOTS, bool PRE>
 __global__ void __launch_bounds__(TcCfg<BN, STAGES, NCWG, PAIR, HALO, SLOTS>::THREADS, 1)
 conv_tc_kernel(const __grid_constant__ TcArgs a) {
   using Cfg = TcCfg<BN, STAGES, NCWG, PAIR, HALO, SLOTS>;
+  static_assert(!PRE || !HALO, "pre-activation outputs: generic and 2-CTA kernels");
   constexpr int WN = Cfg::WN;
   constexpr int NR = WN / 2;                          // accumulator registers per thread (64 rows x WN / 128 threads)
   constexpr int NGT = BN / 64;                        // 64-column groups (slots) per tile
@@ -392,6 +430,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
     if (SLOTS) {
       tma_prefetch_desc(&a.tm_o_hi); tma_prefetch_desc(&a.tm_o_lo);
       if (a.res_hi) { tma_prefetch_desc(&a.tm_r_hi); tma_prefetch_desc(&a.tm_r_lo); }
+      if (PRE && a.out_hi) { tma_prefetch_desc(&a.tm_p_hi); tma_prefetch_desc(&a.tm_p_lo); }
     }
   }
   if (PAIR) cluster_sync_all();        // both CTAs' barriers exist before either multicasts into the other
@@ -644,11 +683,13 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
           row_ok[hrow] = valid;
         }
         bool ovf = false;
+        const bool p_only = PRE && a.out_hi == nullptr;
 #pragma unroll
         for (int i = 0; i < WN / 64; ++i) {
           const int cg = wcol / 64 + i;
           const uint32_t gs = gslot + cg, sl = gs % SLOTS;
           uint8_t* sb = slots + sl * Cfg::SLOT_BYTES;
+          const int oc = n0 - wcol + cg * 64;
           mbar_wait(&slot_full_bar[sl], (gs / SLOTS) & 1u);
 #pragma unroll
           for (int jl = 0; jl < 8; ++jl) {
@@ -677,6 +718,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
               const uint32_t ab = *reinterpret_cast<const uint32_t*>(&h2);
               ovf |= row_ok[hrow] && c0 < a.cout &&
                      (((ab & 0x7C00u) == 0x7C00u) || ((ab & 0x7C000000u) == 0x7C000000u));
+              if (p_only) ovf |= row_ok[hrow] && c0 < a.cout && tc_preact(h2, l2, a.pre_scale, a.pre_bias, c0);
               *ph = h2;                                 // in place: each thread rewrites only what it read
               *pl = l2;
             }
@@ -684,10 +726,38 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
           fence_proxy_async();                          // the generic-proxy writes, before the TMA store reads them
           named_bar_sync(2 + cg, 256);                  // the two warpgroups that own rows 0-63 / 64-127 of these columns
           if (slot_issuer) {
-            const int oc = n0 - wcol + cg * 64;
             tma_store_4d(&a.tm_o_hi, sb, oc, x0, y0, img0);
             tma_store_4d(&a.tm_o_lo, sb + TC_A_BYTES, oc, x0, y0, img0);
             bulk_commit_group();
+          }
+          if (PRE && !p_only) {
+            // x + p: once the store of x has read the slot, every thread turns the x^ it wrote into p in place
+            if (slot_issuer) bulk_wait_group_read<0>();
+            named_bar_sync(2 + cg, 256);
+#pragma unroll
+            for (int jl = 0; jl < 8; ++jl) {
+              const int c0 = n0 + (i * 8 + jl) * 8 + lcol;
+#pragma unroll
+              for (int hrow = 0; hrow < 2; ++hrow) {
+                const int row = wrow + lrow + hrow * 8;
+                const int off = row * 128 + ((jl ^ (row & 7)) << 4) + lcol * 2;
+                __half2* ph = reinterpret_cast<__half2*>(sb + off);
+                __half2* pl = reinterpret_cast<__half2*>(sb + TC_A_BYTES + off);
+                __half2 h2 = *ph, l2 = *pl;
+                ovf |= row_ok[hrow] && c0 < a.cout && tc_preact(h2, l2, a.pre_scale, a.pre_bias, c0);
+                *ph = h2;
+                *pl = l2;
+              }
+            }
+            fence_proxy_async();
+            named_bar_sync(2 + cg, 256);
+            if (slot_issuer) {
+              tma_store_4d(&a.tm_p_hi, sb, oc, x0, y0, img0);
+              tma_store_4d(&a.tm_p_lo, sb + TC_A_BYTES, oc, x0, y0, img0);
+              bulk_commit_group();
+            }
+          }
+          if (slot_issuer) {
             if constexpr (NCWG == 4) {                  // one issuer per column group, one slot each (SLOTS == 2)
               bulk_wait_group_read<0>();
               mbar_arrive(&slot_empty_bar[sl]);
@@ -754,8 +824,15 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
               split2_f32(v0, v1, h2, l2);
               const uint32_t ab = *reinterpret_cast<const uint32_t*>(&h2);
               ovf |= ((ab & 0x7C00u) == 0x7C00u) || ((ab & 0x7C000000u) == 0x7C000000u);
-              *reinterpret_cast<__half2*>(a.out_hi + opix * a.cout + c0) = h2;
-              *reinterpret_cast<__half2*>(a.out_lo + opix * a.cout + c0) = l2;
+              if (!PRE || a.out_hi) {
+                *reinterpret_cast<__half2*>(a.out_hi + opix * a.cout + c0) = h2;
+                *reinterpret_cast<__half2*>(a.out_lo + opix * a.cout + c0) = l2;
+              }
+              if constexpr (PRE) {
+                ovf |= tc_preact(h2, l2, a.pre_scale, a.pre_bias, c0);
+                *reinterpret_cast<__half2*>(a.pre_hi + opix * a.cout + c0) = h2;
+                *reinterpret_cast<__half2*>(a.pre_lo + opix * a.cout + c0) = l2;
+              }
             }
           }
           if (ovf && a.overflow) atomicOr(a.overflow, 1);
@@ -876,6 +953,7 @@ bool conv_tc_supported(const ConvLayer& L, const ConvIO& io) {
   if (L.cin % 64 != 0) return false;
   if (io.out_f32 == nullptr && (L.cout % 32) != 0) return false;
   if (io.res.hi && (L.cout % 32) != 0) return false;
+  if (io.pre.hi && (io.out_f32 || !io.pre_scale || !io.pre_bias)) return false;
   return true;
 }
 
@@ -919,10 +997,10 @@ void conv_workspace_free(ConvWorkspace& w) {
   w.partials = nullptr; w.flags = nullptr; w.ctas = 0;
 }
 
-template <int BN, int STAGES, int NCWG, bool PAIR, bool HALO, bool PIPE, int SLOTS>
+template <int BN, int STAGES, int NCWG, bool PAIR, bool HALO, bool PIPE, int SLOTS, bool PRE>
 static void launch_tc_cfg(const TcArgs& a, ConvWorkspace* sk, int streamk, int sm_reserve, cudaStream_t st) {
   using Cfg = TcCfg<BN, STAGES, NCWG, PAIR, HALO, SLOTS>;
-  auto kernel = conv_tc_kernel<BN, STAGES, NCWG, PAIR, HALO, PIPE, SLOTS>;
+  auto kernel = conv_tc_kernel<BN, STAGES, NCWG, PAIR, HALO, PIPE, SLOTS, PRE>;
   // cudaFuncSetAttribute is per device: one flag per (kernel instance, device)
   static bool attr_set[LUMI_MAX_DEVICES] = {false};
   int dev = 0;
@@ -996,11 +1074,19 @@ static void launch_tc_cfg(const TcArgs& a, ConvWorkspace* sk, int streamk, int s
   LUMI_CUDA_CHECK(cudaGetLastError());
 }
 
-// io.pipe selects the double-buffered slice accumulators (the single-buffered loop is kept for A/B runs)
+// io.pipe selects the double-buffered slice accumulators (the single-buffered loop is kept for A/B runs); a
+// pre-activation output selects the PRE instances, which exist for the non-halo kernels only
 template <int BN, int STAGES, int NCWG = 2, bool PAIR = false, bool HALO = false, int SLOTS = 0>
 static void launch_tc(const TcArgs& a, const ConvIO& io, cudaStream_t st) {
-  if (io.pipe) launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, true, SLOTS>(a, io.sk, io.streamk, io.sm_reserve, st);
-  else launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, false, SLOTS>(a, io.sk, io.streamk, io.sm_reserve, st);
+  if constexpr (!HALO) {
+    if (io.pre.hi) {
+      if (io.pipe) launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, true, SLOTS, true>(a, io.sk, io.streamk, io.sm_reserve, st);
+      else launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, false, SLOTS, true>(a, io.sk, io.streamk, io.sm_reserve, st);
+      return;
+    }
+  }
+  if (io.pipe) launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, true, SLOTS, false>(a, io.sk, io.streamk, io.sm_reserve, st);
+  else launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, false, SLOTS, false>(a, io.sk, io.streamk, io.sm_reserve, st);
 }
 
 void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
@@ -1018,7 +1104,7 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
   // generic one.
   bool halo = false;
   if (io.halo && L.kh == 3 && L.kw == 3 && L.stride == 1 && L.rate == 1 && io.pad_t == 1 && io.pad_l == 1 &&
-      !io.res.hi && !io.out_f32 && !io.in_pix_pitch && !io.in_row_pitch && !io.in_img_pitch) {
+      !io.res.hi && !io.out_f32 && !io.pre.hi && !io.in_pix_pitch && !io.in_row_pitch && !io.in_img_pitch) {
     const int h_tiles = cdiv(io.ho, 16), h_th = cdiv(io.ho, h_tiles);
     const long std_tiles = (long)cdiv(io.in.n, nb) * cdiv(io.ho, th) * cdiv(io.wo, tw);
     const long halo_tiles = (long)io.in.n * h_tiles * cdiv(io.wo, TC_HALO_TW);
@@ -1049,6 +1135,7 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
   a.n_tiles = L.cout_pad / bn;
   a.stride = L.stride;
   a.overflow = io.overflow_flag;
+  a.pre_scale = io.pre_scale; a.pre_bias = io.pre_bias; a.pre_hi = io.pre.hi; a.pre_lo = io.pre.lo;
   // operands per stage: 64 KB (BN = 128) or 48 KB (BN = 64), B only for HALO (next to two 72 KB patch buffers)
   if (halo) {
     if (pair) launch_tc<128, 2, 2, true, true>(a, io, st);
@@ -1064,8 +1151,17 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
   // column group) with four consumers, one next to three operand stages for BN = 128 (the 36-slice 3x3 layers want
   // the third stage), two next to three stages for BN = 64.
   if (!io.out_f32 && io.epi_tma) {
-    a.tm_o_hi = cached_act_map(io.out.hi, io.in.n, io.ho, io.wo, L.cout, nb, th, tw, 1, 0, 0, 0, MAP_STORE);
-    a.tm_o_lo = cached_act_map(io.out.lo, io.in.n, io.ho, io.wo, L.cout, nb, th, tw, 1, 0, 0, 0, MAP_STORE);
+    if (io.pre.hi) {
+      a.tm_p_hi = cached_act_map(io.pre.hi, io.in.n, io.ho, io.wo, L.cout, nb, th, tw, 1, 0, 0, 0, MAP_STORE);
+      a.tm_p_lo = cached_act_map(io.pre.lo, io.in.n, io.ho, io.wo, L.cout, nb, th, tw, 1, 0, 0, 0, MAP_STORE);
+    }
+    if (io.out.hi) {
+      a.tm_o_hi = cached_act_map(io.out.hi, io.in.n, io.ho, io.wo, L.cout, nb, th, tw, 1, 0, 0, 0, MAP_STORE);
+      a.tm_o_lo = cached_act_map(io.out.lo, io.in.n, io.ho, io.wo, L.cout, nb, th, tw, 1, 0, 0, 0, MAP_STORE);
+    } else {                                     // p only: the slot's one store carries p
+      a.tm_o_hi = a.tm_p_hi;
+      a.tm_o_lo = a.tm_p_lo;
+    }
     if (io.res.hi) {
       a.tm_r_hi = cached_act_map(io.res.hi, io.res.n, io.res.h, io.res.w, io.res.c, nb, th, tw, io.res_stride, 0, 0, 0);
       a.tm_r_lo = cached_act_map(io.res.lo, io.res.n, io.res.h, io.res.w, io.res.c, nb, th, tw, io.res_stride, 0, 0, 0);

@@ -41,6 +41,13 @@ struct ConvIO {
   Act in;
   Act out;                  // split-plane output (used when out_f32 == nullptr)
   float* out_f32 = nullptr; // optional fp32 NHWC output [n,ho,wo,cout]
+  // optional pre-activation output (pre.hi == nullptr -> none), split planes like `out`:
+  //   p = relu(fmaf(x^, pre_scale[c], pre_bias[c])),  x^ = float(hi) + float(lo) of the layer's output x as split,
+  // i.e. exactly what a separate "read x, batch norm, relu" pass over the stored x gives.  out.hi == nullptr with
+  // pre.hi set writes p only.  pre_scale / pre_bias are padded to a multiple of 128 channels.
+  Act pre;
+  const float* pre_scale = nullptr;
+  const float* pre_bias = nullptr;
   Act res;                  // optional residual (res.hi == nullptr -> none)
   int res_stride = 1;       // residual sampled at (oy*res_stride, ox*res_stride)  (slim `subsample`)
   int pad_t = 0, pad_l = 0;

@@ -203,9 +203,13 @@ void launch_act_to_f32(Act in, float* y, cudaStream_t st) {
 
 // max pool, 8 channels per thread (C % 8 == 0) -- slim max_pool2d / tf.nn.max_pool.
 // Padded cells are ignored (TF pads with -inf).
+// PRE: writes p = relu(fmaf(m^, pre_scale[c], pre_bias[c])) instead of the max m, with m^ = m as split and rejoined
+// (the batch norm follows the max: a negative gamma does not commute with it).
+template <bool PRE>
 __global__ void max_pool_kernel(const __half* __restrict__ ihi, const __half* __restrict__ ilo,
                                 __half* __restrict__ ohi, __half* __restrict__ olo, int n, int h, int w, int c,
-                                int ho, int wo, int k, int stride, int pad_t, int pad_l) {
+                                int ho, int wo, int k, int stride, int pad_t, int pad_l,
+                                const float* __restrict__ pre_scale, const float* __restrict__ pre_bias) {
   const int cv = c >> 3;
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   size_t total = (size_t)n * ho * wo * cv;
@@ -237,17 +241,29 @@ __global__ void max_pool_kernel(const __half* __restrict__ ihi, const __half* __
   __half* qh = reinterpret_cast<__half*>(&oh);
   __half* ql = reinterpret_cast<__half*>(&ol);
 #pragma unroll
-  for (int j = 0; j < 8; ++j) split_f32(best[j], qh[j], ql[j]);
+  for (int j = 0; j < 8; ++j) {
+    split_f32(best[j], qh[j], ql[j]);
+    if constexpr (PRE) {
+      const int ch = c8 * 8 + j;
+      split_f32(fmaxf(fmaf(join_f16(qh[j], ql[j]), pre_scale[ch], pre_bias[ch]), 0.f), qh[j], ql[j]);
+    }
+  }
   size_t ooff = p * c + (size_t)c8 * 8;
   *reinterpret_cast<uint4*>(ohi + ooff) = oh;
   *reinterpret_cast<uint4*>(olo + ooff) = ol;
 }
-void launch_max_pool(Act in, Act out, int k, int stride, int pad_t, int pad_l, cudaStream_t st) {
+void launch_max_pool(Act in, Act out, int k, int stride, int pad_t, int pad_l, cudaStream_t st,
+                     const float* pre_scale, const float* pre_bias) {
   LUMI_REQUIRE(in.c % 8 == 0 && in.c == out.c && in.n == out.n, "max_pool: C must be a multiple of 8");
+  LUMI_REQUIRE(!pre_scale == !pre_bias, "max_pool: pre_scale and pre_bias go together");
   size_t total = (size_t)out.n * out.h * out.w * (out.c / 8);
   if (!total) return;
-  max_pool_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(in.hi, in.lo, out.hi, out.lo, in.n, in.h, in.w, in.c,
-                                                               out.h, out.w, k, stride, pad_t, pad_l);
+  if (pre_scale)
+    max_pool_kernel<true><<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(
+        in.hi, in.lo, out.hi, out.lo, in.n, in.h, in.w, in.c, out.h, out.w, k, stride, pad_t, pad_l, pre_scale, pre_bias);
+  else
+    max_pool_kernel<false><<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(
+        in.hi, in.lo, out.hi, out.lo, in.n, in.h, in.w, in.c, out.h, out.w, k, stride, pad_t, pad_l, nullptr, nullptr);
   count_launch();
   LUMI_CUDA_CHECK(cudaGetLastError());
 }

@@ -58,8 +58,13 @@ struct Tap {
   int64_t shape[4] = {0, 0, 0, 0};
 };
 
-const int RESNET_UNITS_50[4] = {3, 4, 6, 3};
-const int RESNET_UNITS_101[4] = {3, 4, 23, 3};
+// Faster R-CNN base networks (truncated_base_network.py:8-16): units per block; `preact` marks slim resnet_v2, the
+// pre-activation ResNet (each unit starts with relu(BN(x)); conv3 and the projection shortcut carry biases)
+struct ResnetArch { const char* name; int units[4]; bool preact; };
+const ResnetArch RESNETS[6] = {
+    {"resnet_v1_50", {3, 4, 6, 3}, false}, {"resnet_v1_101", {3, 4, 23, 3}, false},
+    {"resnet_v1_152", {3, 8, 36, 3}, false}, {"resnet_v2_50", {3, 4, 6, 3}, true},
+    {"resnet_v2_101", {3, 4, 23, 3}, true}, {"resnet_v2_152", {3, 8, 36, 3}, true}};
 const int BASE_DEPTH[4] = {64, 128, 256, 512};
 const int BLOCK_STRIDE[4] = {2, 2, 2, 1};
 const float RGB_MEANS[3] = {123.68f, 116.78f, 103.94f};
@@ -77,6 +82,7 @@ struct lumi_engine {
   bool debug_taps = false;      // materialise intermediates that the fused path skips (roi_pool)
 
   std::string type, arch;
+  const ResnetArch* resnet = nullptr;         // Faster R-CNN base network
   int num_classes = 0;
   bool with_rcnn = true, use_tail = true, use_mean = true;
   int output_stride = 16;
@@ -188,21 +194,40 @@ void need_conv_bn(lumi_engine* e, const std::string& scope, int kh, int kw, int 
   need_bn(e, scope, cout);
 }
 
+void need_conv_bias(lumi_engine* e, const std::string& scope, int kh, int kw, int cin, int cout) {
+  need(e, scope + "/weights", {kh, kw, cin, cout});
+  need(e, scope + "/biases", {cout});
+}
+
+std::string unit_scope(const lumi_engine* e, int b, int u) {
+  return "truncated_base_network/" + e->arch + "/block" + std::to_string(b + 1) + "/unit_" + std::to_string(u + 1) +
+         (e->resnet->preact ? "/bottleneck_v2" : "/bottleneck_v1");
+}
+
+// slim resnet_v1 / resnet_v2 variables up to block3 (block4 only for the resnet_v1_101 tail); resnet_v2's `postnorm`
+// follows block4 and is never reached
 void spec_resnet(lumi_engine* e) {
   const std::string root = "truncated_base_network/" + e->arch;
-  const int* units = e->arch == "resnet_v1_50" ? RESNET_UNITS_50 : RESNET_UNITS_101;
-  need_conv_bn(e, root + "/conv1", 7, 7, 3, 64);
+  const bool v2 = e->resnet->preact;
+  if (v2) need_conv_bias(e, root + "/conv1", 7, 7, 3, 64);
+  else need_conv_bn(e, root + "/conv1", 7, 7, 3, 64);
   int cin = 64;
   const bool tail = e->arch == "resnet_v1_101" && e->use_tail && e->with_rcnn;
   const int nblocks = tail ? 4 : 3;
   for (int b = 0; b < nblocks; ++b) {
     const int bd = BASE_DEPTH[b], depth = bd * 4;
-    for (int u = 0; u < units[b]; ++u) {
-      const std::string s = root + "/block" + std::to_string(b + 1) + "/unit_" + std::to_string(u + 1) + "/bottleneck_v1";
-      if (cin != depth) need_conv_bn(e, s + "/shortcut", 1, 1, cin, depth);
+    for (int u = 0; u < e->resnet->units[b]; ++u) {
+      const std::string s = unit_scope(e, b, u);
+      if (v2)
+        for (const char* n : {"gamma", "beta", "moving_mean", "moving_variance"}) need(e, s + "/preact/" + n, {cin});
+      if (cin != depth) {
+        if (v2) need_conv_bias(e, s + "/shortcut", 1, 1, cin, depth);
+        else need_conv_bn(e, s + "/shortcut", 1, 1, cin, depth);
+      }
       need_conv_bn(e, s + "/conv1", 1, 1, cin, bd);
       need_conv_bn(e, s + "/conv2", 3, 3, bd, bd);
-      need_conv_bn(e, s + "/conv3", 1, 1, bd, depth);
+      if (v2) need_conv_bias(e, s + "/conv3", 1, 1, bd, depth);
+      else need_conv_bn(e, s + "/conv3", 1, 1, bd, depth);
       cin = depth;
     }
   }
@@ -254,9 +279,13 @@ void parse_config(lumi_engine* e) {
   LUMI_REQUIRE(e->num_classes > 0, "model.network.num_classes must be positive");
   if (e->type == "fasterrcnn") {
     e->arch = c.str("model.base_network.architecture", "resnet_v1_101");
-    if (e->arch != "resnet_v1_50" && e->arch != "resnet_v1_101")
-      throw Error(LUMI_EINVAL, "base_network.architecture '" + e->arch +
-                                   "' is not built yet (resnet_v1_50 | resnet_v1_101)");
+    std::string known;
+    for (const ResnetArch& r : RESNETS) {
+      if (e->arch == r.name) e->resnet = &r;
+      known += std::string(known.empty() ? "" : " | ") + r.name;
+    }
+    if (!e->resnet)
+      throw Error(LUMI_EINVAL, "base_network.architecture '" + e->arch + "' is not built yet (" + known + ")");
     const JVal* ep = c.find("model.base_network.endpoint");
     if (ep && ep->t == JVal::Str && ep->s != "block3") throw Error(LUMI_EINVAL, "only endpoint block3 is supported");
     e->with_rcnn = c.boolean("model.network.with_rcnn", false);
@@ -429,11 +458,36 @@ void make_conv_bias(lumi_engine* e, const std::string& key, const std::vector<st
   e->layers[key] = L;
 }
 
+// resnet_v2 `preact` batch norm (slim batch_norm, eps 1e-5) folded like make_conv_bn, as the device vectors
+// <scope>/preact#scale and #bias that the producing conv epilogue (or the stem's max pool) applies; padded to a
+// multiple of 128 channels for the tensor-core epilogue's vector loads
+void make_preact(lumi_engine* e, const std::string& scope) {
+  const HostTensor& g = W(e, scope + "/preact/gamma");
+  const HostTensor& b = W(e, scope + "/preact/beta");
+  const HostTensor& m = W(e, scope + "/preact/moving_mean");
+  const HostTensor& v = W(e, scope + "/preact/moving_variance");
+  const int c = (int)g.v.size(), cpad = cdiv(c, 128) * 128;
+  std::vector<float> sc(cpad, 0.f), bi(cpad, 0.f);
+  for (int i = 0; i < c; ++i) {
+    const double s = (double)g.v[i] / std::sqrt((double)v.v[i] + 1e-5);
+    sc[i] = (float)s;
+    bi[i] = (float)((double)b.v[i] - (double)m.v[i] * s);
+  }
+  for (int k = 0; k < 2; ++k) {
+    float* d = nullptr;
+    LUMI_CUDA_CHECK(cudaMalloc(&d, cpad * sizeof(float)));
+    e->dev_vecs[scope + (k ? "/preact#bias" : "/preact#scale")] = d;
+    LUMI_CUDA_CHECK(cudaMemcpy(d, (k ? bi : sc).data(), cpad * sizeof(float), cudaMemcpyHostToDevice));
+  }
+}
+
 void build_layers(lumi_engine* e) {
   if (e->type == "fasterrcnn") {
     const std::string root = "truncated_base_network/" + e->arch;
-    const int* units = e->arch == "resnet_v1_50" ? RESNET_UNITS_50 : RESNET_UNITS_101;
-    make_conv_bn(e, root + "/conv1", 2, 1, ACT_RELU);
+    const int* units = e->resnet->units;
+    const bool v2 = e->resnet->preact;
+    if (v2) make_conv_bias(e, root + "/conv1", {root + "/conv1/weights"}, {root + "/conv1/biases"}, 2, 1, ACT_NONE);
+    else make_conv_bn(e, root + "/conv1", 2, 1, ACT_RELU);
     {   // tensor-core form of the stem: 7x7/2 over 3 channels == 4x4/1 over the 12(+4 pad)-channel
         // space-to-depth input; one filter row r' = 4 taps x 16 ch = one K=64 slice  (kh=4, kw=1, cin=64)
       const HostTensor& w = W(e, root + "/conv1/weights");
@@ -453,7 +507,7 @@ void build_layers(lumi_engine* e) {
       LUMI_CUDA_CHECK(cudaMemcpy(sc.data(), base.scale, 64 * sizeof(float), cudaMemcpyDeviceToHost));
       LUMI_CUDA_CHECK(cudaMemcpy(bi.data(), base.bias, 64 * sizeof(float), cudaMemcpyDeviceToHost));
       ConvLayer L;
-      L.kh = 4; L.kw = 1; L.cin = 64; L.cout = 64; L.stride = 1; L.rate = 1; L.act = ACT_RELU;
+      L.kh = 4; L.kw = 1; L.cin = 64; L.cout = 64; L.stride = 1; L.rate = 1; L.act = base.act;
       conv_layer_upload(L, w2.data(), sc.data(), bi.data());
       e->layers[root + "/conv1#s2d"] = L;
     }
@@ -465,16 +519,26 @@ void build_layers(lumi_engine* e) {
     for (int b = 0; b < nblocks; ++b) {
       const int bd = BASE_DEPTH[b], depth = bd * 4;
       for (int u = 0; u < units[b]; ++u) {
-        const std::string s = root + "/block" + std::to_string(b + 1) + "/unit_" + std::to_string(u + 1) + "/bottleneck_v1";
+        const std::string s = unit_scope(e, b, u);
         int unit_stride = (u == units[b] - 1) ? BLOCK_STRIDE[b] : 1;
         int st = unit_stride, rt = 1;
         if (b == 3) { st = 1; rt = 1; }                       // tail: stack_blocks_dense w/o output_stride, stride 1
         else if (current == target) { st = 1; rt = rate; rate *= unit_stride; }
         else { current *= unit_stride; }
-        if (cin != depth) make_conv_bn(e, s + "/shortcut", st, 1, ACT_NONE);
-        make_conv_bn(e, s + "/conv1", 1, 1, ACT_RELU);
-        make_conv_bn(e, s + "/conv2", st, rt, ACT_RELU);
-        make_conv_bn(e, s + "/conv3", 1, 1, ACT_RELU);        // relu applied after the residual add
+        if (v2) {
+          // bottleneck_v2: preact = relu(BN(x)); shortcut and conv3 with biases, no BN or activation; out = the raw sum
+          make_preact(e, s);
+          if (cin != depth) make_conv_bias(e, s + "/shortcut", {s + "/shortcut/weights"}, {s + "/shortcut/biases"}, st, 1,
+                                           ACT_NONE);
+          make_conv_bn(e, s + "/conv1", 1, 1, ACT_RELU);
+          make_conv_bn(e, s + "/conv2", st, rt, ACT_RELU);
+          make_conv_bias(e, s + "/conv3", {s + "/conv3/weights"}, {s + "/conv3/biases"}, 1, 1, ACT_NONE);
+        } else {
+          if (cin != depth) make_conv_bn(e, s + "/shortcut", st, 1, ACT_NONE);
+          make_conv_bn(e, s + "/conv1", 1, 1, ACT_RELU);
+          make_conv_bn(e, s + "/conv2", st, rt, ACT_RELU);
+          make_conv_bn(e, s + "/conv3", 1, 1, ACT_RELU);      // relu applied after the residual add
+        }
         cin = depth;
       }
     }
@@ -618,9 +682,25 @@ NmsWorkspace ws_view(const NmsWorkspace& ws, int off) {
   return v;
 }
 
+// Pre-activation output of a conv (ConvIO::pre): the next resnet_v2 unit's relu(BN(x)), written by the epilogue as
+// p; keep_x = false leaves x unwritten (run_conv then returns an Act without planes).
+struct PreAct {
+  const float* scale = nullptr;
+  const float* bias = nullptr;
+  bool keep_x = true;
+  Act p;
+};
+PreAct preact_of(lumi_engine* e, const std::string& unit, bool keep_x) {
+  PreAct pa;
+  pa.scale = e->dev_vecs.at(unit + "/preact#scale");
+  pa.bias = e->dev_vecs.at(unit + "/preact#bias");
+  pa.keep_x = keep_x;
+  return pa;
+}
+
 // padding: 0 VALID, 1 SAME, 2 slim conv2d_same (explicit pad + VALID when stride > 1)
 Act run_conv(Ctx& cx, const std::string& key, Act in, int padding, const Act* res, int res_stride, float** out_f32,
-             const long* view_pitch = nullptr, double algorithmic_flops = -1.0) {
+             const long* view_pitch = nullptr, double algorithmic_flops = -1.0, PreAct* pre = nullptr) {
   auto it = cx.e->layers.find(key);
   if (it == cx.e->layers.end()) throw Error(LUMI_ESTATE, "layer '" + key + "' missing (internal)");
   const ConvLayer& L = it->second;
@@ -645,9 +725,14 @@ Act run_conv(Ctx& cx, const std::string& key, Act in, int padding, const Act* re
   if (out_f32) {
     *out_f32 = cx.f32((size_t)in.n * ho * wo * L.cout);
     io.out_f32 = *out_f32;
-  } else {
+  } else if (!pre || pre->keep_x) {
     out = cx.act(in.n, ho, wo, L.cout);
     io.out = out;
+  }
+  if (pre) {
+    LUMI_REQUIRE(!out_f32, "conv '" + key + "': pre-activation outputs are split planes (internal)");
+    pre->p = cx.act(in.n, ho, wo, L.cout);
+    io.pre = pre->p; io.pre_scale = pre->scale; io.pre_bias = pre->bias;
   }
   if (res) { io.res = *res; io.res_stride = res_stride; }
   if (view_pitch) { io.in_pix_pitch = view_pitch[0]; io.in_row_pitch = view_pitch[1]; io.in_img_pitch = view_pitch[2]; }
@@ -673,13 +758,17 @@ Act run_conv(Ctx& cx, const std::string& key, Act in, int padding, const Act* re
   return out;
 }
 
-Act run_pool(Ctx& cx, Act in, int k, int stride, bool same) {
+// pre: returns relu(BN(max pool)) instead of the max pool (the resnet_v2 stem feeds only the first unit's preact)
+Act run_pool(Ctx& cx, Act in, int k, int stride, bool same, const PreAct* pre = nullptr) {
   int ho, wo, pt = 0, pl = 0;
   if (same) { tf_same(in.h, k, stride, 1, ho, pt); tf_same(in.w, k, stride, 1, wo, pl); }
   else { ho = tf_valid(in.h, k, stride, 1); wo = tf_valid(in.w, k, stride, 1); }
   LUMI_REQUIRE(ho > 0 && wo > 0, "max_pool: input too small");
   Act out = cx.act(in.n, ho, wo, in.c);
-  if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_POOL); launch_max_pool(in, out, k, stride, pt, pl, cx.st); }
+  if (!cx.dry) {
+    ProfScope ps(cx.e, cx.dry, PC_POOL);
+    launch_max_pool(in, out, k, stride, pt, pl, cx.st, pre ? pre->scale : nullptr, pre ? pre->bias : nullptr);
+  }
   return out;
 }
 
@@ -692,6 +781,19 @@ Act bottleneck(Ctx& cx, const std::string& s, Act x, int depth) {
   Act r = run_conv(cx, s + "/conv1", x, 1, nullptr, 1, nullptr);
   r = run_conv(cx, s + "/conv2", r, 2, nullptr, 1, nullptr);
   return run_conv(cx, s + "/conv3", r, 1, &shortcut, res_stride, nullptr);
+}
+
+// slim bottleneck_v2 on (x, p = relu(BN_preact(x))); x may be absent when the unit projects its shortcut from p.
+// conv3 writes what the next unit reads, from `next` (nullptr: the endpoint, x only): p always, and x as well when
+// that unit's shortcut is the identity (its depth equals this unit's).
+Act bottleneck_v2(Ctx& cx, const std::string& s, Act x, Act p, int depth, PreAct* next) {
+  const ConvLayer& c2 = cx.e->layers.at(s + "/conv2");
+  Act shortcut = x;
+  int res_stride = c2.stride;                        // subsample(x, stride)
+  if (p.c != depth) { shortcut = run_conv(cx, s + "/shortcut", p, 1, nullptr, 1, nullptr); res_stride = 1; }
+  Act r = run_conv(cx, s + "/conv1", p, 1, nullptr, 1, nullptr);
+  r = run_conv(cx, s + "/conv2", r, 2, nullptr, 1, nullptr);
+  return run_conv(cx, s + "/conv3", r, 1, &shortcut, res_stride, nullptr, nullptr, -1.0, next);
 }
 
 // ---------------------------------------------------------------- Faster R-CNN forward
@@ -730,7 +832,8 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
   int* out_counts = e->d_counts + io;
   float* out_records = e->d_records ? e->d_records + (size_t)io * (1 + 6 * (size_t)e->kmax) : nullptr;
   const std::string root = "truncated_base_network/" + e->arch;
-  const int* units = e->arch == "resnet_v1_50" ? RESNET_UNITS_50 : RESNET_UNITS_101;
+  const int* units = e->resnet->units;
+  const bool v2 = e->resnet->preact;
   Act x;
   if (e->conv_impl == 1) {
     // stem on the tensor cores: mean-subtract + zero-pad + space-to-depth staging, then 4 taps of K=64
@@ -745,12 +848,30 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
     x = cx.act(n, h, w, 3);
     if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_u8_to_act(images, cx.img_f32, x, RGB_MEANS, cx.st); }  // base_network.py:153-177
     x = run_conv(cx, root + "/conv1", x, 2, nullptr, 1, nullptr);        // conv2d_same(64, 7, stride 2) + BN + relu
+  }                                                                      // (v2: + bias, no activation)
+  if (!v2) {
+    x = run_pool(cx, x, 3, 2, true);                                     // pool1 3x3/2 SAME
+    for (int b = 0; b < 3; ++b)
+      for (int u = 0; u < units[b]; ++u) x = bottleneck(cx, unit_scope(e, b, u), x, BASE_DEPTH[b] * 4);
+  } else {
+    // block1/unit_1 projects from its preact: the stem's pool emits only p = relu(BN(pool1))
+    const PreAct first = preact_of(e, unit_scope(e, 0, 0), false);
+    Act p = run_pool(cx, x, 3, 2, true, &first);
+    x = Act();
+    for (int b = 0; b < 3; ++b)
+      for (int u = 0; u < units[b]; ++u) {
+        const bool last_of_block = u + 1 == units[b];
+        if (b == 2 && last_of_block) {                                   // the endpoint: x only
+          x = bottleneck_v2(cx, unit_scope(e, b, u), x, p, BASE_DEPTH[b] * 4, nullptr);
+          break;
+        }
+        // the next unit's shortcut is the identity (reads x) unless it opens the next block (projects from p)
+        PreAct next = last_of_block ? preact_of(e, unit_scope(e, b + 1, 0), false)
+                                    : preact_of(e, unit_scope(e, b, u + 1), true);
+        x = bottleneck_v2(cx, unit_scope(e, b, u), x, p, BASE_DEPTH[b] * 4, &next);
+        p = next.p;
+      }
   }
-  x = run_pool(cx, x, 3, 2, true);                                       // pool1 3x3/2 SAME
-  for (int b = 0; b < 3; ++b)
-    for (int u = 0; u < units[b]; ++u)
-      x = bottleneck(cx, root + "/block" + std::to_string(b + 1) + "/unit_" + std::to_string(u + 1) + "/bottleneck_v1",
-                     x, BASE_DEPTH[b] * 4);
   const Act fmap = x;                                                    // endpoint block3
   cx.tap_act("conv_feature_map", fmap);
   const int fh = fmap.h, fw = fmap.w;

@@ -12,7 +12,9 @@ void launch_stem_s2d(const void* img, bool img_f32, int n, int h, int w, Act x2,
 void launch_resize_bilinear(const void* src, bool src_f32, int h0, int w0, float* dst, int h, int w, cudaStream_t st);
 void launch_pack_c3(const void* img, bool img_f32, int n, int h, int w, Act x2 /*(n,h+2,w+3,16)*/, cudaStream_t st);
 void launch_act_to_f32(Act in, float* y, cudaStream_t st);
-void launch_max_pool(Act in, Act out, int k, int stride, int pad_t, int pad_l, cudaStream_t st);
+// pre_scale / pre_bias [c] (both or neither): out = relu(BN(max)) instead of the max (see elementwise.cu)
+void launch_max_pool(Act in, Act out, int k, int stride, int pad_t, int pad_l, cudaStream_t st,
+                     const float* pre_scale = nullptr, const float* pre_bias = nullptr);
 void launch_l2norm_scale(Act in, Act out, const float* gamma, float eps, cudaStream_t st);
 void launch_spatial_mean(Act in, Act out, cudaStream_t st);               // (R,h,w,C) -> (R,1,1,C)
 void launch_softmax_rows(const float* x, float* y, int rows, int cols, int in_stride, cudaStream_t st);

@@ -32,23 +32,14 @@ struct ActBuf {
 };
 
 int op_fail(const Error& e) { g_op_error = e.what(); return e.code; }
-}  // namespace
 
-#define OP_BEGIN try {
-#define OP_END                                           \
-  }                                                      \
-  catch (const Error& err) { return op_fail(err); }      \
-  catch (const std::exception& ex) { g_op_error = ex.what(); return LUMI_EINVAL; }
-
-extern "C" {
-
-const char* lumi_op_last_error(void) { return g_op_error.c_str(); }
-
-int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout, int stride,
-                   int rate, int padding, const float* scale, const float* bias, const float* residual, int act,
-                   int impl, float* y, int* ho_out, int* wo_out, void* stream) {
-  OP_BEGIN
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+// The arguments of lumi_op_conv2d, plus the pre-activation output of lumi_op_conv2d_preact (pre_scale == nullptr:
+// none; then y is required, else y == nullptr writes p only).
+int op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout, int stride,
+              int rate, int padding, const float* scale, const float* bias, const float* residual, int act, int impl,
+              const float* pre_scale, const float* pre_bias, float* y, float* p, int* ho_out, int* wo_out,
+              cudaStream_t st) {
+  const bool preact = pre_scale != nullptr;
   ConvLayer L;
   L.kh = kh; L.kw = kw; L.cin = cin; L.cout = cout; L.stride = stride; L.rate = rate; L.act = act;
   const size_t nw = (size_t)kh * kw * cin * cout;
@@ -71,7 +62,8 @@ int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wg
   LUMI_REQUIRE(ho > 0 && wo > 0, "conv2d: empty output");
   if (ho_out) *ho_out = ho;
   if (wo_out) *wo_out = wo;
-  if (!y) return LUMI_OK;                 // shape query
+  if (!y && !p) return LUMI_OK;           // shape query
+  LUMI_REQUIRE(preact ? (p && pre_bias) : (y && !p), "conv2d: bad output arguments");
   ActBuf in(n, h, w, cin);
   launch_f32_to_act(x, in.a, st);
   ConvIO io;
@@ -81,6 +73,49 @@ int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wg
     res.reset(new ActBuf(n, ho, wo, cout));
     launch_f32_to_act(residual, res->a, st);
     io.res = res->a; io.res_stride = 1;
+  }
+  if (preact) {
+    // split planes only: x (when y is given) and p, each read back as fp32; the vectors padded like the layer's
+    LUMI_REQUIRE(impl == 0 || (impl >= 3 && impl <= 7) || impl == 12,
+                 "conv2d_preact: impl must be 0 (SIMT) or one of the split-output codes 3-7, 12");
+    LUMI_REQUIRE(cout % 32 == 0, "conv2d_preact: split outputs need cout % 32 == 0");
+    const int cpad = cdiv(cout, 128) * 128;
+    std::vector<float> hv(cpad, 0.f);
+    DevBuf ps(cpad * sizeof(float)), pb(cpad * sizeof(float)), ovf(sizeof(int));
+    LUMI_CUDA_CHECK(cudaMemcpy(hv.data(), pre_scale, cout * sizeof(float), cudaMemcpyDeviceToHost));
+    LUMI_CUDA_CHECK(cudaMemcpy(ps.p, hv.data(), cpad * sizeof(float), cudaMemcpyHostToDevice));
+    LUMI_CUDA_CHECK(cudaMemcpy(hv.data(), pre_bias, cout * sizeof(float), cudaMemcpyDeviceToHost));
+    LUMI_CUDA_CHECK(cudaMemcpy(pb.p, hv.data(), cpad * sizeof(float), cudaMemcpyHostToDevice));
+    LUMI_CUDA_CHECK(cudaMemset(ovf.p, 0, sizeof(int)));
+    std::unique_ptr<ActBuf> xo;
+    if (y) { xo.reset(new ActBuf(n, ho, wo, cout)); io.out = xo->a; }
+    ActBuf po(n, ho, wo, cout);
+    io.out_f32 = nullptr;
+    io.pre = po.a; io.pre_scale = ps.as<float>(); io.pre_bias = pb.as<float>();
+    io.overflow_flag = ovf.as<int>();
+    ConvWorkspace sk;
+    struct SkGuard { ConvWorkspace& w; ~SkGuard() { conv_workspace_free(w); } } skg{sk};
+    if (impl == 0) {
+      launch_conv_simt(L, io, st);
+    } else {
+      io.epi_tma = impl == 12 ? 0 : 1;
+      io.epi16 = (impl == 4 || impl == 5) ? 8 : 0;
+      io.cta2 = (impl == 6 || impl == 7) ? 1 : 0;
+      LUMI_REQUIRE(conv_tc_supported(L, io), "conv2d: this layer shape is not handled by the tensor-core kernel");
+      if (impl == 5 || impl == 7) {
+        conv_workspace_create(sk);
+        io.sk = &sk;
+        io.streamk = 2;
+      }
+      launch_conv_tc(L, io, st);
+    }
+    if (xo) launch_act_to_f32(xo->a, y, st);
+    launch_act_to_f32(po.a, p, st);
+    int flag = 0;
+    LUMI_CUDA_CHECK(cudaMemcpyAsync(&flag, ovf.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
+    if (flag) throw Error(LUMI_EOVERFLOW, "conv2d_preact: an output exceeded the fp16x2 split range (|x| > 65504)");
+    return LUMI_OK;
   }
   if (impl >= 1 && impl <= 12) {
     // 1 whole tiles, 2 stream-K forced (fp32 outputs written by the epilogue);
@@ -116,6 +151,36 @@ int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wg
   }
   LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
   return LUMI_OK;
+}
+}  // namespace
+
+#define OP_BEGIN try {
+#define OP_END                                           \
+  }                                                      \
+  catch (const Error& err) { return op_fail(err); }      \
+  catch (const std::exception& ex) { g_op_error = ex.what(); return LUMI_EINVAL; }
+
+extern "C" {
+
+const char* lumi_op_last_error(void) { return g_op_error.c_str(); }
+
+int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout, int stride,
+                   int rate, int padding, const float* scale, const float* bias, const float* residual, int act,
+                   int impl, float* y, int* ho_out, int* wo_out, void* stream) {
+  OP_BEGIN
+  return op_conv2d(x, n, h, w, cin, wgt, kh, kw, cout, stride, rate, padding, scale, bias, residual, act, impl, nullptr,
+                   nullptr, y, nullptr, ho_out, wo_out, static_cast<cudaStream_t>(stream));
+  OP_END
+}
+
+int lumi_op_conv2d_preact(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout,
+                          int stride, int rate, int padding, const float* scale, const float* bias,
+                          const float* residual, int act, int impl, const float* pre_scale, const float* pre_bias,
+                          float* y, float* p, int* ho_out, int* wo_out, void* stream) {
+  OP_BEGIN
+  LUMI_REQUIRE(pre_scale && pre_bias, "conv2d_preact: pre_scale and pre_bias are required");
+  return op_conv2d(x, n, h, w, cin, wgt, kh, kw, cout, stride, rate, padding, scale, bias, residual, act, impl,
+                   pre_scale, pre_bias, y, p, ho_out, wo_out, static_cast<cudaStream_t>(stream));
   OP_END
 }
 
@@ -138,6 +203,23 @@ int lumi_op_max_pool(const float* x, int n, int h, int w, int c, int k, int stri
   ActBuf in(n, h, w, c), out(n, ho, wo, c);
   launch_f32_to_act(x, in.a, st);
   launch_max_pool(in.a, out.a, k, stride, pt, pl, st);
+  launch_act_to_f32(out.a, y, st);
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
+  return LUMI_OK;
+  OP_END
+}
+
+int lumi_op_max_pool_preact(const float* x, int n, int h, int w, int c, int k, int stride, int padding,
+                            const float* pre_scale, const float* pre_bias, float* y, void* stream) {
+  OP_BEGIN
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  LUMI_REQUIRE(pre_scale && pre_bias, "max_pool_preact: pre_scale and pre_bias are required");
+  int ho, wo, pt = 0, pl = 0;
+  if (padding == 1) { tf_same(h, k, stride, 1, ho, pt); tf_same(w, k, stride, 1, wo, pl); }
+  else { ho = tf_valid(h, k, stride, 1); wo = tf_valid(w, k, stride, 1); }
+  ActBuf in(n, h, w, c), out(n, ho, wo, c);
+  launch_f32_to_act(x, in.a, st);
+  launch_max_pool(in.a, out.a, k, stride, pt, pl, st, pre_scale, pre_bias);
   launch_act_to_f32(out.a, y, st);
   LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
   return LUMI_OK;

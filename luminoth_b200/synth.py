@@ -15,8 +15,12 @@ regressors so probabilities spread and NMS has real work.
 """
 import numpy as np
 
-RESNET_UNITS = {'resnet_v1_50': (3, 4, 6, 3), 'resnet_v1_101': (3, 4, 23, 3)}
+RESNET_UNITS = {'resnet_v1_50': (3, 4, 6, 3), 'resnet_v1_101': (3, 4, 23, 3), 'resnet_v1_152': (3, 8, 36, 3),
+                'resnet_v2_50': (3, 4, 6, 3), 'resnet_v2_101': (3, 4, 23, 3), 'resnet_v2_152': (3, 8, 36, 3)}
 BASE_DEPTH = (64, 128, 256, 512)
+# resnet_v2 adds every unit's conv3 output to the raw residual stream, so its scale grows with depth: conv3 is drawn
+# V2_CONV3_SCALE / sqrt(units in the block) times He init, which keeps block3 at O(1-10) up to resnet_v2_152
+V2_CONV3_SCALE = 0.6
 
 
 def _conv(rng, kh, kw, cin, cout, std=None):
@@ -33,7 +37,44 @@ def _bn(rng, wts, scope, c, gamma_scale=1.0):
     wts[p + 'moving_variance'] = rng.uniform(0.8, 1.2, c).astype(np.float32)
 
 
+def _bias(rng, c):
+    return (rng.standard_normal(c) * 0.05).astype(np.float32)
+
+
+def resnet_v2_weights(rng, arch, scope='truncated_base_network'):
+    """slim resnet_v2 (pre-activation) variables through block3."""
+    wts = {}
+    root = '%s/%s' % (scope, arch)
+    wts[root + '/conv1/weights'] = _conv(rng, 7, 7, 3, 64, std=np.sqrt(2.0 / 147) / 64.0)
+    wts[root + '/conv1/biases'] = _bias(rng, 64)
+    cin = 64
+    for b in range(3):
+        bd = BASE_DEPTH[b]
+        depth = bd * 4
+        for u in range(RESNET_UNITS[arch][b]):
+            s = '%s/block%d/unit_%d/bottleneck_v2' % (root, b + 1, u + 1)
+            p = s + '/preact/'
+            wts[p + 'gamma'] = rng.uniform(0.8, 1.2, cin).astype(np.float32)
+            wts[p + 'beta'] = (rng.standard_normal(cin) * 0.05).astype(np.float32)
+            wts[p + 'moving_mean'] = (rng.standard_normal(cin) * 0.05).astype(np.float32)
+            wts[p + 'moving_variance'] = rng.uniform(0.8, 1.2, cin).astype(np.float32)
+            if cin != depth:
+                wts[s + '/shortcut/weights'] = _conv(rng, 1, 1, cin, depth)
+                wts[s + '/shortcut/biases'] = _bias(rng, depth)
+            wts[s + '/conv1/weights'] = _conv(rng, 1, 1, cin, bd)
+            _bn(rng, wts, s + '/conv1', bd)
+            wts[s + '/conv2/weights'] = _conv(rng, 3, 3, bd, bd)
+            _bn(rng, wts, s + '/conv2', bd)
+            wts[s + '/conv3/weights'] = _conv(rng, 1, 1, bd, depth,
+                                              std=V2_CONV3_SCALE * np.sqrt(2.0 / bd / RESNET_UNITS[arch][b]))
+            wts[s + '/conv3/biases'] = _bias(rng, depth)
+            cin = depth
+    return wts
+
+
 def resnet_weights(rng, arch, with_block4, scope='truncated_base_network'):
+    if arch.startswith('resnet_v2'):
+        return resnet_v2_weights(rng, arch, scope)
     wts = {}
     root = '%s/%s' % (scope, arch)
     # conv1 sees raw pixels minus mean (|x| ~ 60 rms): scale the stem down so
