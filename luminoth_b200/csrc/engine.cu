@@ -270,6 +270,25 @@ void compute_frcnn_anchor_ref(lumi_engine* e) {
   e->A = (int)(ratios.size() * scales.size());
 }
 
+// model.base_network.output_stride, checked as slim's resnet_v1/v2 and resnet_utils.stack_blocks_dense check it over
+// all four blocks (luminoth builds the full network, then truncates it at block3).  null means no atrous
+// convolution: block3 then ends at stride 32, which is the network output_stride 32 builds.
+int frcnn_output_stride(const JVal& c) {
+  const JVal* v = c.find("model.base_network.output_stride");
+  if (v && v->t == JVal::Null) return 32;
+  const double os = c.number("model.base_network.output_stride", 16);
+  if (std::fmod(os, 4.0) != 0.0) throw Error(LUMI_EINVAL, "The output_stride needs to be a multiple of 4.");
+  const double target = os / 4;
+  double current = 1;
+  for (int b = 0; b < 4; ++b)
+    for (int u = 0; u < 3; ++u) {               // 3 units stand for any count: only the last one has a stride
+      if (current > target) throw Error(LUMI_EINVAL, "The target output_stride cannot be reached.");
+      if (current != target && u == 2) current *= BLOCK_STRIDE[b];
+    }
+  if (current != target) throw Error(LUMI_EINVAL, "The target output_stride cannot be reached.");
+  return (int)os;
+}
+
 void parse_config(lumi_engine* e) {
   const JVal& c = e->cfg;
   e->type = c.str("model.type", "");
@@ -290,8 +309,7 @@ void parse_config(lumi_engine* e) {
     if (ep && ep->t == JVal::Str && ep->s != "block3") throw Error(LUMI_EINVAL, "only endpoint block3 is supported");
     e->with_rcnn = c.boolean("model.network.with_rcnn", false);
     e->use_tail = c.boolean("model.base_network.use_tail", true);
-    e->output_stride = (int)c.number("model.base_network.output_stride", 16);
-    LUMI_REQUIRE(e->output_stride == 16, "only output_stride 16 is supported");
+    e->output_stride = frcnn_output_stride(c);
     e->anchor_stride = (int)c.number("model.anchors.stride", 16);
     compute_frcnn_anchor_ref(e);
     e->rpn_channels = (int)c.number("model.rpn.num_channels", 512);
@@ -679,6 +697,10 @@ NmsWorkspace ws_view(const NmsWorkspace& ws, int off) {
     v.alive = ws.alive + (size_t)off * ws.ncap;
     v.nvalid2 = ws.nvalid2 + off;
   }
+  if (ws.cut_hist) {
+    v.cut_hist = ws.cut_hist + (size_t)off * 4 * 256;
+    v.cut_counts = ws.cut_counts + (size_t)off * ws.cut_blocks;
+  }
   return v;
 }
 
@@ -798,10 +820,11 @@ Act bottleneck_v2(Ctx& cx, const std::string& s, Act x, Act p, int depth, PreAct
 
 // ---------------------------------------------------------------- Faster R-CNN forward
 void ensure_frcnn_anchors(lumi_engine* e, int h, int w, cudaStream_t st) {
-  // fasterrcnn.py:261-308; the grid follows the block3 feature map: four ceil-halvings of the image size.
+  // fasterrcnn.py:261-308; the grid follows the block3 feature map, ceil(size / output_stride): every stride-2 stage
+  // (conv2d_same, SAME max pool, subsampled shortcut) gives ceil(x / 2).
   // One buffer per grid shape, kept for the engine's lifetime: captured graphs of other image sizes keep pointing
   // at theirs (a server sees a handful of distinct sizes).
-  const int fh = cdiv(h, 16), fw = cdiv(w, 16);
+  const int fh = cdiv(h, e->output_stride), fw = cdiv(w, e->output_stride);
   if (e->anchors_fh == fh && e->anchors_fw == fw) return;
   auto it = e->anchor_grids.find({fh, fw});
   if (it == e->anchor_grids.end()) {
@@ -1150,7 +1173,7 @@ void ensure_arena(lumi_engine* e, Arena& a, size_t need_bytes) {
 // RPN workspace (the only buffer sized by the image) grows on demand; arenas are re-planned per shape anyway.
 void ensure_image_capacity(lumi_engine* e, int h, int w) {
   if (e->type != "fasterrcnn") return;                 // SSD runs at its configured fixed size only
-  const long na = (long)cdiv(h, 16) * cdiv(w, 16) * e->A;
+  const long na = (long)cdiv(h, e->output_stride) * cdiv(w, e->output_stride) * e->A;
   LUMI_REQUIRE(na < (1L << 30), "lumi_predict: image too large");
   if (na <= e->ws_rpn.cap) return;
   e->drop_graphs();
@@ -1271,7 +1294,7 @@ int lumi_finalize(lumi_engine* e) {
     LUMI_CUDA_CHECK(cudaMalloc(&e->d_anchor_ref, e->anchor_ref.size() * sizeof(int)));
     LUMI_CUDA_CHECK(cudaMemcpy(e->d_anchor_ref, e->anchor_ref.data(), e->anchor_ref.size() * sizeof(int),
                                cudaMemcpyHostToDevice));
-    const int fh = cdiv(e->max_h, 16), fw = cdiv(e->max_w, 16);
+    const int fh = cdiv(e->max_h, e->output_stride), fw = cdiv(e->max_w, e->output_stride);
     nms_workspace_alloc(e->ws_rpn, nb, fh * fw * e->A, e->rpn.post_nms_top_n,
                         std::min(fh * fw * e->A, e->rpn.pre_nms_top_n));
     if (e->with_rcnn) {

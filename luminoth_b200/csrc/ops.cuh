@@ -49,6 +49,10 @@ struct NmsWorkspace {
   int* index_map = nullptr;     // [P][ncap]  compacted row -> row of sboxes
   unsigned char* alive = nullptr;  // [P][ncap]
   int* nvalid2 = nullptr;       // [P]
+  // top-k cut ahead of the sort (ncap < cap, see run_topk_cut): radix-select histograms and per-CTA counts
+  unsigned int* cut_hist = nullptr;         // [P][4 digits][256]
+  unsigned long long* cut_counts = nullptr; // [P][cut_blocks] (candidates above the k-th key << 32 | equal to it)
+  int cut_blocks = 0;
 };
 void nms_workspace_alloc(NmsWorkspace& ws, int problems, int cap, int max_out, int ncap = 0);
 void nms_workspace_free(NmsWorkspace& ws);

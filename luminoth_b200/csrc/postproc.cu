@@ -68,6 +68,8 @@ __device__ __forceinline__ bool iou_gt(float4 a, float4 b, float thr) {
 }
 
 // ------------------------------------------------------------------ workspace
+constexpr int CUT_THREADS = 256, CUT_ITEMS = 16, CUT_CHUNK = CUT_THREADS * CUT_ITEMS;   // candidates per cut CTA
+
 void nms_workspace_alloc(NmsWorkspace& ws, int problems, int cap, int max_out, int ncap) {
   if (ncap <= 0 || ncap > cap) ncap = cap;
   ws.problems = problems; ws.cap = cap; ws.max_out = max_out; ws.ncap = ncap;
@@ -90,11 +92,17 @@ void nms_workspace_alloc(NmsWorkspace& ws, int problems, int cap, int max_out, i
     LUMI_CUDA_CHECK(cudaMalloc(&ws.alive, pn));
     LUMI_CUDA_CHECK(cudaMalloc(&ws.nvalid2, problems * sizeof(int)));
   }
+  if (ncap < cap) {                         // top-k cut scratch (see run_topk_cut)
+    ws.cut_blocks = cdiv(cap, CUT_CHUNK);
+    LUMI_CUDA_CHECK(cudaMalloc(&ws.cut_hist, (size_t)problems * 4 * 256 * sizeof(unsigned int)));
+    LUMI_CUDA_CHECK(cudaMalloc(&ws.cut_counts, (size_t)problems * ws.cut_blocks * sizeof(unsigned long long)));
+  }
 }
 void nms_workspace_free(NmsWorkspace& ws) {
   cudaFree(ws.keys); cudaFree(ws.boxes); cudaFree(ws.order); cudaFree(ws.nvalid); cudaFree(ws.sboxes);
   cudaFree(ws.sscores); cudaFree(ws.mask); cudaFree(ws.keep); cudaFree(ws.nkeep); cudaFree(ws.sort_tmp);
   cudaFree(ws.sboxes2); cudaFree(ws.index_map); cudaFree(ws.alive); cudaFree(ws.nvalid2);
+  cudaFree(ws.cut_hist); cudaFree(ws.cut_counts);
   ws = NmsWorkspace();
 }
 
@@ -110,7 +118,9 @@ __device__ __forceinline__ uint32_t score_key(float s) { return (s >= 0.f) ? (__
 // digit table in shared memory carries the rank across rounds, and one block-wide exclusive scan in
 // digit-major order yields the global offsets.  Two sweeps per pass (count, then scatter) keep register
 // use independent of the problem size; data ping-pongs through L2.
-template <int NWARPS>
+// PAIRS: the input is not `keys` but n_all (~key', original index) pairs already in the first ping-pong buffer,
+// in ascending index order (the output of the top-k cut); `order` then holds those original indices.
+template <int NWARPS, bool PAIRS = false>
 __global__ void __launch_bounds__(NWARPS * 32) sort_desc_radix_kernel(const float* __restrict__ keys, int cap,
                                                                      int n_all, const int* __restrict__ n_in,
                                                                      int topn, unsigned long long* __restrict__ tmp,
@@ -148,7 +158,7 @@ __global__ void __launch_bounds__(NWARPS * 32) sort_desc_radix_kernel(const floa
     unsigned long long* dst = (pass & 1) ? bufA : bufB;
     auto fetch = [&](int i) -> unsigned long long {       // (key', index) of item i of this pass' input
       if (i >= hi) return 0ull;
-      if (pass == 0) {
+      if (pass == 0 && !PAIRS) {
         const uint32_t k = score_key(keys[(size_t)p * cap + i]);
         return ((unsigned long long)(~k) << 32) | (uint32_t)i;
       }
@@ -241,6 +251,207 @@ static void run_sort(const float* keys, int problems, int cap, int n_all, const 
     sort_desc_radix_kernel<32><<<problems, 1024, 0, st>>>(keys, cap, n_all, n_in, topn, tmp, order, nvalid);
   else
     sort_desc_radix_kernel<8><<<problems, 256, 0, st>>>(keys, cap, n_all, n_in, topn, tmp, order, nvalid);
+  count_launch();
+  LUMI_CUDA_CHECK(cudaGetLastError());
+}
+
+// ------------------------------------------------------------------ top-k cut ahead of the sort
+// When a problem has many more candidates than the sort keeps (the RPN at output_stride 8 or 4 has 115 200 or
+// 460 800 anchors per 600x1024 image against pre_nms_top_n = 12 000), the whole GPU first selects the k largest
+// (key', index) pairs and the one-CTA sort then orders only those:
+//   1. radix select, most significant 8-bit digit of key' first: in each of 4 rounds every CTA histograms those of
+//      its candidates that carry the prefix selected so far.  The k-th largest key' T and the count of keys above it
+//      follow from the histograms alone (cut_select, recomputed by every CTA that needs them);
+//   2. stable compaction: every candidate with key' > T plus the first k - count(key' > T) with key' == T, in
+//      ascending index order, written as (~key', index) pairs through per-CTA counts and an exclusive scan;
+//   3. the radix sort of those k pairs.  It is stable and its input is in index order, so `order` and `nvalid` are
+//      the ones the sort of all candidates gives, ties included.
+// The grids depend on the candidate count only, so the chain is captured into CUDA graphs like the rest.
+
+// Radix-select state after `rounds` digits, computed by one warp (every lane gets it): prefix = the top 8 * rounds
+// bits of the k-th largest key', above = the count of keys whose top bits exceed that prefix.
+__device__ __forceinline__ void cut_select(const unsigned int* __restrict__ hist, int rounds, uint32_t k,
+                                           uint32_t& prefix, uint32_t& above) {
+  const int lane = threadIdx.x & 31;
+  prefix = 0; above = 0;
+  uint32_t rem = k;                                   // rank of the wanted key among those carrying the prefix
+  for (int r = 0; r < rounds; ++r) {
+    uint32_t c[8], sum = 0;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { c[j] = hist[r * 256 + 255 - (lane * 8 + j)]; sum += c[j]; }   // digits descending
+    uint32_t incl = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += t;
+    }
+    const int src = __ffs(__ballot_sync(0xffffffffu, incl >= rem)) - 1;
+    uint32_t acc = incl - sum, digit = 0;
+    bool found = false;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      if (!found && acc + c[j] >= rem) { digit = 255 - (lane * 8 + j); found = true; }
+      if (!found) acc += c[j];
+    }
+    digit = __shfl_sync(0xffffffffu, digit, src);
+    acc = __shfl_sync(0xffffffffu, acc, src);
+    rem -= acc; above += acc;
+    prefix = (prefix << 8) | digit;
+  }
+}
+
+// exclusive block-wide scan of v (CUT_THREADS threads); total = the sum over the block
+__device__ __forceinline__ unsigned long long cut_block_scan(unsigned long long v, unsigned long long* s_warp,
+                                                             unsigned long long& total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned long long incl = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += t;
+  }
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  unsigned long long wbase = 0;
+  total = 0;
+#pragma unroll
+  for (int w = 0; w < CUT_THREADS / 32; ++w) {
+    if (w < warp) wbase += s_warp[w];
+    total += s_warp[w];
+  }
+  __syncthreads();
+  return wbase + incl - v;
+}
+
+// round `round` of the select: hist[p][round][d] += candidates carrying the selected prefix, by their next digit d
+__global__ void __launch_bounds__(CUT_THREADS) cut_hist_kernel(const float* __restrict__ keys, int cap, int n, int k,
+                                                               int round, unsigned int* __restrict__ hist) {
+  __shared__ unsigned int sh[256];
+  __shared__ uint32_t s_prefix;
+  const int p = blockIdx.y;
+  unsigned int* H = hist + (size_t)p * 4 * 256;
+  sh[threadIdx.x] = 0;
+  if (threadIdx.x < 32) {
+    uint32_t prefix, above;
+    cut_select(H, round, (uint32_t)k, prefix, above);
+    if (threadIdx.x == 0) s_prefix = prefix;
+  }
+  __syncthreads();
+  const uint32_t prefix = s_prefix;
+  const int shift = 24 - 8 * round;
+  const float* K = keys + (size_t)p * cap;
+  const int base = blockIdx.x * CUT_CHUNK;
+  const uint32_t lt_mask = (1u << (threadIdx.x & 31)) - 1u;
+#pragma unroll 4
+  for (int it = 0; it < CUT_ITEMS; ++it) {
+    const int i = base + it * CUT_THREADS + threadIdx.x;
+    const uint32_t key = i < n ? score_key(K[i]) : 0u;
+    const bool match = i < n && (round == 0 || (key >> (shift + 8)) == prefix);
+    const uint32_t digit = (key >> shift) & 255u;
+    const uint32_t peers = __match_any_sync(0xffffffffu, match ? digit : 256u);   // one shared atomic per digit
+    if (match && (peers & lt_mask) == 0) atomicAdd(&sh[digit], (unsigned int)__popc(peers));
+  }
+  __syncthreads();
+  if (sh[threadIdx.x]) atomicAdd(&H[round * 256 + threadIdx.x], sh[threadIdx.x]);
+}
+
+// per-CTA counts of the candidates above the k-th key' T (high word) and equal to it (low word)
+__global__ void __launch_bounds__(CUT_THREADS) cut_count_kernel(const float* __restrict__ keys, int cap, int n, int k,
+                                                                const unsigned int* __restrict__ hist,
+                                                                unsigned long long* __restrict__ counts, int nblk) {
+  __shared__ uint32_t s_t;
+  __shared__ unsigned long long s_warp[CUT_THREADS / 32];
+  const int p = blockIdx.y;
+  if (threadIdx.x < 32) {
+    uint32_t t, above;
+    cut_select(hist + (size_t)p * 4 * 256, 4, (uint32_t)k, t, above);
+    if (threadIdx.x == 0) s_t = t;
+  }
+  __syncthreads();
+  const uint32_t T = s_t;
+  const float* K = keys + (size_t)p * cap;
+  const int base = blockIdx.x * CUT_CHUNK;
+  unsigned long long c = 0;
+#pragma unroll 4
+  for (int it = 0; it < CUT_ITEMS; ++it) {
+    const int i = base + it * CUT_THREADS + threadIdx.x;
+    if (i < n) {
+      const uint32_t key = score_key(K[i]);
+      c += key > T ? (1ull << 32) : (key == T ? 1ull : 0ull);
+    }
+  }
+  unsigned long long total;
+  cut_block_scan(c, s_warp, total);
+  if (threadIdx.x == 0) counts[(size_t)p * nblk + blockIdx.x] = total;
+}
+
+// stable compaction of the k selected candidates into (~key', index) pairs at out[p][0, k)
+__global__ void __launch_bounds__(CUT_THREADS) cut_scatter_kernel(const float* __restrict__ keys, int cap, int n, int k,
+                                                                  const unsigned int* __restrict__ hist,
+                                                                  const unsigned long long* __restrict__ counts,
+                                                                  int nblk, unsigned long long* __restrict__ tmp) {
+  __shared__ uint32_t s_t, s_above;
+  __shared__ unsigned long long s_warp[CUT_THREADS / 32];
+  const int p = blockIdx.y;
+  if (threadIdx.x < 32) {
+    uint32_t t, above;
+    cut_select(hist + (size_t)p * 4 * 256, 4, (uint32_t)k, t, above);
+    if (threadIdx.x == 0) { s_t = t; s_above = above; }
+  }
+  unsigned long long before = 0;                       // counts of the CTAs before this one
+  for (int j = threadIdx.x; j < blockIdx.x; j += CUT_THREADS) before += counts[(size_t)p * nblk + j];
+  unsigned long long prev;
+  cut_block_scan(before, s_warp, prev);                // also orders s_t / s_above before their reads
+  const uint32_t T = s_t, need_eq = (uint32_t)k - s_above;
+  const float* K = keys + (size_t)p * cap;
+  const int first = blockIdx.x * CUT_CHUNK + threadIdx.x * CUT_ITEMS;   // this thread's contiguous run
+  uint32_t key[CUT_ITEMS];
+  unsigned long long c = 0;
+#pragma unroll
+  for (int j = 0; j < CUT_ITEMS; ++j) {
+    key[j] = first + j < n ? score_key(K[first + j]) : 0u;
+    if (first + j < n) c += key[j] > T ? (1ull << 32) : (key[j] == T ? 1ull : 0ull);
+  }
+  unsigned long long total;
+  const unsigned long long start = prev + cut_block_scan(c, s_warp, total);
+  uint32_t gt = (uint32_t)(start >> 32), eq = (uint32_t)start;
+  unsigned long long* out = tmp + (size_t)p * 2 * cap;
+#pragma unroll
+  for (int j = 0; j < CUT_ITEMS; ++j) {
+    if (first + j >= n) break;
+    const unsigned long long pair = ((unsigned long long)(~key[j]) << 32) | (uint32_t)(first + j);
+    if (key[j] > T) {
+      out[gt + min(eq, need_eq)] = pair;
+      ++gt;
+    } else if (key[j] == T) {
+      if (eq < need_eq) out[gt + eq] = pair;
+      ++eq;
+    }
+  }
+}
+
+// The sort of run_sort over n candidates per problem when only the first k (<= n) are kept; same outputs.
+static void run_topk_cut(const float* keys, int problems, int cap, int n, int k, int* order, int* nvalid,
+                         const NmsWorkspace& ws, cudaStream_t st) {
+  const int nblk = cdiv(n, CUT_CHUNK);
+  LUMI_REQUIRE(ws.cut_hist && nblk <= ws.cut_blocks && k <= n && n <= cap, "top-k cut: missing scratch");
+  LUMI_CUDA_CHECK(cudaMemsetAsync(ws.cut_hist, 0, (size_t)problems * 4 * 256 * sizeof(unsigned int), st));
+  const dim3 g(nblk, problems);
+  for (int r = 0; r < 4; ++r) {
+    cut_hist_kernel<<<g, CUT_THREADS, 0, st>>>(keys, cap, n, k, r, ws.cut_hist);
+    count_launch();
+    LUMI_CUDA_CHECK(cudaGetLastError());
+  }
+  cut_count_kernel<<<g, CUT_THREADS, 0, st>>>(keys, cap, n, k, ws.cut_hist, ws.cut_counts, nblk);
+  count_launch();
+  LUMI_CUDA_CHECK(cudaGetLastError());
+  cut_scatter_kernel<<<g, CUT_THREADS, 0, st>>>(keys, cap, n, k, ws.cut_hist, ws.cut_counts, nblk, ws.sort_tmp);
+  count_launch();
+  LUMI_CUDA_CHECK(cudaGetLastError());
+  if (k > 4096)
+    sort_desc_radix_kernel<32, true><<<problems, 1024, 0, st>>>(keys, cap, k, nullptr, k, ws.sort_tmp, order, nvalid);
+  else
+    sort_desc_radix_kernel<8, true><<<problems, 256, 0, st>>>(keys, cap, k, nullptr, k, ws.sort_tmp, order, nvalid);
   count_launch();
   LUMI_CUDA_CHECK(cudaGetLastError());
 }
@@ -693,6 +904,11 @@ static void run_nms(NmsWorkspace& ws, int problems, float thr, int max_out, cuda
 }
 
 // ------------------------------------------------------------------ RPN chain
+// The top-k cut replaces the one-CTA sort of all anchors from this many anchors per kept candidate on.  On an H100
+// (DESIGN section 4.2) the cut made the R50 step faster at 4 and 6 anchors per kept candidate; at 2.4 its RPN chain
+// was faster but the pipelined step was not, because its full-GPU kernels contend with the other half-batch's convs.
+constexpr long RPN_CUT_RATIO = 4;
+
 __global__ void rpn_decode_kernel(const float* __restrict__ cls, const float* __restrict__ box, long img_stride_cls,
                                   long img_stride_box, int A, const float* __restrict__ anchors, RpnParams p, int cap,
                                   float* __restrict__ keys, float* __restrict__ boxes) {
@@ -757,7 +973,10 @@ void launch_rpn_proposals(const float* cls, const float* box, long img_stride_cl
     LUMI_CUDA_CHECK(cudaMemset2DAsync(ws.keys + p.na, (size_t)ws.cap * sizeof(float), 0xFF,
                                       (size_t)(ws.cap - p.na) * sizeof(float), nimg, st));   // 0xFFFFFFFF = NaN -> invalid
   }
-  run_sort(ws.keys, nimg, ws.cap, p.na, nullptr, p.pre_nms_top_n, ws.order, ws.nvalid, ws.sort_tmp, st);
+  if (ws.cut_hist && (long)p.na >= RPN_CUT_RATIO * (long)p.pre_nms_top_n)
+    run_topk_cut(ws.keys, nimg, ws.cap, p.na, p.pre_nms_top_n, ws.order, ws.nvalid, ws, st);
+  else
+    run_sort(ws.keys, nimg, ws.cap, p.na, nullptr, p.pre_nms_top_n, ws.order, ws.nvalid, ws.sort_tmp, st);
   LUMI_REQUIRE(p.pre_nms_top_n <= ws.ncap || p.na <= ws.ncap, "rpn_proposals: NMS workspace smaller than pre_nms_top_n");
   dim3 g2(cdiv(ws.ncap, 256), nimg);
   gather_sorted_kernel<<<g2, 256, 0, st>>>(ws.boxes, ws.keys, ws.order, ws.nvalid, ws.cap, ws.ncap, ws.sboxes,
