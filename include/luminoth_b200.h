@@ -148,7 +148,9 @@ const char* lumi_op_last_error(void);      /* message of the last failed lumi_op
  * (whole-tile schedule), 2 wgmma with the stream-K schedule forced; 3-11 write the fp16x2 split planes the engine
  * passes between layers: 3 two consumer warpgroups, 4 / 5 four warpgroups on short-K layers (5: + stream-K),
  * 6 / 7 2-CTA clusters multicasting the weight tile (7: + stream-K), 8 / 9 halo-patch kernels on 3x3 stride-1 layers
- * (9: + stream-K), 10 / 11 halo patches on 2-CTA clusters (11: + stream-K). */
+ * (9: + stream-K), 10 / 11 halo patches on 2-CTA clusters (11: + stream-K), 12 as 3 with the register epilogue, 13 the
+ * SIMT kernel writing split planes (what the engine stores under conv_impl = simt).  Returns LUMI_EOVERFLOW when a
+ * split output (codes 3-13) exceeds the split range, |x| > 65504. */
 int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout,
                    int stride, int rate, int padding, const float* scale, const float* bias,
                    const float* residual, int act, int impl, float* y, int* ho, int* wo, void* stream);
@@ -156,12 +158,32 @@ int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wg
 /* lumi_op_conv2d with the pre-activation output of a pre-activation ResNet unit, as the engine fuses it into the conv
  * epilogue: p = relu(fmaf(x^, pre_scale[c], pre_bias[c])) where x^ is the output x as stored in its fp16x2 split
  * planes.  pre_scale / pre_bias [cout] on DEVICE.  y (x) and p are NHWC fp32 read back from the split planes; y may be
- * NULL to write p only; y and p both NULL is a shape query.  impl: 0 SIMT, or one of the split-output codes 3-7, 12
- * (12: as 3 with the register epilogue).  Returns LUMI_EOVERFLOW when x or p exceeds the split range. */
+ * NULL to write p only; y and p both NULL is a shape query.  impl: 0 or 13 SIMT, or one of the split-output codes 3-7,
+ * 12 (12: as 3 with the register epilogue).  Returns LUMI_EOVERFLOW when x or p exceeds the split range. */
 int lumi_op_conv2d_preact(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout,
                           int stride, int rate, int padding, const float* scale, const float* bias,
                           const float* residual, int act, int impl, const float* pre_scale, const float* pre_bias,
                           float* y, float* p, int* ho, int* wo, void* stream);
+
+/* The conv launch with every output and residual option the engine uses.  The arguments of lumi_op_conv2d, plus:
+ *   residual  NHWC fp32 [n,res_h,res_w,cout] on DEVICE or NULL, read at (oy*res_stride, ox*res_stride): res_stride 2
+ *             with the input's resolution is slim's `subsample` shortcut of a bottleneck unit; res_stride 1 with
+ *             res_h = ho, res_w = wo is lumi_op_conv2d's residual.
+ *   pre_scale, pre_bias  NULL (no pre-activation output; y is required) or the pre-activation of
+ *             lumi_op_conv2d_preact (p required, y may be NULL to write p only).
+ * impl: the codes of lumi_op_conv2d; with a pre-activation output those of lumi_op_conv2d_preact.  y and p both NULL
+ * is a shape query.  Returns LUMI_EOVERFLOW when a split output exceeds the split range. */
+int lumi_op_conv2d_io(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout,
+                      int stride, int rate, int padding, const float* scale, const float* bias, const float* residual,
+                      int res_h, int res_w, int res_stride, int act, int impl, const float* pre_scale,
+                      const float* pre_bias, float* y, float* p, int* ho, int* wo, void* stream);
+
+/* The tensor-core weight packing of a conv layer, on HOST pointers and without any CUDA call.  w: TF layout
+ * [kdim = kh*kw*cin][cout] fp32; scale [cout] or NULL (1).  Writes hi, lo: [cout][kdim] fp16 bit patterns of the split
+ * of w[:, c] * 2^e[c], and scale_tc [cout] = scale[c] * 2^-e[c] rounded once to fp32.  e[c] puts max|w[:, c]| in
+ * [2^13, 2^14), clamped to [-126, 126]; an all-zero column gets e = 0 (DESIGN section 2). */
+int lumi_pack_conv_weights(const float* w, int kdim, int cout, const float* scale, uint16_t* hi, uint16_t* lo,
+                           float* scale_tc);
 
 /* tf.image.resize_images(BILINEAR) of TF 1.x (legacy kernel, align_corners=False) on one HWC image with 3 channels,
  * utils/image.py:94-97,139-142.  src: DEVICE uint8 (src_is_f32 = 0) or float32 (1) [h0,w0,3]; dst DEVICE float32 [h,w,3]. */

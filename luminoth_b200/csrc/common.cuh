@@ -50,6 +50,10 @@ enum ActKind { ACT_NONE = 0, ACT_RELU = 1, ACT_RELU6 = 2 };
 
 #define LUMI_F16_MAX 65504.0f
 
+// The split range, one test for every conv epilogue (SIMT, register, slot, pre-activation): a value leaves it iff
+// !(|v| <= 65504), NaN included.  Testing the rounded hi plane for inf instead would let (65504, 65520) through.
+__device__ __forceinline__ bool split_overflows(float v) { return !(fabsf(v) <= LUMI_F16_MAX); }
+
 __device__ __forceinline__ void split_f32(float x, __half& hi, __half& lo) {
   hi = __float2half_rn(x);
   lo = __float2half_rn(x - __half2float(hi));

@@ -20,6 +20,7 @@
 // snt.Conv2D (models/fasterrcnn/rpn.py:69-90, models/ssd/ssd.py:83-96,
 // models/ssd/feature_extractor.py:28-37) and snt.Linear (models/fasterrcnn/rcnn.py:74-98).
 #include "conv.cuh"
+#include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -170,7 +171,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const SimtArgs a) {
       if (a.out_f32) {
         a.out_f32[obase + c] = v;
       } else {
-        if (!(fabsf(v) <= LUMI_F16_MAX) && a.overflow) atomicOr(a.overflow, 1);
+        if (split_overflows(v) && a.overflow) atomicOr(a.overflow, 1);
         __half hi, lo;
         split_f32(v, hi, lo);
         if (!PRE || a.out_hi) {
@@ -179,7 +180,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const SimtArgs a) {
         }
         if constexpr (PRE) {
           const float p = fmaxf(fmaf(join_f16(hi, lo), a.pre_scale[c], a.pre_bias[c]), 0.f);
-          if (!(p <= LUMI_F16_MAX) && a.overflow) atomicOr(a.overflow, 1);
+          if (split_overflows(p) && a.overflow) atomicOr(a.overflow, 1);
           split_f32(p, hi, lo);
           a.pre_hi[obase + c] = hi;
           a.pre_lo[obase + c] = lo;
@@ -353,15 +354,14 @@ __device__ __forceinline__ void tc_slice_mma(float (&d)[WN / 2], const TcSlice& 
 }
 
 // The pre-activation output of a column pair, in place: (h2, l2) holding x as split become p = relu(fmaf(x^, s, b)) as
-// split.  Returns whether p overflows the fp16 hi plane.
+// split.  Returns whether p leaves the split range.
 __device__ __forceinline__ bool tc_preact(__half2& h2, __half2& l2, const float* s, const float* b, int c0) {
   const float2 sc = __ldg(reinterpret_cast<const float2*>(s + c0));
   const float2 bi = __ldg(reinterpret_cast<const float2*>(b + c0));
   const float p0 = fmaxf(fmaf(__low2float(h2) + __low2float(l2), sc.x, bi.x), 0.f);
   const float p1 = fmaxf(fmaf(__high2float(h2) + __high2float(l2), sc.y, bi.y), 0.f);
   split2_f32(p0, p1, h2, l2);
-  const uint32_t ab = *reinterpret_cast<const uint32_t*>(&h2);
-  return ((ab & 0x7C00u) == 0x7C00u) || ((ab & 0x7C000000u) == 0x7C000000u);
+  return split_overflows(p0) || split_overflows(p1);
 }
 
 // Persistent: grid = min(#tiles, #SMs) (or #SMs for stream-K); every CTA (or CTA pair) walks its schedule.  One
@@ -715,9 +715,8 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
               v1 = apply_act(v1, a.act);
               __half2 h2, l2;
               split2_f32(v0, v1, h2, l2);
-              const uint32_t ab = *reinterpret_cast<const uint32_t*>(&h2);
-              ovf |= row_ok[hrow] && c0 < a.cout &&
-                     (((ab & 0x7C00u) == 0x7C00u) || ((ab & 0x7C000000u) == 0x7C000000u));
+              // bitwise, not short-circuit: a branch per column pair would cost the epilogue its straight-line code
+              ovf |= row_ok[hrow] & (c0 < a.cout) & (split_overflows(v0) | split_overflows(v1));
               if (p_only) ovf |= row_ok[hrow] && c0 < a.cout && tc_preact(h2, l2, a.pre_scale, a.pre_bias, c0);
               *ph = h2;                                 // in place: each thread rewrites only what it read
               *pl = l2;
@@ -819,11 +818,10 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
                 if (c0 + 1 < a.cout) op[1] = v1;
               }
             } else {                     // split outputs always have cout % 32 == 0
-              // packed split: hi = rn16(v), lo = rn16(v - hi); an fp16 overflow shows up as inf/nan in the hi plane
+              // packed split: hi = rn16(v), lo = rn16(v - hi)
               __half2 h2, l2;
               split2_f32(v0, v1, h2, l2);
-              const uint32_t ab = *reinterpret_cast<const uint32_t*>(&h2);
-              ovf |= ((ab & 0x7C00u) == 0x7C00u) || ((ab & 0x7C000000u) == 0x7C000000u);
+              ovf |= split_overflows(v0) || split_overflows(v1);
               if (!PRE || a.out_hi) {
                 *reinterpret_cast<__half2*>(a.out_hi + opix * a.cout + c0) = h2;
                 *reinterpret_cast<__half2*>(a.out_lo + opix * a.cout + c0) = l2;
@@ -1177,6 +1175,31 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
 }
 
 // ---------------------------------------------------------------- host: weight packing
+void pack_conv_weights(const float* w, size_t kdim, int cout, const float* scale, __half* hi, __half* lo,
+                       float* scale_tc) {
+  for (int c = 0; c < cout; ++c) {
+    float mx = 0.f;
+    for (size_t k = 0; k < kdim; ++k) mx = std::fmax(mx, std::fabs(w[k * cout + c]));
+    int e = 0;
+    if (mx > 0.f && std::isfinite(mx)) {
+      int ex;
+      std::frexp(mx, &ex);            // mx = f * 2^ex, f in [0.5,1)
+      e = 14 - ex;                    // mx * 2^e in [2^13, 2^14)
+      e = std::min(std::max(e, -CONV_PACK_EXP_MAX), CONV_PACK_EXP_MAX);
+    }
+    const float up = std::ldexp(1.f, e);
+    for (size_t k = 0; k < kdim; ++k) {
+      float v = w[k * cout + c] * up;
+      __half h = __float2half_rn(v);
+      __half l = __float2half_rn(v - __half2float(h));
+      hi[(size_t)c * kdim + k] = h;
+      lo[(size_t)c * kdim + k] = l;
+    }
+    // exact in double; one rounding to fp32 (a subnormal scale_tc only for a clamped column and |scale| < 1)
+    scale_tc[c] = (float)((scale ? (double)scale[c] : 1.0) * std::ldexp(1.0, -e));
+  }
+}
+
 void conv_layer_upload(ConvLayer& L, const float* w, const float* scale, const float* bias) {
   const size_t kdim = (size_t)L.kh * L.kw * L.cin;
   const size_t nw = kdim * L.cout;
@@ -1192,32 +1215,14 @@ void conv_layer_upload(ConvLayer& L, const float* w, const float* scale, const f
   LUMI_CUDA_CHECK(cudaMemcpy(L.bias, bi.data(), cpad * sizeof(float), cudaMemcpyHostToDevice));
   L.tc_ready = false;
   if (L.cin % 64 == 0 && (L.stride == 1 || L.stride == 2)) {
-    // [cout_pad][kdim] fp16 hi/lo of w * 2^e[c]; e[c] puts max|w[:,c]| in [2^13, 2^14)
+    // [cout_pad][kdim] fp16 hi/lo of w * 2^e[c], zero rows for the padding channels
     L.cout_pad = cdiv(L.cout, 64) * 64;
     if (L.cout_pad > 64 && L.cout_pad % 128 != 0) L.cout_pad = cdiv(L.cout, 128) * 128;
     std::vector<__half> hi((size_t)L.cout_pad * kdim), lo((size_t)L.cout_pad * kdim);
     std::vector<float> sct(L.cout_pad, 0.f);
     std::memset(hi.data(), 0, hi.size() * sizeof(__half));
     std::memset(lo.data(), 0, lo.size() * sizeof(__half));
-    for (int c = 0; c < L.cout; ++c) {
-      float mx = 0.f;
-      for (size_t k = 0; k < kdim; ++k) mx = std::fmax(mx, std::fabs(w[k * L.cout + c]));
-      int e = 0;
-      if (mx > 0.f && std::isfinite(mx)) {
-        int ex;
-        std::frexp(mx, &ex);          // mx = f * 2^ex, f in [0.5,1)
-        e = 14 - ex;                  // mx * 2^e in [2^13, 2^14)
-      }
-      const float up = std::ldexp(1.f, e), down = std::ldexp(1.f, -e);
-      for (size_t k = 0; k < kdim; ++k) {
-        float v = w[k * L.cout + c] * up;
-        __half h = __float2half_rn(v);
-        __half l = __float2half_rn(v - __half2float(h));
-        hi[(size_t)c * kdim + k] = h;
-        lo[(size_t)c * kdim + k] = l;
-      }
-      sct[c] = sc[c] * down;
-    }
+    pack_conv_weights(w, kdim, L.cout, sc.data(), hi.data(), lo.data(), sct.data());
     LUMI_CUDA_CHECK(cudaMalloc(&L.w_hi, hi.size() * sizeof(__half)));
     LUMI_CUDA_CHECK(cudaMalloc(&L.w_lo, lo.size() * sizeof(__half)));
     LUMI_CUDA_CHECK(cudaMemcpy(L.w_hi, hi.data(), hi.size() * sizeof(__half), cudaMemcpyHostToDevice));

@@ -68,6 +68,16 @@ struct ConvIO {
   long in_pix_pitch = 0, in_row_pitch = 0, in_img_pitch = 0;
 };
 
+// Tensor-core weight packing, host only (no CUDA calls).  w: TF layout [kdim][cout] on host.  For every output channel
+// c < cout: rows c of hi / lo ([cout][kdim] fp16) hold the split of w[:, c] * 2^e[c], and scale_tc[c] = scale[c] * 2^-e[c]
+// (scale == nullptr: 1), computed in double and rounded once.  e[c] puts max|w[:, c]| in [2^13, 2^14) so the lo plane
+// stays in fp16's normal range; it is clamped to [-126, 126] so 2^e and 2^-e are normal fp32.  A clamped column
+// (0 < max|w[:, c]| < 2^-112) packs to small or subnormal fp16; its whole contribution is below 2^-112 * |s| * sum|x|.
+// An all-zero (or non-finite) column gets e = 0.
+constexpr int CONV_PACK_EXP_MAX = 126;
+void pack_conv_weights(const float* w, size_t kdim, int cout, const float* scale, __half* hi, __half* lo,
+                       float* scale_tc);
+
 // host-side packing (w: TF layout on host)
 void conv_layer_upload(ConvLayer& L, const float* w_host, const float* scale_host, const float* bias_host);
 void conv_layer_free(ConvLayer& L);

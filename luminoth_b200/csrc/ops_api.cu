@@ -33,13 +33,15 @@ struct ActBuf {
 
 int op_fail(const Error& e) { g_op_error = e.what(); return e.code; }
 
-// The arguments of lumi_op_conv2d, plus the pre-activation output of lumi_op_conv2d_preact (pre_scale == nullptr:
+// The arguments of lumi_op_conv2d_io: those of lumi_op_conv2d, the residual's own resolution and sampling stride
+// (res_h <= 0: the output's, stride 1) and the pre-activation output of lumi_op_conv2d_preact (pre_scale == nullptr:
 // none; then y is required, else y == nullptr writes p only).
 int op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout, int stride,
-              int rate, int padding, const float* scale, const float* bias, const float* residual, int act, int impl,
-              const float* pre_scale, const float* pre_bias, float* y, float* p, int* ho_out, int* wo_out,
-              cudaStream_t st) {
+              int rate, int padding, const float* scale, const float* bias, const float* residual, int res_h,
+              int res_w, int res_stride, int act, int impl, const float* pre_scale, const float* pre_bias, float* y,
+              float* p, int* ho_out, int* wo_out, cudaStream_t st) {
   const bool preact = pre_scale != nullptr;
+  LUMI_REQUIRE(impl >= 0 && impl <= 13, "conv2d: impl must be one of 0-13");
   ConvLayer L;
   L.kh = kh; L.kw = kw; L.cin = cin; L.cout = cout; L.stride = stride; L.rate = rate; L.act = act;
   const size_t nw = (size_t)kh * kw * cin * cout;
@@ -64,92 +66,78 @@ int op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, in
   if (wo_out) *wo_out = wo;
   if (!y && !p) return LUMI_OK;           // shape query
   LUMI_REQUIRE(preact ? (p && pre_bias) : (y && !p), "conv2d: bad output arguments");
+  // 0: SIMT, fp32 outputs; 1 whole tiles, 2 stream-K forced (fp32 outputs written by the epilogue);
+  // 3 / 4 / 5: the engine's inter-layer form -- fp16x2 split planes -- with two consumer warpgroups (3), the
+  // four-warpgroup short-K kernel allowed (4), and 4 + stream-K (5), all through the shared-memory slot epilogue;
+  // 6 / 7: the 2-CTA cluster kernel wherever it applies (7: + stream-K); 8-11: the halo-patch kernels (10, 11 on
+  // cluster pairs; 9, 11: + stream-K); 12: as 3 with the register epilogue; 13: SIMT writing split planes (the engine's
+  // conv_impl = simt).  A pre-activation output is written in split planes only: SIMT (0 or 13), 3-7 or 12.
+  const bool simt = impl == 0 || impl == 13;
+  const bool split = preact || impl >= 3;
+  if (preact)
+    LUMI_REQUIRE(simt || (impl >= 3 && impl <= 7) || impl == 12,
+                 "conv2d_preact: impl must be 0 or 13 (SIMT) or one of the split-output codes 3-7, 12");
+  if (split) LUMI_REQUIRE(cout % 32 == 0, "conv2d: split outputs need cout % 32 == 0");
   ActBuf in(n, h, w, cin);
   launch_f32_to_act(x, in.a, st);
   ConvIO io;
   io.in = in.a; io.pad_t = pt; io.pad_l = pl; io.ho = ho; io.wo = wo; io.out_f32 = y;
   std::unique_ptr<ActBuf> res;
   if (residual) {
-    res.reset(new ActBuf(n, ho, wo, cout));
+    if (res_h <= 0) { res_h = ho; res_w = wo; res_stride = 1; }
+    LUMI_REQUIRE((res_stride == 1 || res_stride == 2) && (ho - 1) * res_stride < res_h &&
+                     (wo - 1) * res_stride < res_w,
+                 "conv2d: the residual (sampling stride 1 or 2) must cover every output pixel");
+    res.reset(new ActBuf(n, res_h, res_w, cout));
     launch_f32_to_act(residual, res->a, st);
-    io.res = res->a; io.res_stride = 1;
+    io.res = res->a; io.res_stride = res_stride;
+  }
+  // split planes: x (when y is given) and p, each read back as fp32; the pre-activation vectors padded like the layer's
+  std::unique_ptr<ActBuf> xo, po;
+  std::unique_ptr<DevBuf> ps, pb;
+  DevBuf ovf(sizeof(int));
+  LUMI_CUDA_CHECK(cudaMemset(ovf.p, 0, sizeof(int)));
+  if (split) {
+    io.out_f32 = nullptr;
+    io.overflow_flag = ovf.as<int>();
+    if (y) { xo.reset(new ActBuf(n, ho, wo, cout)); io.out = xo->a; }
   }
   if (preact) {
-    // split planes only: x (when y is given) and p, each read back as fp32; the vectors padded like the layer's
-    LUMI_REQUIRE(impl == 0 || (impl >= 3 && impl <= 7) || impl == 12,
-                 "conv2d_preact: impl must be 0 (SIMT) or one of the split-output codes 3-7, 12");
-    LUMI_REQUIRE(cout % 32 == 0, "conv2d_preact: split outputs need cout % 32 == 0");
     const int cpad = cdiv(cout, 128) * 128;
     std::vector<float> hv(cpad, 0.f);
-    DevBuf ps(cpad * sizeof(float)), pb(cpad * sizeof(float)), ovf(sizeof(int));
+    ps.reset(new DevBuf(cpad * sizeof(float)));
+    pb.reset(new DevBuf(cpad * sizeof(float)));
     LUMI_CUDA_CHECK(cudaMemcpy(hv.data(), pre_scale, cout * sizeof(float), cudaMemcpyDeviceToHost));
-    LUMI_CUDA_CHECK(cudaMemcpy(ps.p, hv.data(), cpad * sizeof(float), cudaMemcpyHostToDevice));
+    LUMI_CUDA_CHECK(cudaMemcpy(ps->p, hv.data(), cpad * sizeof(float), cudaMemcpyHostToDevice));
     LUMI_CUDA_CHECK(cudaMemcpy(hv.data(), pre_bias, cout * sizeof(float), cudaMemcpyDeviceToHost));
-    LUMI_CUDA_CHECK(cudaMemcpy(pb.p, hv.data(), cpad * sizeof(float), cudaMemcpyHostToDevice));
-    LUMI_CUDA_CHECK(cudaMemset(ovf.p, 0, sizeof(int)));
-    std::unique_ptr<ActBuf> xo;
-    if (y) { xo.reset(new ActBuf(n, ho, wo, cout)); io.out = xo->a; }
-    ActBuf po(n, ho, wo, cout);
-    io.out_f32 = nullptr;
-    io.pre = po.a; io.pre_scale = ps.as<float>(); io.pre_bias = pb.as<float>();
-    io.overflow_flag = ovf.as<int>();
-    ConvWorkspace sk;
-    struct SkGuard { ConvWorkspace& w; ~SkGuard() { conv_workspace_free(w); } } skg{sk};
-    if (impl == 0) {
-      launch_conv_simt(L, io, st);
-    } else {
-      io.epi_tma = impl == 12 ? 0 : 1;
-      io.epi16 = (impl == 4 || impl == 5) ? 8 : 0;
-      io.cta2 = (impl == 6 || impl == 7) ? 1 : 0;
-      LUMI_REQUIRE(conv_tc_supported(L, io), "conv2d: this layer shape is not handled by the tensor-core kernel");
-      if (impl == 5 || impl == 7) {
-        conv_workspace_create(sk);
-        io.sk = &sk;
-        io.streamk = 2;
-      }
-      launch_conv_tc(L, io, st);
-    }
-    if (xo) launch_act_to_f32(xo->a, y, st);
-    launch_act_to_f32(po.a, p, st);
-    int flag = 0;
-    LUMI_CUDA_CHECK(cudaMemcpyAsync(&flag, ovf.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
-    if (flag) throw Error(LUMI_EOVERFLOW, "conv2d_preact: an output exceeded the fp16x2 split range (|x| > 65504)");
-    return LUMI_OK;
+    LUMI_CUDA_CHECK(cudaMemcpy(pb->p, hv.data(), cpad * sizeof(float), cudaMemcpyHostToDevice));
+    po.reset(new ActBuf(n, ho, wo, cout));
+    io.pre = po->a; io.pre_scale = ps->as<float>(); io.pre_bias = pb->as<float>();
   }
-  if (impl >= 1 && impl <= 12) {
-    // 1 whole tiles, 2 stream-K forced (fp32 outputs written by the epilogue);
-    // 3 / 4 / 5: the engine's inter-layer form -- fp16x2 split planes -- with two consumer warpgroups (3), the
-    // four-warpgroup short-K kernel allowed (4), and 4 + stream-K (5), all through the shared-memory slot epilogue;
-    // 6 / 7: the 2-CTA cluster kernel wherever it applies (7: + stream-K); 8-11: the halo-patch kernels (10, 11 on
-    // cluster pairs; 9, 11: + stream-K); 12: as 3 with the register epilogue
-    std::unique_ptr<ActBuf> split_out;
-    if (impl >= 3) {
-      LUMI_REQUIRE(cout % 32 == 0, "conv2d: split outputs need cout % 32 == 0");
-      split_out.reset(new ActBuf(n, ho, wo, cout));
-      io.out = split_out->a;
-      io.out_f32 = nullptr;
-      io.epi_tma = impl == 12 ? 0 : 1;
-      io.epi16 = (impl == 4 || impl == 5) ? 8 : 0;
-      io.cta2 = (impl == 6 || impl == 7 || impl == 10 || impl == 11) ? 1 : 0;
-      io.halo = (impl >= 8 && impl <= 11) ? 1 : 0;
-      io.halo_tiles_pct = 1000000;                  // test hook: whenever the shape allows
-    }
+  ConvWorkspace sk;
+  struct SkGuard { ConvWorkspace& w; ~SkGuard() { conv_workspace_free(w); } } skg{sk};
+  if (simt) {
+    launch_conv_simt(L, io, st);
+  } else {
+    io.epi_tma = impl == 12 ? 0 : 1;
+    io.epi16 = (impl == 4 || impl == 5) ? 8 : 0;
+    io.cta2 = (impl == 6 || impl == 7 || impl == 10 || impl == 11) ? 1 : 0;
+    io.halo = (impl >= 8 && impl <= 11) ? 1 : 0;
+    io.halo_tiles_pct = 1000000;                    // test hook: whenever the shape allows
     LUMI_REQUIRE(conv_tc_supported(L, io), "conv2d: this layer shape is not handled by the tensor-core kernel");
-    ConvWorkspace sk;
-    struct SkGuard { ConvWorkspace& w; ~SkGuard() { conv_workspace_free(w); } } skg{sk};
     if (impl == 2 || impl == 5 || impl == 7 || impl == 9 || impl == 11) {
       conv_workspace_create(sk);
       io.sk = &sk;
       io.streamk = 2;
     }
     launch_conv_tc(L, io, st);
-    if (split_out) launch_act_to_f32(split_out->a, y, st);
-    LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
-  } else {
-    launch_conv_simt(L, io, st);
   }
+  if (xo) launch_act_to_f32(xo->a, y, st);
+  if (po) launch_act_to_f32(po->a, p, st);
+  int flag = 0;
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(&flag, ovf.p, sizeof(int), cudaMemcpyDeviceToHost, st));
   LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
+  if (flag) throw Error(LUMI_EOVERFLOW, "conv2d: an output exceeded the fp16x2 split range (|x| > 65504)");
   return LUMI_OK;
 }
 }  // namespace
@@ -168,8 +156,8 @@ int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wg
                    int rate, int padding, const float* scale, const float* bias, const float* residual, int act,
                    int impl, float* y, int* ho_out, int* wo_out, void* stream) {
   OP_BEGIN
-  return op_conv2d(x, n, h, w, cin, wgt, kh, kw, cout, stride, rate, padding, scale, bias, residual, act, impl, nullptr,
-                   nullptr, y, nullptr, ho_out, wo_out, static_cast<cudaStream_t>(stream));
+  return op_conv2d(x, n, h, w, cin, wgt, kh, kw, cout, stride, rate, padding, scale, bias, residual, 0, 0, 1, act, impl,
+                   nullptr, nullptr, y, nullptr, ho_out, wo_out, static_cast<cudaStream_t>(stream));
   OP_END
 }
 
@@ -179,8 +167,31 @@ int lumi_op_conv2d_preact(const float* x, int n, int h, int w, int cin, const fl
                           float* y, float* p, int* ho_out, int* wo_out, void* stream) {
   OP_BEGIN
   LUMI_REQUIRE(pre_scale && pre_bias, "conv2d_preact: pre_scale and pre_bias are required");
-  return op_conv2d(x, n, h, w, cin, wgt, kh, kw, cout, stride, rate, padding, scale, bias, residual, act, impl,
+  return op_conv2d(x, n, h, w, cin, wgt, kh, kw, cout, stride, rate, padding, scale, bias, residual, 0, 0, 1, act, impl,
                    pre_scale, pre_bias, y, p, ho_out, wo_out, static_cast<cudaStream_t>(stream));
+  OP_END
+}
+
+int lumi_op_conv2d_io(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout,
+                      int stride, int rate, int padding, const float* scale, const float* bias, const float* residual,
+                      int res_h, int res_w, int res_stride, int act, int impl, const float* pre_scale,
+                      const float* pre_bias, float* y, float* p, int* ho_out, int* wo_out, void* stream) {
+  OP_BEGIN
+  LUMI_REQUIRE(!residual || res_h > 0, "conv2d_io: res_h and res_w are required with a residual");
+  LUMI_REQUIRE(!pre_scale == !pre_bias, "conv2d_io: pre_scale and pre_bias go together");
+  return op_conv2d(x, n, h, w, cin, wgt, kh, kw, cout, stride, rate, padding, scale, bias, residual, res_h, res_w,
+                   res_stride, act, impl, pre_scale, pre_bias, y, p, ho_out, wo_out, static_cast<cudaStream_t>(stream));
+  OP_END
+}
+
+int lumi_pack_conv_weights(const float* w, int kdim, int cout, const float* scale, uint16_t* hi, uint16_t* lo,
+                           float* scale_tc) {
+  OP_BEGIN
+  LUMI_REQUIRE(w && hi && lo && scale_tc && kdim > 0 && cout > 0, "pack_conv_weights: bad arguments");
+  static_assert(sizeof(__half) == sizeof(uint16_t), "fp16 bits");
+  pack_conv_weights(w, (size_t)kdim, cout, scale, reinterpret_cast<__half*>(hi), reinterpret_cast<__half*>(lo),
+                    scale_tc);
+  return LUMI_OK;
   OP_END
 }
 

@@ -71,6 +71,10 @@ SIGNATURES = {
     'lumi_op_conv2d_preact': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] +
                               [ctypes.c_int] * 6 + [ctypes.c_void_p] * 3 + [ctypes.c_int] * 2 +
                               [ctypes.c_void_p] * 4 + [_c_int_p, _c_int_p, ctypes.c_void_p]),
+    'lumi_op_conv2d_io': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] +
+                          [ctypes.c_int] * 6 + [ctypes.c_void_p] * 3 + [ctypes.c_int] * 5 +
+                          [ctypes.c_void_p] * 4 + [_c_int_p, _c_int_p, ctypes.c_void_p]),
+    'lumi_pack_conv_weights': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 4),
     'lumi_op_max_pool': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 7 + [ctypes.c_void_p, ctypes.c_void_p]),
     'lumi_op_max_pool_preact': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 7 + [ctypes.c_void_p] * 4),
     'lumi_op_roi_pool': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p, ctypes.c_void_p,
