@@ -210,6 +210,43 @@ int lumi_op_sort_desc(const float* scores, int n, int32_t* idx_out, void* stream
 int lumi_op_nms_sorted(const float* boxes_sorted, int n, float iou_threshold, int max_out,
                        int32_t* keep, int32_t* num_keep, void* stream);
 
+/* Which NMS path `problems` lists of up to ncap sorted candidates take at this IoU threshold: 0 the one-phase staged
+ * scan, 1 the two-phase NMS (>= 3 lists of >= 4096 candidates, 0 < thr < inf, or env LUMI_NMS_LAZY=1; =0 turns it
+ * off), 2 the one-phase unstaged scan (lists too long for the staged scan's shared memory).  Host only. */
+int lumi_nms_path(int problems, int ncap, float iou_threshold);
+
+/* lumi_op_nms_sorted on `problems` lists at once, through the engine's batched NMS: boxes_sorted [problems,cap,4],
+ * nvalid [problems] int32 (each in [0, cap]), all on DEVICE.  keep [problems,max_out] int32 (entries past
+ * num_keep[p] undefined), num_keep [problems].  The path is lumi_nms_path(problems, cap, iou_threshold). */
+int lumi_op_nms_batched(const float* boxes_sorted, const int32_t* nvalid, int problems, int cap, float iou_threshold,
+                        int max_out, int32_t* keep, int32_t* num_keep, void* stream);
+
+/* The RPN proposal chain as the engine runs it on a (half-)batch: cls / box hold nimg images at the given per-image
+ * strides (floats), each [na / A cells][channels]; anchor a of a cell reads its two class values at
+ * cell * cls_stride + cls_off + 2a (logits = 1: softmax logits, 0: probabilities, foreground second) and its deltas at
+ * cell * box_stride + box_off + 4a.  anchors [na,4] shared by the images.  The workspace holds cap >= na candidates
+ * per image (the engine sizes it for its largest image) and min(cap, pre_nms_top_n) after the top-n cut.  Outputs
+ * proposals [nimg,post_nms_top_n,4], scores [nimg,post_nms_top_n], counts [nimg] on DEVICE. */
+int lumi_op_rpn_proposals_batched(const float* cls, const float* box, int64_t img_stride_cls, int64_t img_stride_box,
+                                  int A, const float* anchors, int nimg, int na, int cap, float im_h, float im_w,
+                                  int pre_nms_top_n, int post_nms_top_n, float nms_threshold, float min_prob,
+                                  int filter_outside, int clip_after_nms, int apply_nms, int logits, int cls_stride,
+                                  int cls_off, int box_stride, int box_off, float* proposals, float* scores,
+                                  int32_t* counts, void* stream);
+
+/* The per-class detection chain as the engine runs it on nimg images: boxes_in [nimg][r][4] at boxes_img_stride
+ * floats per image (0: one set of anchors shared by all images), row_counts [nimg] valid rows per image or NULL (all
+ * r), cls_prob rows of prob_stride floats and deltas rows of delta_stride floats ([nimg * r] rows each; deltas hold 4
+ * values per class, or 4 shared ones when shared_deltas = 1).  Outputs objects [nimg,total_max,4], labels, probs
+ * [nimg,total_max], count [nimg] and, when records is not NULL, the packed rows of lumi_set_record_output
+ * [nimg][1 + 6 * total_max], all on DEVICE. */
+int lumi_op_class_detections_batched(const float* boxes_in, int64_t boxes_img_stride, const int32_t* row_counts,
+                                     const float* deltas, const float* cls_prob, int nimg, int r, int nc, float im_h,
+                                     float im_w, float var0, float var1, float min_prob, float nms_threshold,
+                                     int class_max, int total_max, int shared_deltas, int prob_stride,
+                                     int delta_stride, float* objects, int32_t* labels, float* probs, int32_t* count,
+                                     float* records, void* stream);
+
 /* RPN proposal chain (rpn_proposal.py:41-197) for one image: cls_prob [na,2], bbox_pred [na,4],
  * anchors [na,4] float; outputs proposals [post_nms_top_n,4], scores, count (device). */
 int lumi_op_rpn_proposals(const float* cls_prob, const float* bbox_pred, const float* anchors, int na,

@@ -56,6 +56,11 @@ struct NmsWorkspace {
 };
 void nms_workspace_alloc(NmsWorkspace& ws, int problems, int cap, int max_out, int ncap = 0);
 void nms_workspace_free(NmsWorkspace& ws);
+// The NMS path of `problems` lists of up to ncap candidates at IoU threshold thr (host only, honours LUMI_NMS_LAZY):
+// staged one-phase scan, two-phase (see postproc.cu), or the unstaged scan when the staged one's shared memory would
+// exceed 200 KiB.
+enum { NMS_PATH_STAGED = 0, NMS_PATH_TWO_PHASE = 1, NMS_PATH_UNSTAGED = 2 };
+int nms_path(int problems, int ncap, float thr);
 
 struct RpnParams {
   int na;                 // anchors per image
@@ -92,5 +97,8 @@ void launch_pack_records(const float* boxes, const float* scores, const int* lab
 void launch_sort_desc(const float* scores, int n, int* idx_out, NmsWorkspace& ws, cudaStream_t st);
 void launch_nms_sorted(const float* boxes_sorted, int n, float thr, int max_out, NmsWorkspace& ws, int* keep,
                        int* nkeep, cudaStream_t st);
+// boxes_sorted [problems][ws.cap][4], nvalid [problems] (device); keep [problems][max_out], nkeep [problems]
+void launch_nms_batched(const float* boxes_sorted, const int* nvalid, int problems, float thr, int max_out,
+                        NmsWorkspace& ws, int* keep, int* nkeep, cudaStream_t st);
 
 }  // namespace lumi

@@ -278,6 +278,76 @@ int lumi_op_nms_sorted(const float* boxes_sorted, int n, float iou_threshold, in
   OP_END
 }
 
+int lumi_nms_path(int problems, int ncap, float iou_threshold) { return nms_path(problems, ncap, iou_threshold); }
+
+int lumi_op_nms_batched(const float* boxes_sorted, const int32_t* nvalid, int problems, int cap, float iou_threshold,
+                        int max_out, int32_t* keep, int32_t* num_keep, void* stream) {
+  OP_BEGIN
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  LUMI_REQUIRE(problems > 0 && cap > 0 && max_out > 0, "nms_batched: problems, cap and max_out must be positive");
+  std::vector<int> hn(problems);
+  LUMI_CUDA_CHECK(cudaMemcpy(hn.data(), nvalid, problems * sizeof(int), cudaMemcpyDeviceToHost));
+  for (int v : hn) LUMI_REQUIRE(v >= 0 && v <= cap, "nms_batched: nvalid must lie in [0, cap]");
+  NmsWorkspace ws;
+  struct G { NmsWorkspace& w; ~G() { nms_workspace_free(w); } } g{ws};
+  nms_workspace_alloc(ws, problems, cap, max_out);
+  launch_nms_batched(boxes_sorted, nvalid, problems, iou_threshold, max_out, ws, keep, num_keep, st);
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
+  return LUMI_OK;
+  OP_END
+}
+
+int lumi_op_rpn_proposals_batched(const float* cls, const float* box, int64_t img_stride_cls, int64_t img_stride_box,
+                                  int A, const float* anchors, int nimg, int na, int cap, float im_h, float im_w,
+                                  int pre_nms_top_n, int post_nms_top_n, float nms_threshold, float min_prob,
+                                  int filter_outside, int clip_after_nms, int apply_nms, int logits, int cls_stride,
+                                  int cls_off, int box_stride, int box_off, float* proposals, float* scores,
+                                  int32_t* counts, void* stream) {
+  OP_BEGIN
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  LUMI_REQUIRE(nimg > 0 && A > 0 && na > 0 && na % A == 0 && cap >= na && pre_nms_top_n > 0 && post_nms_top_n > 0,
+               "rpn_proposals_batched: need positive sizes, na a multiple of A and cap >= na");
+  NmsWorkspace ws;
+  struct G { NmsWorkspace& w; ~G() { nms_workspace_free(w); } } g{ws};
+  nms_workspace_alloc(ws, nimg, cap, post_nms_top_n, std::min(cap, pre_nms_top_n));   // as the engine sizes ws_rpn
+  RpnParams p{};
+  p.na = na; p.im_h = im_h; p.im_w = im_w; p.pre_nms_top_n = pre_nms_top_n; p.post_nms_top_n = post_nms_top_n;
+  p.nms_threshold = nms_threshold; p.min_prob = min_prob; p.filter_outside = filter_outside;
+  p.clip_after_nms = clip_after_nms; p.apply_nms = apply_nms; p.logits = logits;
+  p.cls_stride = cls_stride; p.cls_off = cls_off; p.box_stride = box_stride; p.box_off = box_off;
+  launch_rpn_proposals(cls, box, (long)img_stride_cls, (long)img_stride_box, A, anchors, nimg, p, ws, proposals, scores,
+                       counts, st);
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
+  return LUMI_OK;
+  OP_END
+}
+
+int lumi_op_class_detections_batched(const float* boxes_in, int64_t boxes_img_stride, const int32_t* row_counts,
+                                     const float* deltas, const float* cls_prob, int nimg, int r, int nc, float im_h,
+                                     float im_w, float var0, float var1, float min_prob, float nms_threshold,
+                                     int class_max, int total_max, int shared_deltas, int prob_stride,
+                                     int delta_stride, float* objects, int32_t* labels, float* probs, int32_t* count,
+                                     float* records, void* stream) {
+  OP_BEGIN
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  LUMI_REQUIRE(nimg > 0 && r > 0 && nc > 0 && class_max > 0 && total_max > 0 && boxes_img_stride >= 0 &&
+                   prob_stride >= nc + 1 && delta_stride >= (shared_deltas ? 4 : 4 * nc),
+               "class_detections_batched: bad sizes or strides");
+  NmsWorkspace ws;
+  struct G { NmsWorkspace& w; ~G() { nms_workspace_free(w); } } g{ws};
+  nms_workspace_alloc(ws, nimg * nc, r, class_max);
+  DevBuf fk(det_final_scratch_bytes(nimg, nc, class_max));
+  DetParams p{};
+  p.r = r; p.nc = nc; p.im_h = im_h; p.im_w = im_w; p.var0 = var0; p.var1 = var1; p.min_prob = min_prob;
+  p.nms_threshold = nms_threshold; p.class_max = class_max; p.total_max = total_max;
+  p.shared_deltas = shared_deltas ? 1 : 0; p.prob_stride = prob_stride; p.delta_stride = delta_stride;
+  launch_class_detections(boxes_in, (long)boxes_img_stride, row_counts, deltas, cls_prob, nimg, p, ws, fk.as<float>(),
+                          objects, labels, probs, count, st, records);
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
+  return LUMI_OK;
+  OP_END
+}
+
 int lumi_op_rpn_proposals(const float* cls_prob, const float* bbox_pred, const float* anchors, int na, float im_h,
                           float im_w, int pre_nms_top_n, int post_nms_top_n, float nms_threshold, float min_prob,
                           int filter_outside, int clip_after_nms, float* proposals, float* scores, int32_t* count,

@@ -70,10 +70,13 @@ __device__ __forceinline__ bool iou_gt(float4 a, float4 b, float thr) {
 // ------------------------------------------------------------------ workspace
 constexpr int CUT_THREADS = 256, CUT_ITEMS = 16, CUT_CHUNK = CUT_THREADS * CUT_ITEMS;   // candidates per cut CTA
 
+// u64 words per mask row; even: mask rows stay 16 B aligned for cp.async.bulk
+static int nms_words(int ncap) { return (cdiv(ncap, 64) + 1) & ~1; }
+
 void nms_workspace_alloc(NmsWorkspace& ws, int problems, int cap, int max_out, int ncap) {
   if (ncap <= 0 || ncap > cap) ncap = cap;
   ws.problems = problems; ws.cap = cap; ws.max_out = max_out; ws.ncap = ncap;
-  ws.words = (cdiv(ncap, 64) + 1) & ~1;     // even: mask rows stay 16 B aligned for cp.async.bulk
+  ws.words = nms_words(ncap);
   size_t pc = (size_t)problems * cap;
   size_t pn = (size_t)problems * ncap;
   LUMI_CUDA_CHECK(cudaMalloc(&ws.keys, pc * sizeof(float)));
@@ -762,6 +765,19 @@ __global__ void __launch_bounds__(256) nms_scan_staged_kernel(const unsigned lon
 constexpr int NMS_LAZY_R1 = 2048;
 constexpr int NMS_LAZY_MIN = 4096;
 
+// shared memory of nms_scan_staged_kernel: the removed words plus two chunks of 64 mask rows
+static size_t staged_scan_smem(int words) { return ((size_t)words + 2 * 64 * (size_t)words) * sizeof(unsigned long long); }
+constexpr size_t NMS_STAGED_SMEM_MAX = 200 * 1024;
+
+int nms_path(int problems, int ncap, float thr) {
+  if (staged_scan_smem(nms_words(ncap)) > NMS_STAGED_SMEM_MAX) return NMS_PATH_UNSTAGED;
+  // two-phase when the mask kernel is a full-GPU kernel (several long lists at once): it shortens the step at
+  // batch 8, but its longer kernel chain adds latency when one or two images are in flight.  LUMI_NMS_LAZY=0 / 1 forces it off / on.
+  static const int lazy_env = [] { const char* e = getenv("LUMI_NMS_LAZY"); return e ? (atoi(e) != 0 ? 1 : 0) : -1; }();
+  const bool lazy_ok = ncap >= NMS_LAZY_MIN && thr > 0.f && thr < INFINITY;
+  return lazy_ok && (lazy_env == 1 || (lazy_env < 0 && problems >= 3)) ? NMS_PATH_TWO_PHASE : NMS_PATH_STAGED;
+}
+
 __global__ void __launch_bounds__(256) nms_prefilter_kernel(const float* __restrict__ sboxes,
                                                             const int* __restrict__ nvalid, int cap, float thr,
                                                             const int* __restrict__ keep, const int* __restrict__ nkeep,
@@ -829,13 +845,13 @@ __global__ void __launch_bounds__(1024) nms_compact_kernel(const float* __restri
 
 static void launch_scan_staged(NmsWorkspace& ws, const unsigned long long* mask, const int* nvalid, int problems,
                                int max_out, int limit, const int* base_count, const int* index_map, cudaStream_t st) {
-  const size_t staged_smem = ((size_t)ws.words + 2 * 64 * (size_t)ws.words) * sizeof(unsigned long long);
+  const size_t staged_smem = staged_scan_smem(ws.words);
   static bool attr[64] = {false};        // cudaFuncSetAttribute is per device
   int dev = 0;
   LUMI_CUDA_CHECK(cudaGetDevice(&dev));
   if (dev < 0 || dev >= 64 || !__atomic_load_n(&attr[dev], __ATOMIC_ACQUIRE)) {
     LUMI_CUDA_CHECK(cudaFuncSetAttribute(nms_scan_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         200 * 1024));
+                                         (int)NMS_STAGED_SMEM_MAX));
     if (dev >= 0 && dev < 64) __atomic_store_n(&attr[dev], true, __ATOMIC_RELEASE);
   }
   nms_scan_staged_kernel<<<problems, 256, staged_smem, st>>>(mask, nvalid, ws.ncap, ws.words, max_out, ws.keep, ws.nkeep,
@@ -861,14 +877,9 @@ static dim3 mask_grid(const NmsWorkspace& ws, int problems, int n_max) {
 
 static void run_nms(NmsWorkspace& ws, int problems, float thr, int max_out, cudaStream_t st) {
   if (!problems) return;
-  const size_t staged_smem = ((size_t)ws.words + 2 * 64 * (size_t)ws.words) * sizeof(unsigned long long);
-  const bool staged = staged_smem <= 200 * 1024;
-  // two-phase when the mask kernel is a full-GPU kernel (several long lists at once): it shortens the step at
-  // batch 8, but its longer kernel chain adds latency when one or two images are in flight.  LUMI_NMS_LAZY=0 / 1 forces it off / on.
-  static const int lazy_env = [] { const char* e = getenv("LUMI_NMS_LAZY"); return e ? (atoi(e) != 0 ? 1 : 0) : -1; }();
-  const bool lazy_ok = staged && ws.sboxes2 && ws.ncap >= NMS_LAZY_MIN && thr > 0.f && thr < INFINITY;
-  const bool lazy = lazy_ok && (lazy_env == 1 || (lazy_env < 0 && problems >= 3));
-  if (lazy) {
+  const int path = nms_path(problems, ws.ncap, thr);
+  if (path == NMS_PATH_TWO_PHASE) {
+    LUMI_REQUIRE(ws.sboxes2 != nullptr, "nms: missing two-phase scratch");
     const int R1 = NMS_LAZY_R1;
     nms_mask_kernel<<<mask_grid(ws, problems, R1), 64, 0, st>>>(ws.sboxes, ws.nvalid, ws.ncap, ws.words, thr, ws.mask, R1);
     count_launch();
@@ -893,7 +904,7 @@ static void run_nms(NmsWorkspace& ws, int problems, float thr, int max_out, cuda
                                                                   0x7fffffff);
   count_launch();
   LUMI_CUDA_CHECK(cudaGetLastError());
-  if (staged) {
+  if (path == NMS_PATH_STAGED) {
     launch_scan_staged(ws, ws.mask, ws.nvalid, problems, max_out, 0x7fffffff, nullptr, nullptr, st);
   } else {
     size_t smem = (size_t)ws.words * sizeof(unsigned long long);
@@ -1142,6 +1153,19 @@ void launch_sort_desc(const float* scores, int n, int* idx_out, NmsWorkspace& ws
   LUMI_CUDA_CHECK(cudaMemcpyAsync(ws.keys, scores, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
   run_sort(ws.keys, 1, ws.cap, n, nullptr, ws.cap, ws.order, ws.nvalid, ws.sort_tmp, st);
   LUMI_CUDA_CHECK(cudaMemcpyAsync(idx_out, ws.order, (size_t)n * sizeof(int), cudaMemcpyDeviceToDevice, st));
+}
+
+void launch_nms_batched(const float* boxes_sorted, const int* nvalid, int problems, float thr, int max_out,
+                        NmsWorkspace& ws, int* keep, int* nkeep, cudaStream_t st) {
+  LUMI_REQUIRE(problems <= ws.problems && ws.ncap == ws.cap && max_out <= ws.max_out, "nms_batched: workspace too small");
+  if (!problems) return;
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(ws.sboxes, boxes_sorted, (size_t)problems * ws.cap * 4 * sizeof(float),
+                                  cudaMemcpyDeviceToDevice, st));
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(ws.nvalid, nvalid, (size_t)problems * sizeof(int), cudaMemcpyDeviceToDevice, st));
+  run_nms(ws, problems, thr, max_out, st);
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(keep, ws.keep, (size_t)problems * max_out * sizeof(int), cudaMemcpyDeviceToDevice,
+                                  st));                  // run_nms writes keep rows of max_out entries
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(nkeep, ws.nkeep, (size_t)problems * sizeof(int), cudaMemcpyDeviceToDevice, st));
 }
 
 __global__ void set_int_kernel(int* p, int v) { *p = v; }

@@ -85,6 +85,16 @@ SIGNATURES = {
     'lumi_op_sort_desc': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     'lumi_op_nms_sorted': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_int, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p]),
+    'lumi_nms_path': (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_float]),
+    'lumi_op_nms_batched': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_float,
+                                           ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    'lumi_op_rpn_proposals_batched': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64,
+                                                     ctypes.c_int, ctypes.c_void_p] + [ctypes.c_int] * 3 +
+                                      [ctypes.c_float] * 2 + [ctypes.c_int] * 2 + [ctypes.c_float] * 2 +
+                                      [ctypes.c_int] * 8 + [ctypes.c_void_p] * 4),
+    'lumi_op_class_detections_batched': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64] + [ctypes.c_void_p] * 3 +
+                                         [ctypes.c_int] * 3 + [ctypes.c_float] * 6 + [ctypes.c_int] * 5 +
+                                         [ctypes.c_void_p] * 6),
     'lumi_op_rpn_proposals': (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int, ctypes.c_float, ctypes.c_float,
                                                                      ctypes.c_int, ctypes.c_int, ctypes.c_float,
                                                                      ctypes.c_float, ctypes.c_int, ctypes.c_int] +

@@ -90,6 +90,64 @@ def nms_sorted(boxes, thr, max_out):
     return keep.cpu().numpy()[:k]
 
 
+def nms_path(problems, ncap, thr):
+    return _lib().lumi_nms_path(problems, ncap, float(thr))
+
+
+def nms_batched(boxes, nvalid, thr, max_out):
+    """boxes [P, cap, 4] sorted lists, nvalid [P] -> list of P keep-index arrays."""
+    lib = _lib()
+    P, cap, _ = boxes.shape
+    bd, nd = _dev(boxes, np.float32), _dev(np.asarray(nvalid), np.int32)
+    keep = torch.full((P, max_out), -1, dtype=torch.int32, device='cuda')
+    nk = torch.zeros((P,), dtype=torch.int32, device='cuda')
+    _check(lib.lumi_op_nms_batched(_p(bd), _p(nd), P, cap, float(thr), max_out, _p(keep), _p(nk), None))
+    keep, nk = keep.cpu().numpy(), nk.cpu().numpy()
+    return [keep[p, :nk[p]] for p in range(P)]
+
+
+def rpn_proposals_batched(heads, A, anchors, na, cap, im_shape, cfg, logits=True, cls_off=0, box_off=None):
+    """heads [nimg, cells, hc]: the engine's fused head, class pair of anchor a at cls_off + 2a, deltas at
+    box_off + 4a (default 2A).  Returns (proposals [nimg, post, 4], scores [nimg, post], counts [nimg])."""
+    lib = _lib()
+    nimg, cells, hc = heads.shape
+    assert cells * A == na
+    post = int(cfg['post_nms_top_n'])
+    hd, ad = _dev(heads, np.float32), _dev(anchors, np.float32)
+    props = torch.zeros((nimg, post, 4), dtype=torch.float32, device='cuda')
+    scores = torch.zeros((nimg, post), dtype=torch.float32, device='cuda')
+    cnt = torch.zeros((nimg,), dtype=torch.int32, device='cuda')
+    _check(lib.lumi_op_rpn_proposals_batched(
+        _p(hd), _p(hd), cells * hc, cells * hc, A, _p(ad), nimg, na, cap, float(im_shape[0]), float(im_shape[1]),
+        int(cfg['pre_nms_top_n']), post, float(cfg['nms_threshold']), float(cfg.get('min_prob_threshold', 0.0)),
+        int(bool(cfg.get('filter_outside_anchors', False))), int(bool(cfg.get('clip_after_nms', False))),
+        int(bool(cfg.get('apply_nms', True))), int(logits), hc, cls_off, hc, 2 * A if box_off is None else box_off,
+        _p(props), _p(scores), _p(cnt), None))
+    return props.cpu().numpy(), scores.cpu().numpy(), cnt.cpu().numpy()
+
+
+def class_detections_batched(boxes_in, boxes_img_stride, row_counts, deltas, delta_stride, cls_prob, nimg, r, nc,
+                             im_shape, cfg, variances, shared_deltas, records=False):
+    """boxes_in / deltas / cls_prob: flat float32 arrays in the engine's layouts (see lumi_op_class_detections_batched).
+    Returns (objects [nimg, tm, 4], labels, probs [nimg, tm], counts [nimg], records [nimg, 1 + 6 tm] or None)."""
+    lib = _lib()
+    tm, cm = int(cfg['total_max_detections']), int(cfg['class_max_detections'])
+    bd, dd, pd = _dev(boxes_in, np.float32), _dev(deltas, np.float32), _dev(cls_prob, np.float32)
+    rc = _dev(np.asarray(row_counts), np.int32) if row_counts is not None else None
+    obj = torch.zeros((nimg, tm, 4), dtype=torch.float32, device='cuda')
+    lab = torch.zeros((nimg, tm), dtype=torch.int32, device='cuda')
+    prob = torch.zeros((nimg, tm), dtype=torch.float32, device='cuda')
+    cnt = torch.zeros((nimg,), dtype=torch.int32, device='cuda')
+    rec = torch.full((nimg, 1 + 6 * tm), np.nan, dtype=torch.float32, device='cuda') if records else None
+    v = variances or [1., 1.]
+    _check(lib.lumi_op_class_detections_batched(
+        _p(bd), boxes_img_stride, _p(rc), _p(dd), _p(pd), nimg, r, nc, float(im_shape[0]), float(im_shape[1]),
+        float(v[0]), float(v[1]), float(cfg.get('min_prob_threshold') or 0.0), float(cfg['class_nms_threshold']), cm, tm,
+        int(shared_deltas), nc + 1, delta_stride, _p(obj), _p(lab), _p(prob), _p(cnt), _p(rec), None))
+    return (obj.cpu().numpy(), lab.cpu().numpy(), prob.cpu().numpy(), cnt.cpu().numpy(),
+            rec.cpu().numpy() if records else None)
+
+
 def rpn_proposals(cls_prob, bbox_pred, anchors, im_shape, cfg):
     lib = _lib()
     na = cls_prob.shape[0]
