@@ -197,10 +197,36 @@ int lumi_op_max_pool(const float* x, int n, int h, int w, int c, int k, int stri
 int lumi_op_max_pool_preact(const float* x, int n, int h, int w, int c, int k, int stride, int padding,
                             const float* pre_scale, const float* pre_bias, float* y, void* stream);
 
-/* ROI crop (2ph x 2pw bilinear) + 2x2 max pool: roi_pool.py:68-95.
- * rois [r,4] (x1,y1,x2,y2) px of image 0..; roi_batch [r] image index; y [r,ph,pw,c]. */
+/* ROI crop + 2x2 max pool: roi_pool.py:68-95.  Like the reference, the crop is 2pw rows x 2ph columns (quirk Q4), so
+ * y is [r,pw,ph,c].  rois [r,4] (x1,y1,x2,y2) px, all pooled from image 0 of fmap; roi_batch is not read (it must be
+ * NULL when n > 1).  C a multiple of 8, ph, pw >= 1, 2 * (ph + pw) <= 64. */
 int lumi_op_roi_pool(const float* fmap, int n, int fh, int fw, int c, const float* rois, const int32_t* roi_batch,
                      int r, float im_h, float im_w, int ph, int pw, float* y, void* stream);
+
+/* The ROI kernel instance lumi_op_roi_pool / the engine launch for c channels at a ph x pw pooled size: 0-2 the
+ * row-walk kernel at 6 / 5 / 4 resident CTAs per SM, 3-4 the column-walk kernel at 4 / 8 channels per lane, 5-8 the
+ * cell kernel <channels per lane, rois per CTA, warps> = <8,4,4>, <8,4,8>, <8,1,8>, <4,1,8>; -1 when no instance
+ * takes the shape.  Honours LUMI_ROI_KERNEL, _MINB, _COLS_CPL, _CPL, _RB and _NW (each read once per process).  Host
+ * only. */
+int lumi_roi_kernel(int c, int ph, int pw);
+
+/* The ROI stage as the engine runs it on n images: fmap [n,fh,fw,c] fp32, rois [n,rmax,4] (x1,y1,x2,y2) px, counts [n]
+ * valid rois per image or NULL (all rmax), all on DEVICE.  kernel: -1 for lumi_roi_kernel(c, ph, pw), else a code of
+ * lumi_roi_kernel (LUMI_EINVAL when its shape preconditions fail).  Outputs, each NULL or DEVICE: pooled
+ * [n*rmax,pw,ph,c] and mean [n*rmax,c], the fused tf.reduce_mean over the pooled cells; at least one is required.
+ * Rows r >= counts[img] come out 0.  Both are written through the engine's fp16x2 split planes, which start out as
+ * NaN, so an element the kernel skips reads back as NaN. */
+int lumi_op_roi_pool_batched(const float* fmap, int n, int fh, int fw, int c, const float* rois, const int32_t* counts,
+                             int rmax, float im_h, float im_w, int ph, int pw, int kernel, float* pooled, float* mean,
+                             void* stream);
+
+/* tf.reduce_mean(x, [1, 2]) through split planes, as the engine's RCNN head runs it after the resnet_v1_101 tail and
+ * for pooled features that did not fuse the mean: x [r,h,w,c] fp32 on DEVICE (split into planes first), y [r,c]. */
+int lumi_op_spatial_mean(const float* x, int r, int h, int w, int c, float* y, void* stream);
+
+/* Softmax over the first cols entries of each of rows rows of x (in_stride floats apart, >= cols); y [rows,cols]
+ * dense.  The engine reads the C + 1 class logits out of fc rows 5C + 1 wide.  DEVICE pointers. */
+int lumi_op_softmax_rows(const float* x, int rows, int cols, int in_stride, float* y, void* stream);
 
 /* Sort scores descending (ties: lower index first); idx_out [n] int32. */
 int lumi_op_sort_desc(const float* scores, int n, int32_t* idx_out, void* stream);

@@ -336,6 +336,11 @@ void parse_config(lumi_engine* e) {
       if (mode != "crop") throw Error(LUMI_EINVAL, "Pooling mode " + mode + " is not implemented (roi_pool.py:97-102)");
       e->pooled_w = (int)c.number("model.rcnn.roi.pooled_width", 7);
       e->pooled_h = (int)c.number("model.rcnn.roi.pooled_height", 7);
+      // the ROI kernels keep the 2 * (pooled_width + pooled_height) crop sample coordinates of a roi in 64 slots
+      if (e->pooled_w < 1 || e->pooled_h < 1 || 2 * (e->pooled_w + e->pooled_h) > 64)
+        throw Error(LUMI_EINVAL, "model.rcnn.roi.pooled_width and pooled_height must be >= 1 with 2 * (pooled_width + "
+                                 "pooled_height) <= 64, got " + std::to_string(e->pooled_w) + " x " +
+                                 std::to_string(e->pooled_h));
       LUMI_REQUIRE(c.str("model.rcnn.roi.padding", "VALID") == "VALID", "roi.padding must be VALID");
       DetParams& d = e->det;
       d.nc = e->num_classes;

@@ -23,9 +23,20 @@ void launch_frcnn_anchors(const int* ref /*A x 4*/, int A, int fh, int fw, int s
 // ---- ROI crop + 2x2 max pool (roi.cu) : roi_pool.py:68-95
 // rois [nimg][rmax][4] (x1,y1,x2,y2 px), counts [nimg] (nullptr -> all rmax valid); out (nimg*rmax, pw, ph, C)
 // and/or mean (nimg*rmax, 1, 1, C) = tf.reduce_mean over the pooled cells (either may be an empty Act).
-// fmap_f32: fp32 NHWC copy of the feature map (n, fh, fw, c).
+// fmap_f32: fp32 NHWC copy of the feature map (n, fh, fw, c).  kernel: one of the ROI_* instance codes below, or -1
+// for roi_kernel(c, ph, pw); a code whose shape preconditions fail throws LUMI_EINVAL.
 void launch_roi_pool(const float* fmap_f32, int n, int fh, int fw, int c, const float* rois, const int* counts, int rmax,
-                     float im_h, float im_w, int ph, int pw, Act out, Act mean, cudaStream_t st);
+                     float im_h, float im_w, int ph, int pw, Act out, Act mean, cudaStream_t st, int kernel = -1);
+// Every kernel instance launch_roi_pool can start: the row-walk kernel at 6 / 5 / 4 resident CTAs per SM, the
+// column-walk kernel at 4 / 8 channels per lane, and the round-1 cell kernel roi_pool_kernel<CPL, RB, NW>.
+enum {
+  ROI_ROWS_MINB6 = 0, ROI_ROWS_MINB5 = 1, ROI_ROWS_MINB4 = 2, ROI_COLS_CPL4 = 3, ROI_COLS_CPL8 = 4,
+  ROI_CELLS_8_4_4 = 5, ROI_CELLS_8_4_8 = 6, ROI_CELLS_8_1_8 = 7, ROI_CELLS_4_1_8 = 8, ROI_KERNEL_COUNT = 9
+};
+// The instance launch_roi_pool picks for C channels and a ph x pw pooled size (host only; honours LUMI_ROI_KERNEL,
+// LUMI_ROI_MINB, LUMI_ROI_COLS_CPL, LUMI_ROI_CPL, LUMI_ROI_RB and LUMI_ROI_NW, each read once per process), or -1
+// when no instance takes the shape (C not a multiple of 8, a pooled side below 1, or 2 * (ph + pw) > 64).
+int roi_kernel(int c, int ph, int pw);
 
 // ---- proposal / detection chains (postproc.cu)
 struct NmsWorkspace {

@@ -244,8 +244,66 @@ int lumi_op_roi_pool(const float* fmap, int n, int fh, int fw, int c, const floa
   LUMI_REQUIRE(n == 1 || roi_batch == nullptr, "roi_pool op: single image (roi_batch must be NULL or n == 1)");
   (void)roi_batch;
   ActBuf out(r, pw, ph, c);
-  launch_roi_pool(fmap, n, fh, fw, c, rois, nullptr, r, im_h, im_w, ph, pw, out.a, Act(), st);
+  // every roi is pooled from image 0 (the launcher reads n * r rows: n images of r rois each)
+  launch_roi_pool(fmap, 1, fh, fw, c, rois, nullptr, r, im_h, im_w, ph, pw, out.a, Act(), st);
   launch_act_to_f32(out.a, y, st);
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
+  return LUMI_OK;
+  OP_END
+}
+
+int lumi_roi_kernel(int c, int ph, int pw) { return roi_kernel(c, ph, pw); }
+
+int lumi_op_roi_pool_batched(const float* fmap, int n, int fh, int fw, int c, const float* rois, const int32_t* counts,
+                             int rmax, float im_h, float im_w, int ph, int pw, int kernel, float* pooled, float* mean,
+                             void* stream) {
+  OP_BEGIN
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  LUMI_REQUIRE(n > 0 && fh > 0 && fw > 0 && c > 0 && rmax > 0, "roi_pool_batched: sizes must be positive");
+  LUMI_REQUIRE(pooled || mean, "roi_pool_batched: pooled or mean is required");
+  LUMI_REQUIRE(ph >= 1 && pw >= 1, "roi_pool_batched: pooled size must be >= 1");
+  const int rows = n * rmax;
+  // both split planes start as 0xFFFF (an fp16 NaN): a cell or row the kernel skips reads back as NaN
+  std::unique_ptr<ActBuf> out, m;
+  if (pooled) {
+    out.reset(new ActBuf(rows, pw, ph, c));
+    LUMI_CUDA_CHECK(cudaMemsetAsync(out->a.hi, 0xFF, out->a.numel() * sizeof(__half), st));
+    LUMI_CUDA_CHECK(cudaMemsetAsync(out->a.lo, 0xFF, out->a.numel() * sizeof(__half), st));
+  }
+  if (mean) {
+    m.reset(new ActBuf(rows, 1, 1, c));
+    LUMI_CUDA_CHECK(cudaMemsetAsync(m->a.hi, 0xFF, m->a.numel() * sizeof(__half), st));
+    LUMI_CUDA_CHECK(cudaMemsetAsync(m->a.lo, 0xFF, m->a.numel() * sizeof(__half), st));
+  }
+  launch_roi_pool(fmap, n, fh, fw, c, rois, counts, rmax, im_h, im_w, ph, pw, out ? out->a : Act(), m ? m->a : Act(),
+                  st, kernel);
+  if (out) launch_act_to_f32(out->a, pooled, st);
+  if (m) launch_act_to_f32(m->a, mean, st);
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
+  return LUMI_OK;
+  OP_END
+}
+
+int lumi_op_spatial_mean(const float* x, int r, int h, int w, int c, float* y, void* stream) {
+  OP_BEGIN
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  LUMI_REQUIRE(r > 0 && h > 0 && w > 0 && c > 0, "spatial_mean: sizes must be positive");
+  ActBuf in(r, h, w, c), out(r, 1, 1, c);
+  launch_f32_to_act(x, in.a, st);
+  LUMI_CUDA_CHECK(cudaMemsetAsync(out.a.hi, 0xFF, out.a.numel() * sizeof(__half), st));
+  LUMI_CUDA_CHECK(cudaMemsetAsync(out.a.lo, 0xFF, out.a.numel() * sizeof(__half), st));
+  launch_spatial_mean(in.a, out.a, st);
+  launch_act_to_f32(out.a, y, st);
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
+  return LUMI_OK;
+  OP_END
+}
+
+int lumi_op_softmax_rows(const float* x, int rows, int cols, int in_stride, float* y, void* stream) {
+  OP_BEGIN
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  LUMI_REQUIRE(rows > 0 && cols > 0 && in_stride >= cols, "softmax_rows: need rows, cols > 0 and in_stride >= cols");
+  launch_softmax_rows(x, y, rows, cols, in_stride, st);
   LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
   return LUMI_OK;
   OP_END

@@ -8,6 +8,7 @@
 // instruction / L1-bound (12.8 G bilinear taps per batch at R = 2000), not HBM-bound.
 #include "ops.cuh"
 #include <cstdlib>
+#include <string>
 
 namespace lumi {
 
@@ -629,10 +630,61 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) roi_pool_rows_kernel(const R
   }
 }
 
+// Shape preconditions of each instance (crop_h = 2*pw, crop_w = 2*ph, both even): the row-walk kernel keeps the
+// crop_h + crop_w sample tables in the lanes of one warp and a 2-bit plan per sample row in 32 bits; the column-walk
+// kernel keeps the tables in the lanes; the cell kernel keeps RB tables of up to 64 samples in shared memory and fills
+// them with one thread per sample.
+static bool roi_kernel_fits(int k, int c, int ph, int pw) {
+  if (c % 8 != 0 || ph < 1 || pw < 1 || 2 * (ph + pw) > 64) return false;
+  const int crop_h = 2 * pw, nsamp = 2 * (ph + pw);
+  switch (k) {
+    case ROI_ROWS_MINB6: case ROI_ROWS_MINB5: case ROI_ROWS_MINB4: return crop_h <= 16 && nsamp <= 32;
+    case ROI_COLS_CPL4: case ROI_COLS_CPL8: return nsamp <= 32;
+    case ROI_CELLS_8_4_4: return 4 * nsamp <= 128;
+    case ROI_CELLS_8_4_8: return 4 * nsamp <= 256;
+    case ROI_CELLS_8_1_8: case ROI_CELLS_4_1_8: return true;
+    default: return false;
+  }
+}
+
+int roi_kernel(int c, int ph, int pw) {
+  if (!roi_kernel_fits(ROI_CELLS_8_1_8, c, ph, pw)) return -1;
+  // LUMI_ROI_KERNEL: "rows" (default, round-2 row-walk kernel) | "cols" (round-2 first design) | "cells" (round-1 kernel);
+  // the older ones are kept for A/B measurement
+  static const int variant = [] {
+    const char* e = getenv("LUMI_ROI_KERNEL");
+    if (e && e[0] == 'c' && e[1] == 'e') return 0;
+    if (e && e[0] == 'c' && e[1] == 'o') return 1;
+    return 2;
+  }();
+  // occupancy: 4 / 5 / 6 resident CTAs per SM (<= 128 / 102 / 80 registers) measured 1.308 / 1.269 / 1.241 ms per step: 6
+  static const int minb = [] { const char* e = getenv("LUMI_ROI_MINB"); const int v = e ? atoi(e) : 6; return (v == 4 || v == 5) ? v : 6; }();
+  if (variant == 2 && roi_kernel_fits(ROI_ROWS_MINB6, c, ph, pw))
+    return minb == 5 ? ROI_ROWS_MINB5 : minb == 4 ? ROI_ROWS_MINB4 : ROI_ROWS_MINB6;
+  static const int cols_cpl = [] { const char* e = getenv("LUMI_ROI_COLS_CPL"); return (e && atoi(e) == 8) ? 8 : 4; }();
+  if (variant == 1 && roi_kernel_fits(ROI_COLS_CPL4, c, ph, pw)) return cols_cpl == 8 ? ROI_COLS_CPL8 : ROI_COLS_CPL4;
+  static const int cpl = [] { const char* e = getenv("LUMI_ROI_CPL"); return (e && atoi(e) == 4) ? 4 : 8; }();
+  // (measured alternatives at R = 2000, batch 8: 4 channels/lane 3.1 ms, straight-line 16-tap loads
+  //  without sharing 3.0 ms, this kernel 2.7 ms)
+  static const int rb = [] { const char* e = getenv("LUMI_ROI_RB"); return (e && atoi(e) == 1) ? 1 : 4; }();
+  // 4 warps x 4 ROIs: 196 cells = 49 per warp, no tail at all (measured 2.49 vs 2.51 ms with 8 warps, 2.73 ms with
+  // one ROI per CTA)
+  static const int nw = [] { const char* e = getenv("LUMI_ROI_NW"); return (e && atoi(e) == 8) ? 8 : 4; }();
+  if (cpl == 4) return ROI_CELLS_4_1_8;  // 4 channels per lane: half the registers (measured slower: 3.1 vs 2.7 ms at R = 2000)
+  if (rb == 4 && nw == 4 && roi_kernel_fits(ROI_CELLS_8_4_4, c, ph, pw)) return ROI_CELLS_8_4_4;
+  if (rb == 4 && roi_kernel_fits(ROI_CELLS_8_4_8, c, ph, pw)) return ROI_CELLS_8_4_8;
+  return ROI_CELLS_8_1_8;
+}
+
 void launch_roi_pool(const float* fmap_f32, int n, int fh, int fw, int c, const float* rois, const int* counts, int rmax,
-                     float im_h, float im_w, int ph, int pw, Act out, Act mean, cudaStream_t st) {
+                     float im_h, float im_w, int ph, int pw, Act out, Act mean, cudaStream_t st, int kernel) {
   LUMI_REQUIRE(c % 8 == 0, "roi_pool: C must be a multiple of 8");
-  LUMI_REQUIRE(2 * (ph + pw) <= 64, "roi_pool: pooled size too large");
+  LUMI_REQUIRE(ph >= 1 && pw >= 1 && 2 * (ph + pw) <= 64, "roi_pool: pooled size must be >= 1 with 2 * (ph + pw) <= 64");
+  LUMI_REQUIRE(kernel >= -1 && kernel < ROI_KERNEL_COUNT, "roi_pool: kernel must be -1 or one of the codes 0-8");
+  const int k = kernel < 0 ? roi_kernel(c, ph, pw) : kernel;
+  LUMI_REQUIRE(roi_kernel_fits(k, c, ph, pw), "roi_pool: kernel " + std::to_string(k) + " does not take C = " +
+                                                  std::to_string(c) + " at " + std::to_string(ph) + " x " +
+                                                  std::to_string(pw));
   RoiArgs a;
   a.fmap = fmap_f32; a.n = n; a.fh = fh; a.fw = fw; a.c = c;
   a.rois = rois; a.counts = counts; a.rmax = rmax; a.im_h = im_h; a.im_w = im_w;
@@ -642,63 +694,45 @@ void launch_roi_pool(const float* fmap_f32, int n, int fh, int fw, int c, const 
   LUMI_REQUIRE(out.hi || mean.hi, "roi_pool: no output requested");
   long rows = (long)n * rmax;
   if (!rows) return;
-  // LUMI_ROI_KERNEL: "rows" (default, round-2 row-walk kernel) | "cols" (round-2 first design) | "cells" (round-1 kernel);
-  // the older ones are kept for A/B measurement
-  static const int variant = [] {
-    const char* e = getenv("LUMI_ROI_KERNEL");
-    if (e && e[0] == 'c' && e[1] == 'e') return 0;
-    if (e && e[0] == 'c' && e[1] == 'o') return 1;
-    return 2;
-  }();
-  if (variant == 2 && a.crop_h <= 16 && a.crop_h + a.crop_w <= 32 && (a.crop_h & 1) == 0 && (a.crop_w & 1) == 0 &&
-      c % 4 == 0) {
-    constexpr int W = 4;
-    dim3 grid((unsigned)rows, (unsigned)cdiv(c, 128 * W));
-    // occupancy: 4 / 5 / 6 resident CTAs per SM (<= 128 / 102 / 80 registers) measured 1.308 / 1.269 / 1.241 ms per step: 6
-    static const int minb = [] { const char* e = getenv("LUMI_ROI_MINB"); const int v = e ? atoi(e) : 6; return (v == 4 || v == 5) ? v : 6; }();
-    if (minb == 5) roi_pool_rows_kernel<W, 5><<<grid, 32 * W, 0, st>>>(a);
-    else if (minb == 4) roi_pool_rows_kernel<W, 4><<<grid, 32 * W, 0, st>>>(a);
-    else roi_pool_rows_kernel<W, 6><<<grid, 32 * W, 0, st>>>(a);
-    count_launch();
-    LUMI_CUDA_CHECK(cudaGetLastError());
-    return;
-  }
-  static const int cols_cpl = [] { const char* e = getenv("LUMI_ROI_COLS_CPL"); return (e && atoi(e) == 8) ? 8 : 4; }();
-  if (variant == 1 && a.crop_h + a.crop_w <= 32 && (a.crop_h & 1) == 0 && (a.crop_w & 1) == 0 && c % cols_cpl == 0) {
-    constexpr int W = 4;
-    if (cols_cpl == 8) {
+  constexpr int W = 4;
+  switch (k) {
+    case ROI_ROWS_MINB6: case ROI_ROWS_MINB5: case ROI_ROWS_MINB4: {
+      dim3 grid((unsigned)rows, (unsigned)cdiv(c, 128 * W));
+      if (k == ROI_ROWS_MINB5) roi_pool_rows_kernel<W, 5><<<grid, 32 * W, 0, st>>>(a);
+      else if (k == ROI_ROWS_MINB4) roi_pool_rows_kernel<W, 4><<<grid, 32 * W, 0, st>>>(a);
+      else roi_pool_rows_kernel<W, 6><<<grid, 32 * W, 0, st>>>(a);
+      break;
+    }
+    case ROI_COLS_CPL8: {
       dim3 grid((unsigned)rows, (unsigned)cdiv(c, 256 * W));
       roi_pool_cols_kernel<8, W><<<grid, 32 * W, 0, st>>>(a);
-    } else {
+      break;
+    }
+    case ROI_COLS_CPL4: {
       dim3 grid((unsigned)rows, (unsigned)cdiv(c, 128 * W));
       roi_pool_cols_kernel<4, W><<<grid, 32 * W, 0, st>>>(a);
+      break;
     }
-    count_launch();
-    LUMI_CUDA_CHECK(cudaGetLastError());
-    return;
-  }
-  static const int cpl = [] { const char* e = getenv("LUMI_ROI_CPL"); return (e && atoi(e) == 4) ? 4 : 8; }();
-  // (measured alternatives at R = 2000, batch 8: 4 channels/lane 3.1 ms, straight-line 16-tap loads
-  //  without sharing 3.0 ms, this kernel 2.7 ms)
-  static const int rb = [] { const char* e = getenv("LUMI_ROI_RB"); return (e && atoi(e) == 1) ? 1 : 4; }();
-  LUMI_REQUIRE(pw * 2 + ph * 2 <= 64, "roi_pool: pooled size too large");
-  // 4 warps x 4 ROIs: 196 cells = 49 per warp, no tail at all (measured 2.49 vs 2.51 ms with 8 warps, 2.73 ms with
-  // one ROI per CTA)
-  static const int nw = [] { const char* e = getenv("LUMI_ROI_NW"); return (e && atoi(e) == 8) ? 8 : 4; }();
-  if (cpl == 8) {
-    if (rb == 4 && nw == 4 && 4 * (a.crop_h + a.crop_w) <= 128) {
+    case ROI_CELLS_8_4_4: {
       dim3 grid((unsigned)cdiv64(rows, 4), (unsigned)cdiv(c, 256));
       roi_pool_kernel<8, 4, 4><<<grid, 128, 0, st>>>(a);
-    } else if (rb == 4 && 4 * (a.crop_h + a.crop_w) <= 256) {
+      break;
+    }
+    case ROI_CELLS_8_4_8: {
       dim3 grid((unsigned)cdiv64(rows, 4), (unsigned)cdiv(c, 256));
       roi_pool_kernel<8, 4, 8><<<grid, 256, 0, st>>>(a);
-    } else {
+      break;
+    }
+    case ROI_CELLS_8_1_8: {
       dim3 grid((unsigned)rows, (unsigned)cdiv(c, 256));
       roi_pool_kernel<8, 1, 8><<<grid, 256, 0, st>>>(a);
+      break;
     }
-  } else {                 // 4 channels per lane: half the registers (measured slower: 3.1 vs 2.7 ms at R = 2000)
-    dim3 grid((unsigned)rows, (unsigned)cdiv(c, 128));
-    roi_pool_kernel<4, 1, 8><<<grid, 256, 0, st>>>(a);
+    default: {
+      dim3 grid((unsigned)rows, (unsigned)cdiv(c, 128));
+      roi_pool_kernel<4, 1, 8><<<grid, 256, 0, st>>>(a);
+      break;
+    }
   }
   count_launch();
   LUMI_CUDA_CHECK(cudaGetLastError());

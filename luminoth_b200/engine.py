@@ -82,6 +82,12 @@ SIGNATURES = {
                                                                                 ctypes.c_float, ctypes.c_int,
                                                                                 ctypes.c_int, ctypes.c_void_p,
                                                                                 ctypes.c_void_p]),
+    'lumi_roi_kernel': (ctypes.c_int, [ctypes.c_int] * 3),
+    'lumi_op_roi_pool_batched': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] * 2 +
+                                 [ctypes.c_int, ctypes.c_float, ctypes.c_float] + [ctypes.c_int] * 3 +
+                                 [ctypes.c_void_p] * 3),
+    'lumi_op_spatial_mean': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] * 2),
+    'lumi_op_softmax_rows': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 2),
     'lumi_op_sort_desc': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     'lumi_op_nms_sorted': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_int, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p]),

@@ -72,6 +72,46 @@ def roi_pool(fmap, rois, im_shape, ph, pw):
     return y.cpu().numpy()
 
 
+def roi_kernel(c, ph, pw):
+    return _lib().lumi_roi_kernel(c, ph, pw)
+
+
+def roi_pool_batched(fmap, rois, counts, im_shape, ph, pw, kernel=-1, pooled=True, mean=True):
+    """fmap [n, fh, fw, c], rois [n, rmax, 4], counts [n] or None -> (pooled [n*rmax, pw, ph, c] or None,
+    mean [n*rmax, c] or None) as CUDA float32 tensors.  fmap / rois may be numpy arrays or CUDA tensors."""
+    lib = _lib()
+    n, fh, fw, c = fmap.shape
+    rmax = rois.shape[1]
+    fd = fmap if torch.is_tensor(fmap) else _dev(fmap, np.float32)
+    rd = rois if torch.is_tensor(rois) else _dev(rois, np.float32)
+    cd = _dev(np.asarray(counts), np.int32) if counts is not None else None
+    y = torch.empty((n * rmax, pw, ph, c), dtype=torch.float32, device='cuda') if pooled else None
+    m = torch.empty((n * rmax, c), dtype=torch.float32, device='cuda') if mean else None
+    _check(lib.lumi_op_roi_pool_batched(_p(fd), n, fh, fw, c, _p(rd), _p(cd), rmax, float(im_shape[0]),
+                                        float(im_shape[1]), ph, pw, kernel, _p(y), _p(m), None))
+    return y, m
+
+
+def spatial_mean(x):
+    """x [r, h, w, c] -> [r, c] through the split planes."""
+    lib = _lib()
+    r, h, w, c = x.shape
+    xd = _dev(x, np.float32)
+    y = torch.empty((r, c), dtype=torch.float32, device='cuda')
+    _check(lib.lumi_op_spatial_mean(_p(xd), r, h, w, c, _p(y), None))
+    return y.cpu().numpy()
+
+
+def softmax_rows(x, cols):
+    """x [rows, in_stride] -> softmax of the first cols entries of each row, [rows, cols]."""
+    lib = _lib()
+    rows, stride = x.shape
+    xd = _dev(x, np.float32)
+    y = torch.empty((rows, cols), dtype=torch.float32, device='cuda')
+    _check(lib.lumi_op_softmax_rows(_p(xd), rows, cols, stride, _p(y), None))
+    return y.cpu().numpy()
+
+
 def sort_desc(scores):
     lib = _lib()
     sd = _dev(scores, np.float32)
