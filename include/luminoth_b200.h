@@ -149,8 +149,9 @@ const char* lumi_op_last_error(void);      /* message of the last failed lumi_op
  * passes between layers: 3 two consumer warpgroups, 4 / 5 four warpgroups on short-K layers (5: + stream-K),
  * 6 / 7 2-CTA clusters multicasting the weight tile (7: + stream-K), 8 / 9 halo-patch kernels on 3x3 stride-1 layers
  * (9: + stream-K), 10 / 11 halo patches on 2-CTA clusters (11: + stream-K), 12 as 3 with the register epilogue, 13 the
- * SIMT kernel writing split planes (what the engine stores under conv_impl = simt).  Returns LUMI_EOVERFLOW when a
- * split output (codes 3-13) exceeds the split range, |x| > 65504. */
+ * SIMT kernel writing split planes (what the engine stores under conv_impl = simt), 14 / 15 as 3 on 128 x 256 tiles
+ * (15: + stream-K; C_out padded to a multiple of 256 only).  Returns LUMI_EOVERFLOW when a split output (codes 3-15)
+ * exceeds the split range, |x| > 65504. */
 int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout,
                    int stride, int rate, int padding, const float* scale, const float* bias,
                    const float* residual, int act, int impl, float* y, int* ho, int* wo, void* stream);

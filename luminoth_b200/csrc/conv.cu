@@ -13,8 +13,9 @@
 //    zero-filled by TMA, which IS the TF SAME zero padding.  Persistent CTAs
 //    (whole tiles or stream-K) of one producer and two or four consumer
 //    warpgroups, mbarrier operand ring; split-plane outputs leave through shared-memory
-//    epilogue slots (TMA residual prefetch, TMA stores).  Variants: 2-CTA clusters that
-//    multicast the weight tile, and halo-patch kernels for 3x3 layers.
+//    epilogue slots (TMA residual prefetch, TMA stores).  Variants: 128 x 256 tiles for the
+//    long-K layers with C_out >= 256, 2-CTA clusters that multicast the weight tile, and halo-patch kernels for 3x3
+//    layers.
 //
 // Replaces slim conv2d+batch_norm+relu (luminoth/models/base/base_network.py:143-151),
 // snt.Conv2D (models/fasterrcnn/rpn.py:69-90, models/ssd/ssd.py:83-96,
@@ -278,6 +279,7 @@ struct TcSched {
 };
 
 constexpr int TC_A_BYTES = 128 * 128;       // 128 pixel rows x 64 fp16 (one 128 B swizzle row each)
+constexpr int TC_BN_MAX = 256;              // widest N tile: sizes the stream-K partial-sum slots
 // HALO (3x3, stride 1, rate 1): the nine taps of a 64-channel slice read the SAME input pixels, shifted.  The HALO
 // kernels fetch the (th + 2) x (8 + 2)-pixel patch of the slice ONCE (one TMA box per patch row and plane, zero-filled
 // outside the image = SAME padding) and hand the tensor core nine shifted VIEWS of it: M tile = th rows x 8 pixels,
@@ -297,10 +299,12 @@ constexpr int TC_HALO_PLANE_BYTES = TC_HALO_ROWS * TC_HALO_PITCH;
 // SLOTS > 0: split-plane outputs leave through a ring of SLOTS epilogue slots (one 64-column group of the tile, hi and
 // lo plane, in the SWIZZLE_128B layout of a box {64 ch, tw, th, nb}): the producer prefetches the residual into the
 // slot, the consumers overwrite it with the result in place and one thread TMA-stores it.  0: register epilogue.
+// BN = 256 (wide tile): two consumer warpgroups of 64 rows x 256 columns, slot epilogue; see conv_tc_kernel.
 template <int BN, int STAGES, int NCWG = 2, bool PAIR = false, bool HALO = false, int SLOTS = 0>
 struct TcCfg {
   static_assert(NCWG == 2 || NCWG == 4, "two or four consumer warpgroups");
   static_assert(!PAIR || BN == 128, "the cluster pair exists for BN = 128");
+  static_assert(BN != 256 || (NCWG == 2 && !HALO && SLOTS > 0), "the wide tile: generic kernel, two consumers, slots");
   static constexpr int WN = BN * 2 / NCWG;                         // columns per consumer warpgroup
   static_assert(SLOTS == 0 || (!PAIR && !HALO && WN % 64 == 0), "slot epilogue: generic kernel, whole column groups");
   // four warpgroups: each column group's pair waits only on its own groups' slot phases, so every slot must carry
@@ -375,6 +379,11 @@ __device__ __forceinline__ bool tc_preact(__half2& h2, __half2& l2, const float*
 // PIPE: two slice tiles d0 / d1 alternate, so slice k + 1's wgmma run while slice k is waited for, released and
 // folded; without it every slice drains the warpgroup's wgmma queue before the fold.  Both orders fold the same tiles
 // in ascending k, so the results are bit-identical.
+// BN = 256 (wide tile, for C_out >= 256 on long K): the A tile of a stage serves twice the columns, a quarter less
+// L2 -> shared-memory operand traffic per FLOP than BN = 128.  A 128 x 256 register tile d next to the 128-register
+// running sum does not fit, so each slice runs as two 128-column halves: the BN = 128 slice chain on the B descriptors
+// of one half into a 64-register d, waited for and folded into that half of the running sum before the next half is
+// issued.  Every output element gets the BN = 128 kernel's MMA chain and fold order, so the results are bit-identical.
 // Epilogue: scale/bias (folded BN) -> +residual -> relu/relu6 -> fp32 or hi/lo split.
 // SLOTS > 0 (split outputs): per 64-column group of a tile, in order, the slot ring carries
 //   producer: wait slot empty -> TMA-load the residual boxes (hi, lo) into it, or arrive without bytes;
@@ -393,6 +402,7 @@ __global__ void __launch_bounds__(TcCfg<BN, STAGES, NCWG, PAIR, HALO, SLOTS>::TH
 conv_tc_kernel(const __grid_constant__ TcArgs a) {
   using Cfg = TcCfg<BN, STAGES, NCWG, PAIR, HALO, SLOTS>;
   static_assert(!PRE || !HALO, "pre-activation outputs: generic and 2-CTA kernels");
+  static_assert(BN != 256 || (!PIPE && !PRE), "the wide tile: single-buffered, no pre-activation output");
   constexpr int WN = Cfg::WN;
   constexpr int NR = WN / 2;                          // accumulator registers per thread (64 rows x WN / 128 threads)
   constexpr int NGT = BN / 64;                        // 64-column groups (slots) per tile
@@ -579,7 +589,28 @@ conv_tc_kernel(const __grid_constant__ TcArgs a) {
 #pragma unroll
         for (int j = 0; j < NR; ++j) racc[j] = __fadd_rn(racc[j], d[j]);
       };
-      if constexpr (PIPE) {
+      if constexpr (BN == 256) {
+        // two 128-column halves per slice (see above); the stage is freed once the second half has read it
+        constexpr uint64_t HALF_B = (128 * 128) >> 4;   // 128 weight rows, in 16 B descriptor units
+        for (int k = item.k0; k < item.k1; ++k, ++git) {
+          const TcSlice s = acquire(k, git);
+          float d[NR / 2];
+          tc_slice_mma<128>(d, s);
+          wgmma_wait0();
+          wgmma_fence_operand(d);
+#pragma unroll
+          for (int j = 0; j < NR / 2; ++j) racc[j] = __fadd_rn(racc[j], d[j]);
+          TcSlice s1 = s;
+          s1.bhi += HALF_B;
+          s1.blo += HALF_B;
+          tc_slice_mma<128>(d, s1);
+          wgmma_wait0();
+          release(k, s);
+          wgmma_fence_operand(d);
+#pragma unroll
+          for (int j = 0; j < NR / 2; ++j) racc[NR / 2 + j] = __fadd_rn(racc[NR / 2 + j], d[j]);
+        }
+      } else if constexpr (PIPE) {
         // slices alternate between d0 and d1 at compile-time-known places (a run-time choice of the tile serialises
         // the wgmma); the loop runs two slices per trip, the tail finishes one or two
         const int k1 = item.k1;
@@ -985,7 +1016,7 @@ void conv_workspace_create(ConvWorkspace& w) {
   LUMI_CUDA_CHECK(cudaGetDevice(&dev));
   LUMI_CUDA_CHECK(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
   w.ctas = n;
-  LUMI_CUDA_CHECK(cudaMalloc(&w.partials, (size_t)n * 128 * 128 * sizeof(float)));
+  LUMI_CUDA_CHECK(cudaMalloc(&w.partials, (size_t)n * 128 * TC_BN_MAX * sizeof(float)));
   LUMI_CUDA_CHECK(cudaMalloc(&w.flags, (size_t)n * sizeof(int)));
   LUMI_CUDA_CHECK(cudaMemset(w.flags, 0, (size_t)n * sizeof(int)));
   w.epoch = 0;
@@ -1095,13 +1126,20 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
   std::memset(&a, 0, sizeof(a));
   int nb, th, tw;
   pick_tile(io.in.n, io.ho, io.wo, nb, th, tw);
-  const int bn = (L.cout_pad % 128 == 0) ? 128 : 64;
+  const long n_iters_all = (long)L.kh * L.kw * (L.cin >> 6);
+  // 128 x 256 tiles (slot epilogue, no pre-activation output) on the layers with at least io.wide K slices and enough
+  // of those tiles for io.wide_sm_pct % of the SMs: on SSD's small extra layers (1-64 tiles) they measured up to 1.8x
+  // slower (DESIGN 7.1).  They are never halo or cluster-pair layers.
+  const long wide_tiles = (long)cdiv(io.in.n, nb) * cdiv(io.ho, th) * cdiv(io.wo, tw) * (L.cout_pad / 256);
+  const bool wide = io.wide && L.cout_pad % 256 == 0 && n_iters_all >= io.wide && !io.out_f32 && io.epi_tma &&
+                    !io.pre.hi && wide_tiles * 100 >= (long)sm_budget(io.sm_reserve) * io.wide_sm_pct;
+  const int bn = wide ? 256 : (L.cout_pad % 128 == 0) ? 128 : 64;
   // halo-patch kernels (3x3, stride 1, rate 1, SAME): tiles of th x 8 pixels of one image, th <= 16 chosen so that the
   // rows of the map split evenly.  They trade M-tile occupancy (th * 8 <= 128 rows, and the weights stream once per
   // tile) for ~6x less activation traffic, so they are used while the tile count stays within io.halo_tiles_pct of the
   // generic one.
   bool halo = false;
-  if (io.halo && L.kh == 3 && L.kw == 3 && L.stride == 1 && L.rate == 1 && io.pad_t == 1 && io.pad_l == 1 &&
+  if (io.halo && !wide && L.kh == 3 && L.kw == 3 && L.stride == 1 && L.rate == 1 && io.pad_t == 1 && io.pad_l == 1 &&
       !io.res.hi && !io.out_f32 && !io.pre.hi && !io.in_pix_pitch && !io.in_row_pitch && !io.in_img_pitch) {
     const int h_tiles = cdiv(io.ho, 16), h_th = cdiv(io.ho, h_tiles);
     const long std_tiles = (long)cdiv(io.in.n, nb) * cdiv(io.ho, th) * cdiv(io.wo, tw);
@@ -1118,7 +1156,6 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
                                io.in_row_pitch, io.in_img_pitch);
   }
   // CTA pairs on the long-K layers: each CTA of a pair loads (and multicasts) 64 of the 128 weight rows
-  const long n_iters_all = (long)L.kh * L.kw * (L.cin >> 6);
   const bool pair = io.cta2 && bn == 128 && !io.out_f32 && n_iters_all >= io.cta2;
   const int kdim = L.kh * L.kw * L.cin;
   a.tm_b_hi = cached_wgt_map(L.w_hi, L.cout_pad, kdim, pair ? bn / 2 : bn);
@@ -1164,7 +1201,10 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
       a.tm_r_hi = cached_act_map(io.res.hi, io.res.n, io.res.h, io.res.w, io.res.c, nb, th, tw, io.res_stride, 0, 0, 0);
       a.tm_r_lo = cached_act_map(io.res.lo, io.res.n, io.res.h, io.res.w, io.res.c, nb, th, tw, io.res_stride, 0, 0, 0);
     }
-    if (epi16) launch_tc<128, 2, 4, false, false, 2>(a, io, st);
+    // the wide tile: 2 x 96 KB stages + one slot (224 KB); a slice is twice the MMA work of a BN = 128 slice, so two
+    // stages keep as much of it in flight as four do there
+    if (wide) launch_tc_cfg<256, 2, 2, false, false, false, 1, false>(a, io.sk, io.streamk, io.sm_reserve, st);
+    else if (epi16) launch_tc<128, 2, 4, false, false, 2>(a, io, st);
     else if (bn == 128) launch_tc<128, 3, 2, false, false, 1>(a, io, st);
     else launch_tc<64, 3, 2, false, false, 2>(a, io, st);
     return;

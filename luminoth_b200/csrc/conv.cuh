@@ -60,6 +60,8 @@ struct ConvIO {
   int halo_tiles_pct = 150;     // ... while their M-tile count stays within this percentage of the generic kernel's
   int pipe = 1;                 // 1: double-buffered slice accumulators (slice k + 1's MMAs overlap slice k's fold); 0: single (the engine's default, LUMI_CONV_PIPE)
   int epi16 = 0;                // four-consumer-warpgroup (16 epilogue warps) kernel on layers with at most this many K slices per tile (0 = never)
+  int wide = 16;                // 128 x 256 tiles on split-output layers with cout_pad % 256 == 0 and at least this many K slices per tile (0 = never)
+  int wide_sm_pct = 50;         // ... while those tiles number at least this percentage of the SMs the launch may use
   int epi_tma = 1;              // 1: split outputs of the generic kernel leave through the shared-memory slot epilogue (TMA); 0: register epilogue
   int sm_reserve = 0;           // SMs a persistent launch leaves free (the engine's two-stream pipeline sets 8)
   // Optional strided ("Toeplitz") view of the input for the tensor-core path: element pitches between

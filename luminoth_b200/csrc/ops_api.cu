@@ -41,7 +41,7 @@ int op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, in
               int res_w, int res_stride, int act, int impl, const float* pre_scale, const float* pre_bias, float* y,
               float* p, int* ho_out, int* wo_out, cudaStream_t st) {
   const bool preact = pre_scale != nullptr;
-  LUMI_REQUIRE(impl >= 0 && impl <= 13, "conv2d: impl must be one of 0-13");
+  LUMI_REQUIRE(impl >= 0 && impl <= 15, "conv2d: impl must be one of 0-15");
   ConvLayer L;
   L.kh = kh; L.kw = kw; L.cin = cin; L.cout = cout; L.stride = stride; L.rate = rate; L.act = act;
   const size_t nw = (size_t)kh * kw * cin * cout;
@@ -71,7 +71,9 @@ int op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, in
   // four-warpgroup short-K kernel allowed (4), and 4 + stream-K (5), all through the shared-memory slot epilogue;
   // 6 / 7: the 2-CTA cluster kernel wherever it applies (7: + stream-K); 8-11: the halo-patch kernels (10, 11 on
   // cluster pairs; 9, 11: + stream-K); 12: as 3 with the register epilogue; 13: SIMT writing split planes (the engine's
-  // conv_impl = simt).  A pre-activation output is written in split planes only: SIMT (0 or 13), 3-7 or 12.
+  // conv_impl = simt); 14 / 15: as 3 on 128 x 256 tiles whatever the K-slice and tile counts (15: + stream-K), for layers with
+  // cout_pad % 256 == 0.  Codes 1-12 never take the 128 x 256 tile.  A pre-activation output is written in split planes
+  // only: SIMT (0 or 13), 3-7 or 12.
   const bool simt = impl == 0 || impl == 13;
   const bool split = preact || impl >= 3;
   if (preact)
@@ -124,8 +126,12 @@ int op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, in
     io.cta2 = (impl == 6 || impl == 7 || impl == 10 || impl == 11) ? 1 : 0;
     io.halo = (impl >= 8 && impl <= 11) ? 1 : 0;
     io.halo_tiles_pct = 1000000;                    // test hook: whenever the shape allows
+    const bool wide = impl == 14 || impl == 15;
+    io.wide = wide ? 1 : 0;
+    io.wide_sm_pct = 0;
     LUMI_REQUIRE(conv_tc_supported(L, io), "conv2d: this layer shape is not handled by the tensor-core kernel");
-    if (impl == 2 || impl == 5 || impl == 7 || impl == 9 || impl == 11) {
+    if (wide) LUMI_REQUIRE(L.cout_pad % 256 == 0, "conv2d: impl 14 / 15 need C_out padded to a multiple of 256");
+    if (impl == 2 || impl == 5 || impl == 7 || impl == 9 || impl == 11 || impl == 15) {
       conv_workspace_create(sk);
       io.sk = &sk;
       io.streamk = 2;
