@@ -6,7 +6,7 @@
 //
 // Reference structure restated here (not ported):
 //   models/fasterrcnn/fasterrcnn.py:70-156   FasterRCNN._build
-//   models/base/truncated_base_network.py:39-95  endpoint block3 / R101 block4 tail
+//   models/base/truncated_base_network.py:18-169 endpoint / R101 block4 tail
 //   models/fasterrcnn/rpn.py:136-180, rcnn.py:148-253
 //   models/ssd/ssd.py:37-195, models/ssd/feature_extractor.py:39-132
 #include "../../include/luminoth_b200.h"
@@ -69,6 +69,18 @@ const int BASE_DEPTH[4] = {64, 128, 256, 512};
 const int BLOCK_STRIDE[4] = {2, 2, 2, 1};
 const float RGB_MEANS[3] = {123.68f, 116.78f, 103.94f};
 
+// The part of a bottleneck unit a Faster R-CNN endpoint stops at: one of its collected convs, or the unit's output
+enum UnitPart { UP_CONV1, UP_CONV2, UP_CONV3, UP_SHORTCUT, UP_UNIT };
+
+// model.base_network.endpoint (truncated_base_network.py:18-37, 146-169): the trunk output that feeds the RPN and
+// the ROI pool.  block -1 is the stem conv; a block endpoint is its last unit's output.
+struct Endpoint {
+  std::string name = "block3";
+  int block = 0, unit = 0, part = UP_UNIT;
+  int depth = 0;
+  int stride = 0;               // feature stride of the endpoint map: the anchor grid is ceil(image size / stride)
+};
+
 }  // namespace
 
 struct lumi_engine {
@@ -85,7 +97,9 @@ struct lumi_engine {
   const ResnetArch* resnet = nullptr;         // Faster R-CNN base network
   int num_classes = 0;
   bool with_rcnn = true, use_tail = true, use_mean = true;
+  bool tail = false;                          // the RCNN runs the ROIs through block4 (truncated_base_network.py:56-95)
   int output_stride = 16;
+  Endpoint ep;
 
   std::vector<WeightSpec> required;
   std::map<std::string, HostTensor> staged;
@@ -204,31 +218,43 @@ std::string unit_scope(const lumi_engine* e, int b, int u) {
          (e->resnet->preact ? "/bottleneck_v2" : "/bottleneck_v1");
 }
 
-// slim resnet_v1 / resnet_v2 variables up to block3 (block4 only for the resnet_v1_101 tail); resnet_v2's `postnorm`
-// follows block4 and is never reached
+// Whether `part` of unit (b, u) is computed on the way to the endpoint: every part of an earlier unit, and of the
+// endpoint's own unit what its output reads (the shortcut only feeds the sum).  The tail runs all of block4.
+bool unit_part_runs(const lumi_engine* e, int b, int u, int part) {
+  const Endpoint& ep = e->ep;
+  if (b == 3 && e->tail) return true;
+  if (b != ep.block || u != ep.unit) return b < ep.block || (b == ep.block && u < ep.unit);
+  if (ep.part == UP_UNIT) return true;
+  if (part == UP_SHORTCUT || ep.part == UP_SHORTCUT) return part == ep.part;
+  return part <= ep.part;
+}
+
+// slim resnet_v1 / resnet_v2 variables up to the endpoint (and block4 for the resnet_v1_101 tail); resnet_v2's
+// `postnorm` follows block4 and is never reached
 void spec_resnet(lumi_engine* e) {
   const std::string root = "truncated_base_network/" + e->arch;
   const bool v2 = e->resnet->preact;
   if (v2) need_conv_bias(e, root + "/conv1", 7, 7, 3, 64);
   else need_conv_bn(e, root + "/conv1", 7, 7, 3, 64);
-  int cin = 64;
-  const bool tail = e->arch == "resnet_v1_101" && e->use_tail && e->with_rcnn;
-  const int nblocks = tail ? 4 : 3;
-  for (int b = 0; b < nblocks; ++b) {
+  for (int b = 0; b < 4; ++b) {
     const int bd = BASE_DEPTH[b], depth = bd * 4;
     for (int u = 0; u < e->resnet->units[b]; ++u) {
+      auto runs = [&](int part) { return unit_part_runs(e, b, u, part); };
+      if (!runs(UP_CONV1) && !runs(UP_SHORTCUT)) continue;
+      const int cin = u > 0 ? depth : b > 0 ? BASE_DEPTH[b - 1] * 4 : 64;
       const std::string s = unit_scope(e, b, u);
       if (v2)
         for (const char* n : {"gamma", "beta", "moving_mean", "moving_variance"}) need(e, s + "/preact/" + n, {cin});
-      if (cin != depth) {
+      if (cin != depth && runs(UP_SHORTCUT)) {
         if (v2) need_conv_bias(e, s + "/shortcut", 1, 1, cin, depth);
         else need_conv_bn(e, s + "/shortcut", 1, 1, cin, depth);
       }
-      need_conv_bn(e, s + "/conv1", 1, 1, cin, bd);
-      need_conv_bn(e, s + "/conv2", 3, 3, bd, bd);
-      if (v2) need_conv_bias(e, s + "/conv3", 1, 1, bd, depth);
-      else need_conv_bn(e, s + "/conv3", 1, 1, bd, depth);
-      cin = depth;
+      if (runs(UP_CONV1)) need_conv_bn(e, s + "/conv1", 1, 1, cin, bd);
+      if (runs(UP_CONV2)) need_conv_bn(e, s + "/conv2", 3, 3, bd, bd);
+      if (runs(UP_CONV3)) {
+        if (v2) need_conv_bias(e, s + "/conv3", 1, 1, bd, depth);
+        else need_conv_bn(e, s + "/conv3", 1, 1, bd, depth);
+      }
     }
   }
 }
@@ -289,6 +315,67 @@ int frcnn_output_stride(const JVal& c) {
   return (int)os;
 }
 
+// The conv2 stride and atrous rate of unit (b, u), as slim's stack_blocks_dense sets them at output_stride: each
+// block's last unit strides until the target stride is reached, after which its stride multiplies the rate of the
+// units that follow.  A unit's shortcut (projection or subsampled identity) takes the same stride.
+void unit_stride_rate(const lumi_engine* e, int b, int u, int& stride, int& rate) {
+  const int target = e->output_stride / 4;
+  int current = 1, r = 1;
+  for (int bb = 0; bb <= b; ++bb)
+    for (int uu = 0; uu < e->resnet->units[bb]; ++uu) {
+      const int s = uu == e->resnet->units[bb] - 1 ? BLOCK_STRIDE[bb] : 1;
+      const bool atrous = current == target;
+      if (bb == b && uu == u) { stride = atrous ? 1 : s; rate = atrous ? r : 1; return; }
+      if (atrous) r *= s;
+      else current *= s;
+    }
+}
+
+// model.base_network.endpoint (null or empty: block3), matched as _get_endpoint matches it against the outputs slim's
+// resnet collects: the stem conv1, every bottleneck unit and its conv1 / conv2 / conv3 / projection shortcut, and
+// every block.  Then the tail rule: resnet_v1_101's tail reuses block4's variables, whose first unit reads 1024
+// channels.  Needs output_stride, use_tail and with_rcnn.
+void parse_endpoint(lumi_engine* e) {
+  Endpoint& ep = e->ep;
+  const JVal* v = e->cfg.find("model.base_network.endpoint");
+  if (v && v->t != JVal::Null) {
+    if (v->t != JVal::Str) throw Error(LUMI_EINVAL, "model.base_network.endpoint must be a string");
+    if (!v->s.empty()) ep.name = v->s;
+  }
+  const std::string root = "truncated_base_network/" + e->arch, n = root + "/" + ep.name;
+  const char* PARTS[4] = {"/conv1", "/conv2", "/conv3", "/shortcut"};
+  bool found = n == root + "/conv1";
+  if (found) { ep.block = -1; ep.depth = 64; ep.stride = 2; }
+  int stride = 4;                                  // after pool1
+  for (int b = 0; b < 4 && !found; ++b) {
+    const int units = e->resnet->units[b];
+    for (int u = 0; u < units && !found; ++u) {
+      const std::string s = unit_scope(e, b, u);
+      int part = -1;
+      if (n == s || (u == units - 1 && n == root + "/block" + std::to_string(b + 1))) part = UP_UNIT;
+      for (int p = 0; p < 4; ++p)
+        if (n == s + PARTS[p] && (p != UP_SHORTCUT || u == 0)) part = p;   // only a block's first unit projects
+      int st, rt;
+      unit_stride_rate(e, b, u, st, rt);
+      if (part != UP_CONV1) stride *= st;
+      if (part < 0) continue;
+      found = true;
+      ep.block = b; ep.unit = u; ep.part = part;
+      ep.depth = BASE_DEPTH[b] * (part == UP_CONV1 || part == UP_CONV2 ? 1 : 4);
+      ep.stride = stride;
+    }
+  }
+  if (!found) throw Error(LUMI_EINVAL, "\"" + n + "\" is an invalid value of endpoint for this architecture.");
+  e->tail = e->arch == "resnet_v1_101" && e->use_tail && e->with_rcnn;
+  if (e->tail && ep.depth != 1024)
+    throw Error(LUMI_EINVAL, "the resnet_v1_101 tail needs a 1024-channel endpoint: \"" + ep.name + "\" has " +
+                                 std::to_string(ep.depth) + " channels (set model.base_network.use_tail to false)");
+}
+
+// the endpoint map's size along an image side of `size` pixels: every stride-2 stage (conv2d_same, SAME max pool,
+// subsampled shortcut) gives ceil(x / 2)
+int feature_size(const lumi_engine* e, int size) { return cdiv(size, e->ep.stride); }
+
 void parse_config(lumi_engine* e) {
   const JVal& c = e->cfg;
   e->type = c.str("model.type", "");
@@ -305,11 +392,10 @@ void parse_config(lumi_engine* e) {
     }
     if (!e->resnet)
       throw Error(LUMI_EINVAL, "base_network.architecture '" + e->arch + "' is not built yet (" + known + ")");
-    const JVal* ep = c.find("model.base_network.endpoint");
-    if (ep && ep->t == JVal::Str && ep->s != "block3") throw Error(LUMI_EINVAL, "only endpoint block3 is supported");
     e->with_rcnn = c.boolean("model.network.with_rcnn", false);
     e->use_tail = c.boolean("model.base_network.use_tail", true);
     e->output_stride = frcnn_output_stride(c);
+    parse_endpoint(e);
     e->anchor_stride = (int)c.number("model.anchors.stride", 16);
     compute_frcnn_anchor_ref(e);
     e->rpn_channels = (int)c.number("model.rpn.num_channels", 512);
@@ -379,14 +465,14 @@ void build_specs(lumi_engine* e) {
   if (e->type == "fasterrcnn") {
     spec_resnet(e);
     const std::string r = "fasterrcnn/rpn";
-    need(e, r + "/conv/w", {e->rpn_kh, e->rpn_kw, 1024, e->rpn_channels});
+    need(e, r + "/conv/w", {e->rpn_kh, e->rpn_kw, e->ep.depth, e->rpn_channels});
     need(e, r + "/conv/b", {e->rpn_channels});
     need(e, r + "/cls_conv/w", {1, 1, e->rpn_channels, 2 * e->A});
     need(e, r + "/cls_conv/b", {2 * e->A});
     need(e, r + "/bbox_conv/w", {1, 1, e->rpn_channels, 4 * e->A});
     need(e, r + "/bbox_conv/b", {4 * e->A});
     if (e->with_rcnn) {
-      int d = (e->arch == "resnet_v1_101" && e->use_tail) ? 2048 : 1024;
+      int d = e->tail ? 2048 : e->ep.depth;
       if (!e->use_mean) d *= e->pooled_w * e->pooled_h;
       const std::string c = "fasterrcnn/rcnn";
       for (size_t i = 0; i < e->fc_sizes.size(); ++i) {
@@ -534,35 +620,32 @@ void build_layers(lumi_engine* e) {
       conv_layer_upload(L, w2.data(), sc.data(), bi.data());
       e->layers[root + "/conv1#s2d"] = L;
     }
-    int cin = 64;
-    const bool tail = e->arch == "resnet_v1_101" && e->use_tail && e->with_rcnn;
-    const int nblocks = tail ? 4 : 3;
-    int current = 1, rate = 1;
-    const int target = e->output_stride / 4;
-    for (int b = 0; b < nblocks; ++b) {
+    for (int b = 0; b < 4; ++b) {
       const int bd = BASE_DEPTH[b], depth = bd * 4;
       for (int u = 0; u < units[b]; ++u) {
+        auto runs = [&](int part) { return unit_part_runs(e, b, u, part); };
+        if (!runs(UP_CONV1) && !runs(UP_SHORTCUT)) continue;
+        const int cin = u > 0 ? depth : b > 0 ? BASE_DEPTH[b - 1] * 4 : 64;
         const std::string s = unit_scope(e, b, u);
-        int unit_stride = (u == units[b] - 1) ? BLOCK_STRIDE[b] : 1;
-        int st = unit_stride, rt = 1;
-        if (b == 3) { st = 1; rt = 1; }                       // tail: stack_blocks_dense w/o output_stride, stride 1
-        else if (current == target) { st = 1; rt = rate; rate *= unit_stride; }
-        else { current *= unit_stride; }
+        int st = 1, rt = 1;                                   // tail: stack_blocks_dense w/o output_stride, stride 1
+        if (!(b == 3 && e->tail)) unit_stride_rate(e, b, u, st, rt);
         if (v2) {
           // bottleneck_v2: preact = relu(BN(x)); shortcut and conv3 with biases, no BN or activation; out = the raw sum
           make_preact(e, s);
-          if (cin != depth) make_conv_bias(e, s + "/shortcut", {s + "/shortcut/weights"}, {s + "/shortcut/biases"}, st, 1,
-                                           ACT_NONE);
-          make_conv_bn(e, s + "/conv1", 1, 1, ACT_RELU);
-          make_conv_bn(e, s + "/conv2", st, rt, ACT_RELU);
-          make_conv_bias(e, s + "/conv3", {s + "/conv3/weights"}, {s + "/conv3/biases"}, 1, 1, ACT_NONE);
+          if (cin != depth && runs(UP_SHORTCUT))
+            make_conv_bias(e, s + "/shortcut", {s + "/shortcut/weights"}, {s + "/shortcut/biases"}, st, 1, ACT_NONE);
+          if (runs(UP_CONV1)) make_conv_bn(e, s + "/conv1", 1, 1, ACT_RELU);
+          if (runs(UP_CONV2)) make_conv_bn(e, s + "/conv2", st, rt, ACT_RELU);
+          if (runs(UP_CONV3))
+            make_conv_bias(e, s + "/conv3", {s + "/conv3/weights"}, {s + "/conv3/biases"}, 1, 1, ACT_NONE);
         } else {
-          if (cin != depth) make_conv_bn(e, s + "/shortcut", st, 1, ACT_NONE);
-          make_conv_bn(e, s + "/conv1", 1, 1, ACT_RELU);
-          make_conv_bn(e, s + "/conv2", st, rt, ACT_RELU);
-          make_conv_bn(e, s + "/conv3", 1, 1, ACT_RELU);      // relu applied after the residual add
+          if (cin != depth && runs(UP_SHORTCUT)) make_conv_bn(e, s + "/shortcut", st, 1, ACT_NONE);
+          if (runs(UP_CONV1)) make_conv_bn(e, s + "/conv1", 1, 1, ACT_RELU);
+          if (runs(UP_CONV2)) make_conv_bn(e, s + "/conv2", st, rt, ACT_RELU);
+          // relu applied after the residual add; a conv3 endpoint is collected before both
+          const bool conv3_ep = b == e->ep.block && u == e->ep.unit && e->ep.part == UP_CONV3;
+          if (runs(UP_CONV3)) make_conv_bn(e, s + "/conv3", 1, 1, conv3_ep ? ACT_NONE : ACT_RELU);
         }
-        cin = depth;
       }
     }
     const std::string r = "fasterrcnn/rpn";
@@ -799,37 +882,47 @@ Act run_pool(Ctx& cx, Act in, int k, int stride, bool same, const PreAct* pre = 
   return out;
 }
 
-Act bottleneck(Ctx& cx, const std::string& s, Act x, int depth) {
-  const ConvLayer& c2 = cx.e->layers.at(s + "/conv2");
-  const int stride = c2.stride;
+// slim bottleneck_v1; `stop` (a UnitPart) returns that collected conv output instead of the unit's
+Act bottleneck(Ctx& cx, const std::string& s, Act x, int depth, int stop = UP_UNIT) {
+  if (stop == UP_SHORTCUT) return run_conv(cx, s + "/shortcut", x, 1, nullptr, 1, nullptr);
   Act shortcut = x;
-  int res_stride = stride;
-  if (x.c != depth) { shortcut = run_conv(cx, s + "/shortcut", x, 1, nullptr, 1, nullptr); res_stride = 1; }
+  int res_stride = 1;
+  if (stop == UP_UNIT) {
+    res_stride = cx.e->layers.at(s + "/conv2").stride;
+    if (x.c != depth) { shortcut = run_conv(cx, s + "/shortcut", x, 1, nullptr, 1, nullptr); res_stride = 1; }
+  }
   Act r = run_conv(cx, s + "/conv1", x, 1, nullptr, 1, nullptr);
+  if (stop == UP_CONV1) return r;
   r = run_conv(cx, s + "/conv2", r, 2, nullptr, 1, nullptr);
-  return run_conv(cx, s + "/conv3", r, 1, &shortcut, res_stride, nullptr);
+  if (stop == UP_CONV2) return r;
+  return run_conv(cx, s + "/conv3", r, 1, stop == UP_UNIT ? &shortcut : nullptr, res_stride, nullptr);
 }
 
 // slim bottleneck_v2 on (x, p = relu(BN_preact(x))); x may be absent when the unit projects its shortcut from p.
 // conv3 writes what the next unit reads, from `next` (nullptr: the endpoint, x only): p always, and x as well when
-// that unit's shortcut is the identity (its depth equals this unit's).
-Act bottleneck_v2(Ctx& cx, const std::string& s, Act x, Act p, int depth, PreAct* next) {
-  const ConvLayer& c2 = cx.e->layers.at(s + "/conv2");
+// that unit's shortcut is the identity (its depth equals this unit's).  `stop` as in bottleneck().
+Act bottleneck_v2(Ctx& cx, const std::string& s, Act x, Act p, int depth, PreAct* next, int stop = UP_UNIT) {
+  if (stop == UP_SHORTCUT) return run_conv(cx, s + "/shortcut", p, 1, nullptr, 1, nullptr);
   Act shortcut = x;
-  int res_stride = c2.stride;                        // subsample(x, stride)
-  if (p.c != depth) { shortcut = run_conv(cx, s + "/shortcut", p, 1, nullptr, 1, nullptr); res_stride = 1; }
+  int res_stride = 1;
+  if (stop == UP_UNIT) {
+    res_stride = cx.e->layers.at(s + "/conv2").stride;   // subsample(x, stride)
+    if (p.c != depth) { shortcut = run_conv(cx, s + "/shortcut", p, 1, nullptr, 1, nullptr); res_stride = 1; }
+  }
   Act r = run_conv(cx, s + "/conv1", p, 1, nullptr, 1, nullptr);
+  if (stop == UP_CONV1) return r;
   r = run_conv(cx, s + "/conv2", r, 2, nullptr, 1, nullptr);
-  return run_conv(cx, s + "/conv3", r, 1, &shortcut, res_stride, nullptr, nullptr, -1.0, next);
+  if (stop == UP_CONV2) return r;
+  return run_conv(cx, s + "/conv3", r, 1, stop == UP_UNIT ? &shortcut : nullptr, res_stride, nullptr, nullptr, -1.0,
+                  next);
 }
 
 // ---------------------------------------------------------------- Faster R-CNN forward
 void ensure_frcnn_anchors(lumi_engine* e, int h, int w, cudaStream_t st) {
-  // fasterrcnn.py:261-308; the grid follows the block3 feature map, ceil(size / output_stride): every stride-2 stage
-  // (conv2d_same, SAME max pool, subsampled shortcut) gives ceil(x / 2).
+  // fasterrcnn.py:261-308; the grid follows the endpoint's feature map.
   // One buffer per grid shape, kept for the engine's lifetime: captured graphs of other image sizes keep pointing
   // at theirs (a server sees a handful of distinct sizes).
-  const int fh = cdiv(h, e->output_stride), fw = cdiv(w, e->output_stride);
+  const int fh = feature_size(e, h), fw = feature_size(e, w);
   if (e->anchors_fh == fh && e->anchors_fw == fw) return;
   auto it = e->anchor_grids.find({fh, fw});
   if (it == e->anchor_grids.end()) {
@@ -877,20 +970,27 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
     if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_u8_to_act(images, cx.img_f32, x, RGB_MEANS, cx.st); }  // base_network.py:153-177
     x = run_conv(cx, root + "/conv1", x, 2, nullptr, 1, nullptr);        // conv2d_same(64, 7, stride 2) + BN + relu
   }                                                                      // (v2: + bias, no activation)
-  if (!v2) {
+  const Endpoint& ep = e->ep;
+  if (ep.block < 0) {
+    // the stem conv is the endpoint
+  } else if (!v2) {
     x = run_pool(cx, x, 3, 2, true);                                     // pool1 3x3/2 SAME
-    for (int b = 0; b < 3; ++b)
-      for (int u = 0; u < units[b]; ++u) x = bottleneck(cx, unit_scope(e, b, u), x, BASE_DEPTH[b] * 4);
+    for (int b = 0; b <= ep.block; ++b)
+      for (int u = 0; u < units[b]; ++u) {
+        const bool at_ep = b == ep.block && u == ep.unit;
+        x = bottleneck(cx, unit_scope(e, b, u), x, BASE_DEPTH[b] * 4, at_ep ? ep.part : UP_UNIT);
+        if (at_ep) break;
+      }
   } else {
     // block1/unit_1 projects from its preact: the stem's pool emits only p = relu(BN(pool1))
     const PreAct first = preact_of(e, unit_scope(e, 0, 0), false);
     Act p = run_pool(cx, x, 3, 2, true, &first);
     x = Act();
-    for (int b = 0; b < 3; ++b)
+    for (int b = 0; b <= ep.block; ++b)
       for (int u = 0; u < units[b]; ++u) {
         const bool last_of_block = u + 1 == units[b];
-        if (b == 2 && last_of_block) {                                   // the endpoint: x only
-          x = bottleneck_v2(cx, unit_scope(e, b, u), x, p, BASE_DEPTH[b] * 4, nullptr);
+        if (b == ep.block && u == ep.unit) {                             // the endpoint: x only
+          x = bottleneck_v2(cx, unit_scope(e, b, u), x, p, BASE_DEPTH[b] * 4, nullptr, ep.part);
           break;
         }
         // the next unit's shortcut is the identity (reads x) unless it opens the next block (projects from p)
@@ -900,7 +1000,7 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
         p = next.p;
       }
   }
-  const Act fmap = x;                                                    // endpoint block3
+  const Act fmap = x;                                                    // the endpoint
   cx.tap_act("conv_feature_map", fmap);
   const int fh = fmap.h, fw = fmap.w;
 
@@ -952,8 +1052,7 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
   }
 
   // RCNN (rcnn.py:174-232)
-  const bool has_tail = e->arch == "resnet_v1_101" && e->use_tail;      // truncated_base_network.py:56-95
-  const bool fuse_mean = e->use_mean && !has_tail;                        // ROI crop+max-pool+mean in one kernel
+  const bool fuse_mean = e->use_mean && !e->tail;                         // ROI crop+max-pool+mean in one kernel
   const bool need_pooled = !fuse_mean || e->debug_taps;
   Act pooled, feat;
   float* fmap_f32 = cx.f32(fmap.numel());                                  // gather source of the ROI kernel
@@ -971,7 +1070,7 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
   if (need_pooled) cx.tap_act("roi_pool", pooled);
   if (!fuse_mean) {
     feat = pooled;
-    if (has_tail)
+    if (e->tail)                                                         // truncated_base_network.py:56-95
       for (int u = 0; u < 3; ++u)
         feat = bottleneck(cx, root + "/block4/unit_" + std::to_string(u + 1) + "/bottleneck_v1", feat, 2048);
     if (e->use_mean) {
@@ -1178,7 +1277,7 @@ void ensure_arena(lumi_engine* e, Arena& a, size_t need_bytes) {
 // RPN workspace (the only buffer sized by the image) grows on demand; arenas are re-planned per shape anyway.
 void ensure_image_capacity(lumi_engine* e, int h, int w) {
   if (e->type != "fasterrcnn") return;                 // SSD runs at its configured fixed size only
-  const long na = (long)cdiv(h, e->output_stride) * cdiv(w, e->output_stride) * e->A;
+  const long na = (long)feature_size(e, h) * feature_size(e, w) * e->A;
   LUMI_REQUIRE(na < (1L << 30), "lumi_predict: image too large");
   if (na <= e->ws_rpn.cap) return;
   e->drop_graphs();
@@ -1299,7 +1398,7 @@ int lumi_finalize(lumi_engine* e) {
     LUMI_CUDA_CHECK(cudaMalloc(&e->d_anchor_ref, e->anchor_ref.size() * sizeof(int)));
     LUMI_CUDA_CHECK(cudaMemcpy(e->d_anchor_ref, e->anchor_ref.data(), e->anchor_ref.size() * sizeof(int),
                                cudaMemcpyHostToDevice));
-    const int fh = cdiv(e->max_h, e->output_stride), fw = cdiv(e->max_w, e->output_stride);
+    const int fh = feature_size(e, e->max_h), fw = feature_size(e, e->max_w);
     nms_workspace_alloc(e->ws_rpn, nb, fh * fw * e->A, e->rpn.post_nms_top_n,
                         std::min(fh * fw * e->A, e->rpn.pre_nms_top_n));
     if (e->with_rcnn) {

@@ -13,6 +13,8 @@ Init distributions: ``models/fasterrcnn/base_config.yml:185-199,246-261``
 ('reference' profile); the 'peaky' profile scales the classifier / box
 regressors so probabilities spread and NMS has real work.
 """
+import re
+
 import numpy as np
 
 RESNET_UNITS = {'resnet_v1_50': (3, 4, 6, 3), 'resnet_v1_101': (3, 4, 23, 3), 'resnet_v1_152': (3, 8, 36, 3),
@@ -41,34 +43,58 @@ def _bias(rng, c):
     return (rng.standard_normal(c) * 0.05).astype(np.float32)
 
 
+def _v2_block(rng, wts, root, arch, b):
+    """One block of slim resnet_v2 (pre-activation) units."""
+    bd = BASE_DEPTH[b]
+    depth = bd * 4
+    cin = BASE_DEPTH[b - 1] * 4 if b else 64
+    for u in range(RESNET_UNITS[arch][b]):
+        s = '%s/block%d/unit_%d/bottleneck_v2' % (root, b + 1, u + 1)
+        p = s + '/preact/'
+        wts[p + 'gamma'] = rng.uniform(0.8, 1.2, cin).astype(np.float32)
+        wts[p + 'beta'] = (rng.standard_normal(cin) * 0.05).astype(np.float32)
+        wts[p + 'moving_mean'] = (rng.standard_normal(cin) * 0.05).astype(np.float32)
+        wts[p + 'moving_variance'] = rng.uniform(0.8, 1.2, cin).astype(np.float32)
+        if cin != depth:
+            wts[s + '/shortcut/weights'] = _conv(rng, 1, 1, cin, depth)
+            wts[s + '/shortcut/biases'] = _bias(rng, depth)
+        wts[s + '/conv1/weights'] = _conv(rng, 1, 1, cin, bd)
+        _bn(rng, wts, s + '/conv1', bd)
+        wts[s + '/conv2/weights'] = _conv(rng, 3, 3, bd, bd)
+        _bn(rng, wts, s + '/conv2', bd)
+        wts[s + '/conv3/weights'] = _conv(rng, 1, 1, bd, depth,
+                                          std=V2_CONV3_SCALE * np.sqrt(2.0 / bd / RESNET_UNITS[arch][b]))
+        wts[s + '/conv3/biases'] = _bias(rng, depth)
+        cin = depth
+
+
+def _v1_block(rng, wts, root, arch, b):
+    """One block of slim resnet_v1 units."""
+    bd = BASE_DEPTH[b]
+    depth = bd * 4
+    cin = BASE_DEPTH[b - 1] * 4 if b else 64
+    for u in range(RESNET_UNITS[arch][b]):
+        s = '%s/block%d/unit_%d/bottleneck_v1' % (root, b + 1, u + 1)
+        if cin != depth:
+            wts[s + '/shortcut/weights'] = _conv(rng, 1, 1, cin, depth)
+            _bn(rng, wts, s + '/shortcut', depth)
+        wts[s + '/conv1/weights'] = _conv(rng, 1, 1, cin, bd)
+        _bn(rng, wts, s + '/conv1', bd)
+        wts[s + '/conv2/weights'] = _conv(rng, 3, 3, bd, bd)
+        _bn(rng, wts, s + '/conv2', bd)
+        wts[s + '/conv3/weights'] = _conv(rng, 1, 1, bd, depth)
+        _bn(rng, wts, s + '/conv3', depth, gamma_scale=0.25)
+        cin = depth
+
+
 def resnet_v2_weights(rng, arch, scope='truncated_base_network'):
     """slim resnet_v2 (pre-activation) variables through block3."""
     wts = {}
     root = '%s/%s' % (scope, arch)
     wts[root + '/conv1/weights'] = _conv(rng, 7, 7, 3, 64, std=np.sqrt(2.0 / 147) / 64.0)
     wts[root + '/conv1/biases'] = _bias(rng, 64)
-    cin = 64
     for b in range(3):
-        bd = BASE_DEPTH[b]
-        depth = bd * 4
-        for u in range(RESNET_UNITS[arch][b]):
-            s = '%s/block%d/unit_%d/bottleneck_v2' % (root, b + 1, u + 1)
-            p = s + '/preact/'
-            wts[p + 'gamma'] = rng.uniform(0.8, 1.2, cin).astype(np.float32)
-            wts[p + 'beta'] = (rng.standard_normal(cin) * 0.05).astype(np.float32)
-            wts[p + 'moving_mean'] = (rng.standard_normal(cin) * 0.05).astype(np.float32)
-            wts[p + 'moving_variance'] = rng.uniform(0.8, 1.2, cin).astype(np.float32)
-            if cin != depth:
-                wts[s + '/shortcut/weights'] = _conv(rng, 1, 1, cin, depth)
-                wts[s + '/shortcut/biases'] = _bias(rng, depth)
-            wts[s + '/conv1/weights'] = _conv(rng, 1, 1, cin, bd)
-            _bn(rng, wts, s + '/conv1', bd)
-            wts[s + '/conv2/weights'] = _conv(rng, 3, 3, bd, bd)
-            _bn(rng, wts, s + '/conv2', bd)
-            wts[s + '/conv3/weights'] = _conv(rng, 1, 1, bd, depth,
-                                              std=V2_CONV3_SCALE * np.sqrt(2.0 / bd / RESNET_UNITS[arch][b]))
-            wts[s + '/conv3/biases'] = _bias(rng, depth)
-            cin = depth
+        _v2_block(rng, wts, root, arch, b)
     return wts
 
 
@@ -81,33 +107,76 @@ def resnet_weights(rng, arch, with_block4, scope='truncated_base_network'):
     # activations stay O(1) like a trained net.
     wts[root + '/conv1/weights'] = _conv(rng, 7, 7, 3, 64, std=np.sqrt(2.0 / 147) / 64.0)
     _bn(rng, wts, root + '/conv1', 64)
-    cin = 64
-    nblocks = 4 if with_block4 else 3
-    for b in range(nblocks):
-        bd = BASE_DEPTH[b]
-        depth = bd * 4
-        for u in range(RESNET_UNITS[arch][b]):
-            s = '%s/block%d/unit_%d/bottleneck_v1' % (root, b + 1, u + 1)
-            if cin != depth:
-                wts[s + '/shortcut/weights'] = _conv(rng, 1, 1, cin, depth)
-                _bn(rng, wts, s + '/shortcut', depth)
-            wts[s + '/conv1/weights'] = _conv(rng, 1, 1, cin, bd)
-            _bn(rng, wts, s + '/conv1', bd)
-            wts[s + '/conv2/weights'] = _conv(rng, 3, 3, bd, bd)
-            _bn(rng, wts, s + '/conv2', bd)
-            wts[s + '/conv3/weights'] = _conv(rng, 1, 1, bd, depth)
-            _bn(rng, wts, s + '/conv3', depth, gamma_scale=0.25)
-            cin = depth
+    for b in range(4 if with_block4 else 3):
+        _v1_block(rng, wts, root, arch, b)
     return wts
+
+
+ENDPOINT_PARTS = ('conv1', 'conv2', 'conv3', 'shortcut')
+
+
+def parse_endpoint(arch, endpoint):
+    """``(block, unit, part, depth)`` of a Faster R-CNN ``base_network.endpoint`` among the outputs slim's resnet
+    collects: block -1 is the stem ``conv1``, ``part`` None a unit's output (``blockN`` is its last unit's).  Anything
+    else raises the reference's ValueError (``truncated_base_network.py:146-169``)."""
+    units = RESNET_UNITS[arch]
+    kind = 'bottleneck_v2' if arch.startswith('resnet_v2') else 'bottleneck_v1'
+    if endpoint == 'conv1':
+        return -1, 0, None, 64
+    for b in range(4):
+        deep = BASE_DEPTH[b] * 4
+        if endpoint == 'block%d' % (b + 1):
+            return b, units[b] - 1, None, deep
+        for u in range(units[b]):
+            s = 'block%d/unit_%d/%s' % (b + 1, u + 1, kind)
+            if endpoint == s:
+                return b, u, None, deep
+            for p in ENDPOINT_PARTS:
+                if endpoint == s + '/' + p and (p != 'shortcut' or u == 0):    # only a block's first unit projects
+                    return b, u, p, BASE_DEPTH[b] if p in ('conv1', 'conv2') else deep
+    raise ValueError('"truncated_base_network/%s/%s" is an invalid value of endpoint for this architecture.'
+                     % (arch, endpoint))
+
+
+def _truncate(wts, arch, endpoint, tail, scope='truncated_base_network'):
+    """Drop the trunk variables the forward to ``endpoint`` never reads (keeping block4 for the tail)."""
+    eb, eu, epart, _ = parse_endpoint(arch, endpoint)
+    unit_var = re.compile(r'%s/%s/block(\d)/unit_(\d+)/bottleneck_v\d/(\w+)/' % (scope, arch))
+
+    def reads(key):
+        m = unit_var.match(key)
+        if not m:
+            return True                         # the stem, and everything outside the trunk
+        b, u, part = int(m.group(1)) - 1, int(m.group(2)) - 1, m.group(3)
+        if b == 3 and tail:
+            return True
+        if (b, u) != (eb, eu):
+            return (b, u) < (eb, eu)
+        if epart is None or part == 'preact':
+            return True
+        if 'shortcut' in (part, epart):         # the shortcut only feeds the unit's sum
+            return part == epart
+        return ENDPOINT_PARTS.index(part) <= ENDPOINT_PARTS.index(epart)
+    return {k: v for k, v in wts.items() if reads(k)}
 
 
 def fasterrcnn_weights(config, seed=0, profile='peaky'):
     m = config['model']
-    arch = m['base_network']['architecture']
+    bn = m['base_network']
+    arch = bn['architecture']
     if arch not in RESNET_UNITS:
         raise ValueError('synthetic weights: unsupported architecture %r' % arch)
+    endpoint = bn.get('endpoint') or 'block3'
+    block, _, _, depth = parse_endpoint(arch, endpoint)
     rng = np.random.default_rng(seed)
     wts = resnet_weights(rng, arch, with_block4=(arch == 'resnet_v1_101'))
+    if endpoint != 'block3':
+        if block == 3 and arch != 'resnet_v1_101':
+            # a generator of its own: the draws of every block3 configuration stay as they are
+            block4 = _v2_block if arch.startswith('resnet_v2') else _v1_block
+            block4(np.random.default_rng([seed, 4]), wts, 'truncated_base_network/' + arch, arch, 3)
+        tail = arch == 'resnet_v1_101' and bn.get('use_tail', True) and m['network'].get('with_rcnn', False)
+        wts = _truncate(wts, arch, endpoint, tail)
     a = m['anchors']
     A = len(a['scales']) * len(a['ratios'])
     C = m['network']['num_classes']
@@ -115,13 +184,13 @@ def fasterrcnn_weights(config, seed=0, profile='peaky'):
     kh, kw = m['rpn']['kernel_shape']
     peaky = profile == 'peaky'
     r = 'fasterrcnn/rpn'
-    wts[r + '/conv/w'] = _conv(rng, kh, kw, 1024, nch, std=0.01)
+    wts[r + '/conv/w'] = _conv(rng, kh, kw, depth, nch, std=0.01)
     wts[r + '/conv/b'] = (rng.standard_normal(nch) * 0.01).astype(np.float32)
     wts[r + '/cls_conv/w'] = _conv(rng, 1, 1, nch, 2 * A, std=0.02 if peaky else 0.01)
     wts[r + '/cls_conv/b'] = (rng.standard_normal(2 * A) * 0.01).astype(np.float32)
     wts[r + '/bbox_conv/w'] = _conv(rng, 1, 1, nch, 4 * A, std=0.005 if peaky else 0.001)
     wts[r + '/bbox_conv/b'] = (rng.standard_normal(4 * A) * 0.001).astype(np.float32)
-    d = 2048 if arch == 'resnet_v1_101' and m['base_network'].get('use_tail', True) else 1024
+    d = 2048 if arch == 'resnet_v1_101' and bn.get('use_tail', True) and depth == 1024 else depth   # the tail's output
     if not m['rcnn'].get('use_mean', True):
         d *= m['rcnn']['roi']['pooled_width'] * m['rcnn']['roi']['pooled_height']
     c = 'fasterrcnn/rcnn'
