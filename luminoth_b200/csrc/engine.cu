@@ -39,6 +39,28 @@ struct WeightSpec {
   std::vector<int64_t> shape;
 };
 
+// A conv's padding: TF VALID, TF SAME, or slim conv2d_same (explicit pad + VALID when stride > 1)
+enum Padding { PAD_VALID, PAD_SAME, PAD_CONV2D_SAME };
+
+// What a layer record builds: a conv with folded slim batch norm; a conv or fc with biases, where several scopes fuse
+// along C_out; a resnet_v2 `preact` batch norm; SSD's L2-norm gamma; or a tensor-core form of the conv of another
+// record, from whose weights it is built (it reads no variables of its own)
+enum LayerKind { LK_CONV_BN, LK_CONV_BIAS, LK_PREACT, LK_GAMMA, LK_STEM_S2D, LK_CONV1_1_PACK };
+// Variable names of a bias conv: slim weights / biases, Sonnet w / b, or Sonnet Linear w / b with [C_in, C_out] weights
+enum Naming { NM_SLIM, NM_SONNET, NM_LINEAR };
+
+// One record of the engine's layer table (build_net): the variables a layer reads and how it runs
+struct Layer {
+  std::string key;                    // engine key: run_conv's name of the layer, or the dev_vecs prefix
+  int kind = LK_CONV_BIAS, naming = NM_SLIM;
+  std::vector<std::string> scopes;    // variable scopes
+  int kh = 1, kw = 1, cin = 0;        // cin: the channels of a preact or gamma vector
+  std::vector<int> couts;             // per scope
+  int stride = 1, rate = 1, act = ACT_NONE;
+  int padding = PAD_VALID;            // the derived layers read staging buffers that carry their padding
+  ConvLayer conv;                     // the uploaded conv (lumi_finalize)
+};
+
 struct Arena {
   uint8_t* base = nullptr;
   size_t cap = 0, off = 0;
@@ -101,10 +123,11 @@ struct lumi_engine {
   int output_stride = 16;
   Endpoint ep;
 
-  std::vector<WeightSpec> required;
+  std::vector<Layer> net;                     // the layer table, in the order of the variables (build_net)
+  std::map<std::string, size_t> net_index;    // engine key -> record
+  std::vector<WeightSpec> required;           // the variables of the table
   std::map<std::string, HostTensor> staged;
-  std::map<std::string, ConvLayer> layers;
-  std::map<std::string, float*> dev_vecs;     // misc device vectors (l2norm gamma)
+  std::map<std::string, float*> dev_vecs;     // misc device vectors (l2norm gamma, preact scale / bias)
 
   // Faster R-CNN
   int A = 0, anchor_stride = 16;
@@ -175,7 +198,7 @@ struct lumi_engine {
 
   ~lumi_engine() {
     drop_graphs();
-    for (auto& kv : layers) conv_layer_free(kv.second);
+    for (auto& r : net) conv_layer_free(r.conv);
     for (auto& kv : dev_vecs) cudaFree(kv.second);
     nms_workspace_free(ws_rpn); nms_workspace_free(ws_det);
     conv_workspace_free(sk_ws[0]); conv_workspace_free(sk_ws[1]);
@@ -196,23 +219,7 @@ namespace {
 
 thread_local std::string g_create_error;
 
-// ---------------------------------------------------------------- weight specs
-void need(lumi_engine* e, const std::string& name, std::vector<int64_t> shape) {
-  e->required.push_back({name, std::move(shape)});
-}
-void need_bn(lumi_engine* e, const std::string& scope, int c) {
-  for (const char* n : {"gamma", "beta", "moving_mean", "moving_variance"}) need(e, scope + "/BatchNorm/" + n, {c});
-}
-void need_conv_bn(lumi_engine* e, const std::string& scope, int kh, int kw, int cin, int cout) {
-  need(e, scope + "/weights", {kh, kw, cin, cout});
-  need_bn(e, scope, cout);
-}
-
-void need_conv_bias(lumi_engine* e, const std::string& scope, int kh, int kw, int cin, int cout) {
-  need(e, scope + "/weights", {kh, kw, cin, cout});
-  need(e, scope + "/biases", {cout});
-}
-
+// ---------------------------------------------------------------- network structure
 std::string unit_scope(const lumi_engine* e, int b, int u) {
   return "truncated_base_network/" + e->arch + "/block" + std::to_string(b + 1) + "/unit_" + std::to_string(u + 1) +
          (e->resnet->preact ? "/bottleneck_v2" : "/bottleneck_v1");
@@ -229,45 +236,16 @@ bool unit_part_runs(const lumi_engine* e, int b, int u, int part) {
   return part <= ep.part;
 }
 
-// slim resnet_v1 / resnet_v2 variables up to the endpoint (and block4 for the resnet_v1_101 tail); resnet_v2's
-// `postnorm` follows block4 and is never reached
-void spec_resnet(lumi_engine* e) {
-  const std::string root = "truncated_base_network/" + e->arch;
-  const bool v2 = e->resnet->preact;
-  if (v2) need_conv_bias(e, root + "/conv1", 7, 7, 3, 64);
-  else need_conv_bn(e, root + "/conv1", 7, 7, 3, 64);
-  for (int b = 0; b < 4; ++b) {
-    const int bd = BASE_DEPTH[b], depth = bd * 4;
-    for (int u = 0; u < e->resnet->units[b]; ++u) {
-      auto runs = [&](int part) { return unit_part_runs(e, b, u, part); };
-      if (!runs(UP_CONV1) && !runs(UP_SHORTCUT)) continue;
-      const int cin = u > 0 ? depth : b > 0 ? BASE_DEPTH[b - 1] * 4 : 64;
-      const std::string s = unit_scope(e, b, u);
-      if (v2)
-        for (const char* n : {"gamma", "beta", "moving_mean", "moving_variance"}) need(e, s + "/preact/" + n, {cin});
-      if (cin != depth && runs(UP_SHORTCUT)) {
-        if (v2) need_conv_bias(e, s + "/shortcut", 1, 1, cin, depth);
-        else need_conv_bn(e, s + "/shortcut", 1, 1, cin, depth);
-      }
-      if (runs(UP_CONV1)) need_conv_bn(e, s + "/conv1", 1, 1, cin, bd);
-      if (runs(UP_CONV2)) need_conv_bn(e, s + "/conv2", 3, 3, bd, bd);
-      if (runs(UP_CONV3)) {
-        if (v2) need_conv_bias(e, s + "/conv3", 1, 1, bd, depth);
-        else need_conv_bn(e, s + "/conv3", 1, 1, bd, depth);
-      }
-    }
-  }
-}
-
 const char* VGG_NAMES[5] = {"conv1", "conv2", "conv3", "conv4", "conv5"};
 const int VGG_REPS[5] = {2, 2, 3, 3, 3};
 const int VGG_CH[5] = {64, 128, 256, 512, 512};
-struct Extra { const char* name; int k, cin, cout, stride, rate, valid; };
+struct Extra { const char* name; int k, cin, cout, stride, rate, padding; };
 const Extra SSD_EXTRAS[10] = {
-    {"conv6", 3, 512, 1024, 1, 6, 0},   {"conv7", 1, 1024, 1024, 1, 1, 0}, {"conv8_1", 1, 1024, 256, 1, 1, 0},
-    {"conv8_2", 3, 256, 512, 2, 1, 0},  {"conv9_1", 1, 512, 128, 1, 1, 0}, {"conv9_2", 3, 128, 256, 2, 1, 0},
-    {"conv10_1", 1, 256, 128, 1, 1, 0}, {"conv10_2", 3, 128, 256, 1, 1, 1}, {"conv11_1", 1, 256, 128, 1, 1, 0},
-    {"conv11_2", 3, 128, 256, 1, 1, 1}};
+    {"conv6", 3, 512, 1024, 1, 6, PAD_SAME},      {"conv7", 1, 1024, 1024, 1, 1, PAD_SAME},
+    {"conv8_1", 1, 1024, 256, 1, 1, PAD_SAME},    {"conv8_2", 3, 256, 512, 2, 1, PAD_SAME},
+    {"conv9_1", 1, 512, 128, 1, 1, PAD_SAME},     {"conv9_2", 3, 128, 256, 2, 1, PAD_SAME},
+    {"conv10_1", 1, 256, 128, 1, 1, PAD_SAME},    {"conv10_2", 3, 128, 256, 1, 1, PAD_VALID},
+    {"conv11_1", 1, 256, 128, 1, 1, PAD_SAME},    {"conv11_2", 3, 128, 256, 1, 1, PAD_VALID}};
 const int SSD_FMAP_CH[6] = {512, 1024, 512, 256, 256, 256};
 
 // ---------------------------------------------------------------- config
@@ -461,29 +439,80 @@ void parse_config(lumi_engine* e) {
   }
 }
 
-void build_specs(lumi_engine* e) {
+// ---------------------------------------------------------------- layer table
+Layer& add_layer(lumi_engine* e, int kind, const std::string& key, std::vector<std::string> scopes) {
+  e->net_index[key] = e->net.size();
+  e->net.emplace_back();
+  Layer& r = e->net.back();
+  r.kind = kind; r.key = key; r.scopes = std::move(scopes);
+  return r;
+}
+
+void add_conv(lumi_engine* e, int kind, int naming, const std::string& key, std::vector<std::string> scopes,
+              std::vector<int> couts, int kh, int kw, int cin, int stride, int rate, int act, int padding) {
+  Layer& r = add_layer(e, kind, key, std::move(scopes));
+  r.naming = naming; r.couts = std::move(couts);
+  r.kh = kh; r.kw = kw; r.cin = cin; r.stride = stride; r.rate = rate; r.act = act; r.padding = padding;
+}
+
+void add_vector(lumi_engine* e, int kind, const std::string& key, const std::string& scope, int channels) {
+  add_layer(e, kind, key, {scope}).cin = channels;
+}
+
+// The layer table of the configured network, in the order of its variables.  Faster R-CNN: slim resnet_v1 / resnet_v2
+// up to the endpoint (and block4 for the resnet_v1_101 tail; resnet_v2's `postnorm` follows block4 and is never
+// reached), the RPN, the RCNN fcs and heads.  SSD: truncated VGG16, the L2-norm gamma, the extras, the multibox heads.
+void build_net(lumi_engine* e) {
   if (e->type == "fasterrcnn") {
-    spec_resnet(e);
+    const std::string root = "truncated_base_network/" + e->arch;
+    const bool v2 = e->resnet->preact;
+    // conv2d_same(64, 7, stride 2) + BN + relu (v2: + bias, no activation)
+    add_conv(e, v2 ? LK_CONV_BIAS : LK_CONV_BN, NM_SLIM, root + "/conv1", {root + "/conv1"}, {64}, 7, 7, 3, 2, 1,
+             v2 ? ACT_NONE : ACT_RELU, PAD_CONV2D_SAME);
+    add_layer(e, LK_STEM_S2D, root + "/conv1#s2d", {root + "/conv1"});
+    // bottleneck_v2: preact = relu(BN(x)); shortcut and conv3 with biases, no BN or activation; out = the raw sum
+    const int kind3 = v2 ? LK_CONV_BIAS : LK_CONV_BN;   // of the shortcut and conv3
+    for (int b = 0; b < 4; ++b) {
+      const int bd = BASE_DEPTH[b], depth = bd * 4;
+      for (int u = 0; u < e->resnet->units[b]; ++u) {
+        auto runs = [&](int part) { return unit_part_runs(e, b, u, part); };
+        if (!runs(UP_CONV1) && !runs(UP_SHORTCUT)) continue;
+        const int cin = u > 0 ? depth : b > 0 ? BASE_DEPTH[b - 1] * 4 : 64;
+        const std::string s = unit_scope(e, b, u);
+        int st = 1, rt = 1;                                   // tail: stack_blocks_dense w/o output_stride, stride 1
+        if (!(b == 3 && e->tail)) unit_stride_rate(e, b, u, st, rt);
+        if (v2) add_vector(e, LK_PREACT, s + "/preact", s + "/preact", cin);
+        if (cin != depth && runs(UP_SHORTCUT))
+          add_conv(e, kind3, NM_SLIM, s + "/shortcut", {s + "/shortcut"}, {depth}, 1, 1, cin, st, 1, ACT_NONE,
+                   PAD_SAME);
+        if (runs(UP_CONV1))
+          add_conv(e, LK_CONV_BN, NM_SLIM, s + "/conv1", {s + "/conv1"}, {bd}, 1, 1, cin, 1, 1, ACT_RELU, PAD_SAME);
+        if (runs(UP_CONV2))
+          add_conv(e, LK_CONV_BN, NM_SLIM, s + "/conv2", {s + "/conv2"}, {bd}, 3, 3, bd, st, rt, ACT_RELU,
+                   PAD_CONV2D_SAME);
+        // v1: relu applied after the residual add; a conv3 endpoint is collected before both
+        const bool conv3_ep = b == e->ep.block && u == e->ep.unit && e->ep.part == UP_CONV3;
+        if (runs(UP_CONV3))
+          add_conv(e, kind3, NM_SLIM, s + "/conv3", {s + "/conv3"}, {depth}, 1, 1, bd, 1, 1,
+                   v2 || conv3_ep ? ACT_NONE : ACT_RELU, PAD_SAME);
+      }
+    }
     const std::string r = "fasterrcnn/rpn";
-    need(e, r + "/conv/w", {e->rpn_kh, e->rpn_kw, e->ep.depth, e->rpn_channels});
-    need(e, r + "/conv/b", {e->rpn_channels});
-    need(e, r + "/cls_conv/w", {1, 1, e->rpn_channels, 2 * e->A});
-    need(e, r + "/cls_conv/b", {2 * e->A});
-    need(e, r + "/bbox_conv/w", {1, 1, e->rpn_channels, 4 * e->A});
-    need(e, r + "/bbox_conv/b", {4 * e->A});
+    add_conv(e, LK_CONV_BIAS, NM_SONNET, r + "/conv", {r + "/conv"}, {e->rpn_channels}, e->rpn_kh, e->rpn_kw,
+             e->ep.depth, 1, 1, e->rpn_act, PAD_SAME);
+    add_conv(e, LK_CONV_BIAS, NM_SONNET, r + "/heads", {r + "/cls_conv", r + "/bbox_conv"}, {2 * e->A, 4 * e->A}, 1, 1,
+             e->rpn_channels, 1, 1, ACT_NONE, PAD_SAME);
     if (e->with_rcnn) {
       int d = e->tail ? 2048 : e->ep.depth;
       if (!e->use_mean) d *= e->pooled_w * e->pooled_h;
       const std::string c = "fasterrcnn/rcnn";
       for (size_t i = 0; i < e->fc_sizes.size(); ++i) {
-        need(e, c + "/fc_" + std::to_string(i) + "/w", {d, e->fc_sizes[i]});
-        need(e, c + "/fc_" + std::to_string(i) + "/b", {e->fc_sizes[i]});
+        const std::string fc = c + "/fc_" + std::to_string(i);
+        add_conv(e, LK_CONV_BIAS, NM_LINEAR, fc, {fc}, {e->fc_sizes[i]}, 1, 1, d, 1, 1, e->fc_act, PAD_SAME);
         d = e->fc_sizes[i];
       }
-      need(e, c + "/fc_classifier/w", {d, e->num_classes + 1});
-      need(e, c + "/fc_classifier/b", {e->num_classes + 1});
-      need(e, c + "/fc_bbox/w", {d, 4 * e->num_classes});
-      need(e, c + "/fc_bbox/b", {4 * e->num_classes});
+      add_conv(e, LK_CONV_BIAS, NM_LINEAR, c + "/heads", {c + "/fc_classifier", c + "/fc_bbox"},
+               {e->num_classes + 1, 4 * e->num_classes}, 1, 1, d, 1, 1, ACT_NONE, PAD_SAME);
     }
   } else {
     const std::string s = "ssd/ssd_feature_extractor";
@@ -491,21 +520,50 @@ void build_specs(lumi_engine* e) {
     for (int b = 0; b < 5; ++b)
       for (int r = 0; r < VGG_REPS[b]; ++r) {
         const std::string p = s + "/vgg_16/" + VGG_NAMES[b] + "/" + VGG_NAMES[b] + "_" + std::to_string(r + 1);
-        need(e, p + "/weights", {3, 3, cin, VGG_CH[b]});
-        need(e, p + "/biases", {VGG_CH[b]});
+        add_conv(e, LK_CONV_BIAS, NM_SLIM, p, {p}, {VGG_CH[b]}, 3, 3, cin, 1, 1, ACT_RELU, PAD_SAME);
+        if (b == 0 && r == 0) add_layer(e, LK_CONV1_1_PACK, p + "#pack", {p});
         cin = VGG_CH[b];
       }
-    need(e, s + "/conv_4_3_norm/gamma", {1, 1, 1, 512});
+    add_vector(e, LK_GAMMA, "gamma", s + "/conv_4_3_norm", 512);
     for (const Extra& x : SSD_EXTRAS) {
-      need(e, s + "/extra_feature_layers/" + x.name + "/w", {x.k, x.k, x.cin, x.cout});
-      need(e, s + "/extra_feature_layers/" + x.name + "/b", {x.cout});
+      const std::string p = s + "/extra_feature_layers/" + x.name;
+      add_conv(e, LK_CONV_BIAS, NM_SONNET, p, {p}, {x.cout}, x.k, x.k, x.cin, x.stride, x.rate, ACT_RELU, x.padding);
     }
     for (int i = 0; i < 6; ++i) {
       const std::string n = "ssd/MultiBox_" + std::to_string(i);
-      need(e, n + "_offsets_conv/w", {3, 3, SSD_FMAP_CH[i], 4 * e->ssd_app[i]});
-      need(e, n + "_offsets_conv/b", {4 * e->ssd_app[i]});
-      need(e, n + "_classes_conv/w", {3, 3, SSD_FMAP_CH[i], (e->num_classes + 1) * e->ssd_app[i]});
-      need(e, n + "_classes_conv/b", {(e->num_classes + 1) * e->ssd_app[i]});
+      add_conv(e, LK_CONV_BIAS, NM_SONNET, n, {n + "_offsets_conv", n + "_classes_conv"},
+               {4 * e->ssd_app[i], (e->num_classes + 1) * e->ssd_app[i]}, 3, 3, SSD_FMAP_CH[i], 1, 1, ACT_NONE,
+               PAD_SAME);
+    }
+  }
+}
+
+Layer& layer(lumi_engine* e, const std::string& key) {
+  auto it = e->net_index.find(key);
+  if (it == e->net_index.end()) throw Error(LUMI_ESTATE, "layer '" + key + "' missing (internal)");
+  return e->net[it->second];
+}
+
+const char* BN_VARS[4] = {"gamma", "beta", "moving_mean", "moving_variance"};
+std::string weights_var(const Layer& r, size_t i) { return r.scopes[i] + (r.naming == NM_SLIM ? "/weights" : "/w"); }
+std::string biases_var(const Layer& r, size_t i) { return r.scopes[i] + (r.naming == NM_SLIM ? "/biases" : "/b"); }
+
+void build_specs(lumi_engine* e) {
+  auto need = [e](const std::string& name, std::vector<int64_t> shape) { e->required.push_back({name, shape}); };
+  for (const Layer& r : e->net) {
+    if (r.kind == LK_CONV_BN) {
+      need(weights_var(r, 0), {r.kh, r.kw, r.cin, r.couts[0]});
+      for (const char* n : BN_VARS) need(r.scopes[0] + "/BatchNorm/" + n, {r.couts[0]});
+    } else if (r.kind == LK_CONV_BIAS) {
+      for (size_t i = 0; i < r.scopes.size(); ++i) {
+        if (r.naming == NM_LINEAR) need(weights_var(r, i), {r.cin, r.couts[i]});
+        else need(weights_var(r, i), {r.kh, r.kw, r.cin, r.couts[i]});
+        need(biases_var(r, i), {r.couts[i]});
+      }
+    } else if (r.kind == LK_PREACT) {
+      for (const char* n : BN_VARS) need(r.scopes[0] + "/" + n, {r.cin});
+    } else if (r.kind == LK_GAMMA) {
+      need(r.scopes[0] + "/gamma", {1, 1, 1, r.cin});
     }
   }
 }
@@ -518,11 +576,12 @@ const HostTensor& W(lumi_engine* e, const std::string& name) {
 }
 
 // conv + folded inference BN (slim batch_norm, eps 1e-5): y = conv*s + (beta - mean*s), s = gamma/sqrt(var+eps)
-void make_conv_bn(lumi_engine* e, const std::string& scope, int stride, int rate, int act) {
+void make_conv_bn(lumi_engine* e, Layer& r) {
+  const std::string& scope = r.scopes[0];
   const HostTensor& w = W(e, scope + "/weights");
   ConvLayer L;
   L.kh = (int)w.shape[0]; L.kw = (int)w.shape[1]; L.cin = (int)w.shape[2]; L.cout = (int)w.shape[3];
-  L.stride = stride; L.rate = rate; L.act = act;
+  L.stride = r.stride; L.rate = r.rate; L.act = r.act;
   const HostTensor& g = W(e, scope + "/BatchNorm/gamma");
   const HostTensor& b = W(e, scope + "/BatchNorm/beta");
   const HostTensor& m = W(e, scope + "/BatchNorm/moving_mean");
@@ -534,47 +593,44 @@ void make_conv_bn(lumi_engine* e, const std::string& scope, int stride, int rate
     bi[c] = (float)((double)b.v[c] - (double)m.v[c] * s);
   }
   conv_layer_upload(L, w.v.data(), sc.data(), bi.data());
-  e->layers[scope] = L;
+  r.conv = L;
 }
 
-// conv + bias (Sonnet / slim-VGG), optionally fusing several same-input convs along C_out
-void make_conv_bias(lumi_engine* e, const std::string& key, const std::vector<std::string>& wnames,
-                    const std::vector<std::string>& bnames, int stride, int rate, int act) {
-  const HostTensor& w0 = W(e, wnames[0]);
+// conv + bias (Sonnet / slim-VGG), fusing the convs of several same-input scopes along C_out
+void make_conv_bias(lumi_engine* e, Layer& r) {
+  const HostTensor& w0 = W(e, weights_var(r, 0));
   const bool linear = w0.shape.size() == 2;
   ConvLayer L;
   L.kh = linear ? 1 : (int)w0.shape[0]; L.kw = linear ? 1 : (int)w0.shape[1];
   L.cin = linear ? (int)w0.shape[0] : (int)w0.shape[2];
-  L.stride = stride; L.rate = rate; L.act = act;
+  L.stride = r.stride; L.rate = r.rate; L.act = r.act;
   int cout = 0;
-  for (const auto& n : wnames) cout += (int)W(e, n).shape.back();
+  for (size_t i = 0; i < r.scopes.size(); ++i) cout += (int)W(e, weights_var(r, i)).shape.back();
   L.cout = cout;
   const size_t kdim = (size_t)L.kh * L.kw * L.cin;
   std::vector<float> w(kdim * cout), b(cout, 0.f);
   int off = 0;
-  for (size_t i = 0; i < wnames.size(); ++i) {
-    const HostTensor& wi = W(e, wnames[i]);
+  for (size_t i = 0; i < r.scopes.size(); ++i) {
+    const HostTensor& wi = W(e, weights_var(r, i));
     const int co = (int)wi.shape.back();
-    LUMI_REQUIRE(wi.v.size() == kdim * co, "fused conv '" + key + "': weight shapes disagree");
+    LUMI_REQUIRE(wi.v.size() == kdim * co, "fused conv '" + r.key + "': weight shapes disagree");
     for (size_t k = 0; k < kdim; ++k) std::memcpy(&w[k * cout + off], &wi.v[k * co], co * sizeof(float));
-    if (i < bnames.size() && !bnames[i].empty()) {
-      const HostTensor& bi = W(e, bnames[i]);
-      std::memcpy(&b[off], bi.v.data(), co * sizeof(float));
-    }
+    std::memcpy(&b[off], W(e, biases_var(r, i)).v.data(), co * sizeof(float));
     off += co;
   }
   conv_layer_upload(L, w.data(), nullptr, b.data());
-  e->layers[key] = L;
+  r.conv = L;
 }
 
 // resnet_v2 `preact` batch norm (slim batch_norm, eps 1e-5) folded like make_conv_bn, as the device vectors
-// <scope>/preact#scale and #bias that the producing conv epilogue (or the stem's max pool) applies; padded to a
+// <unit>/preact#scale and #bias that the producing conv epilogue (or the stem's max pool) applies; padded to a
 // multiple of 128 channels for the tensor-core epilogue's vector loads
-void make_preact(lumi_engine* e, const std::string& scope) {
-  const HostTensor& g = W(e, scope + "/preact/gamma");
-  const HostTensor& b = W(e, scope + "/preact/beta");
-  const HostTensor& m = W(e, scope + "/preact/moving_mean");
-  const HostTensor& v = W(e, scope + "/preact/moving_variance");
+void make_preact(lumi_engine* e, const Layer& r) {
+  const std::string& scope = r.scopes[0];
+  const HostTensor& g = W(e, scope + "/gamma");
+  const HostTensor& b = W(e, scope + "/beta");
+  const HostTensor& m = W(e, scope + "/moving_mean");
+  const HostTensor& v = W(e, scope + "/moving_variance");
   const int c = (int)g.v.size(), cpad = cdiv(c, 128) * 128;
   std::vector<float> sc(cpad, 0.f), bi(cpad, 0.f);
   for (int i = 0; i < c; ++i) {
@@ -585,121 +641,68 @@ void make_preact(lumi_engine* e, const std::string& scope) {
   for (int k = 0; k < 2; ++k) {
     float* d = nullptr;
     LUMI_CUDA_CHECK(cudaMalloc(&d, cpad * sizeof(float)));
-    e->dev_vecs[scope + (k ? "/preact#bias" : "/preact#scale")] = d;
+    e->dev_vecs[r.key + (k ? "#bias" : "#scale")] = d;
     LUMI_CUDA_CHECK(cudaMemcpy(d, (k ? bi : sc).data(), cpad * sizeof(float), cudaMemcpyHostToDevice));
   }
 }
 
-void build_layers(lumi_engine* e) {
-  if (e->type == "fasterrcnn") {
-    const std::string root = "truncated_base_network/" + e->arch;
-    const int* units = e->resnet->units;
-    const bool v2 = e->resnet->preact;
-    if (v2) make_conv_bias(e, root + "/conv1", {root + "/conv1/weights"}, {root + "/conv1/biases"}, 2, 1, ACT_NONE);
-    else make_conv_bn(e, root + "/conv1", 2, 1, ACT_RELU);
-    {   // tensor-core form of the stem: 7x7/2 over 3 channels == 4x4/1 over the 12(+4 pad)-channel
-        // space-to-depth input; one filter row r' = 4 taps x 16 ch = one K=64 slice  (kh=4, kw=1, cin=64)
-      const HostTensor& w = W(e, root + "/conv1/weights");
-      const ConvLayer& base = e->layers.at(root + "/conv1");
-      std::vector<float> w2((size_t)4 * 64 * 64, 0.f);
-      for (int rp = 0; rp < 4; ++rp)
-        for (int sp = 0; sp < 4; ++sp)
-          for (int dy = 0; dy < 2; ++dy)
-            for (int dx = 0; dx < 2; ++dx) {
-              const int r = 2 * rp + dy, sx = 2 * sp + dx;
-              if (r >= 7 || sx >= 7) continue;
-              for (int c = 0; c < 3; ++c)
-                for (int co = 0; co < 64; ++co)
-                  w2[((size_t)rp * 64 + sp * 16 + dy * 6 + dx * 3 + c) * 64 + co] = w.v[(((size_t)r * 7 + sx) * 3 + c) * 64 + co];
-            }
-      std::vector<float> sc(64), bi(64);
-      LUMI_CUDA_CHECK(cudaMemcpy(sc.data(), base.scale, 64 * sizeof(float), cudaMemcpyDeviceToHost));
-      LUMI_CUDA_CHECK(cudaMemcpy(bi.data(), base.bias, 64 * sizeof(float), cudaMemcpyDeviceToHost));
-      ConvLayer L;
-      L.kh = 4; L.kw = 1; L.cin = 64; L.cout = 64; L.stride = 1; L.rate = 1; L.act = base.act;
-      conv_layer_upload(L, w2.data(), sc.data(), bi.data());
-      e->layers[root + "/conv1#s2d"] = L;
-    }
-    for (int b = 0; b < 4; ++b) {
-      const int bd = BASE_DEPTH[b], depth = bd * 4;
-      for (int u = 0; u < units[b]; ++u) {
-        auto runs = [&](int part) { return unit_part_runs(e, b, u, part); };
-        if (!runs(UP_CONV1) && !runs(UP_SHORTCUT)) continue;
-        const int cin = u > 0 ? depth : b > 0 ? BASE_DEPTH[b - 1] * 4 : 64;
-        const std::string s = unit_scope(e, b, u);
-        int st = 1, rt = 1;                                   // tail: stack_blocks_dense w/o output_stride, stride 1
-        if (!(b == 3 && e->tail)) unit_stride_rate(e, b, u, st, rt);
-        if (v2) {
-          // bottleneck_v2: preact = relu(BN(x)); shortcut and conv3 with biases, no BN or activation; out = the raw sum
-          make_preact(e, s);
-          if (cin != depth && runs(UP_SHORTCUT))
-            make_conv_bias(e, s + "/shortcut", {s + "/shortcut/weights"}, {s + "/shortcut/biases"}, st, 1, ACT_NONE);
-          if (runs(UP_CONV1)) make_conv_bn(e, s + "/conv1", 1, 1, ACT_RELU);
-          if (runs(UP_CONV2)) make_conv_bn(e, s + "/conv2", st, rt, ACT_RELU);
-          if (runs(UP_CONV3))
-            make_conv_bias(e, s + "/conv3", {s + "/conv3/weights"}, {s + "/conv3/biases"}, 1, 1, ACT_NONE);
-        } else {
-          if (cin != depth && runs(UP_SHORTCUT)) make_conv_bn(e, s + "/shortcut", st, 1, ACT_NONE);
-          if (runs(UP_CONV1)) make_conv_bn(e, s + "/conv1", 1, 1, ACT_RELU);
-          if (runs(UP_CONV2)) make_conv_bn(e, s + "/conv2", st, rt, ACT_RELU);
-          // relu applied after the residual add; a conv3 endpoint is collected before both
-          const bool conv3_ep = b == e->ep.block && u == e->ep.unit && e->ep.part == UP_CONV3;
-          if (runs(UP_CONV3)) make_conv_bn(e, s + "/conv3", 1, 1, conv3_ep ? ACT_NONE : ACT_RELU);
-        }
-      }
-    }
-    const std::string r = "fasterrcnn/rpn";
-    make_conv_bias(e, r + "/conv", {r + "/conv/w"}, {r + "/conv/b"}, 1, 1, e->rpn_act);
-    make_conv_bias(e, r + "/heads", {r + "/cls_conv/w", r + "/bbox_conv/w"}, {r + "/cls_conv/b", r + "/bbox_conv/b"}, 1,
-                   1, ACT_NONE);
-    if (e->with_rcnn) {
-      const std::string c = "fasterrcnn/rcnn";
-      for (size_t i = 0; i < e->fc_sizes.size(); ++i)
-        make_conv_bias(e, c + "/fc_" + std::to_string(i), {c + "/fc_" + std::to_string(i) + "/w"},
-                       {c + "/fc_" + std::to_string(i) + "/b"}, 1, 1, e->fc_act);
-      make_conv_bias(e, c + "/heads", {c + "/fc_classifier/w", c + "/fc_bbox/w"},
-                     {c + "/fc_classifier/b", c + "/fc_bbox/b"}, 1, 1, ACT_NONE);
-    }
-  } else {
-    const std::string s = "ssd/ssd_feature_extractor";
-    for (int b = 0; b < 5; ++b)
-      for (int r = 0; r < VGG_REPS[b]; ++r) {
-        const std::string p = s + "/vgg_16/" + VGG_NAMES[b] + "/" + VGG_NAMES[b] + "_" + std::to_string(r + 1);
-        make_conv_bias(e, p, {p + "/weights"}, {p + "/biases"}, 1, 1, ACT_RELU);
-      }
-    {   // tensor-core form of conv1_1 (3x3 over 3 channels): one filter row = 4 pixels x 16 ch = one K=64 slice
-        // (kh=3, kw=1, cin=64) over the padded 16-channel staging written by launch_pack_c3
-      const std::string p = s + "/vgg_16/conv1/conv1_1";
-      const HostTensor& w = W(e, p + "/weights");
-      const HostTensor& b = W(e, p + "/biases");
-      const int co_n = (int)w.shape[3];
-      LUMI_REQUIRE(w.shape[0] == 3 && w.shape[1] == 3 && w.shape[2] == 3, "conv1_1 must be 3x3x3");
-      std::vector<float> w2((size_t)3 * 64 * co_n, 0.f);
-      for (int r = 0; r < 3; ++r)
-        for (int sx = 0; sx < 3; ++sx)
+// tensor-core form of the resnet stem: 7x7/2 over 3 channels == 4x4/1 over the 12(+4 pad)-channel space-to-depth
+// input; one filter row r' = 4 taps x 16 ch = one K=64 slice  (kh=4, kw=1, cin=64)
+void make_stem_s2d(lumi_engine* e, Layer& r) {
+  const HostTensor& w = W(e, r.scopes[0] + "/weights");
+  const ConvLayer& base = layer(e, r.scopes[0]).conv;
+  std::vector<float> w2((size_t)4 * 64 * 64, 0.f);
+  for (int rp = 0; rp < 4; ++rp)
+    for (int sp = 0; sp < 4; ++sp)
+      for (int dy = 0; dy < 2; ++dy)
+        for (int dx = 0; dx < 2; ++dx) {
+          const int ry = 2 * rp + dy, sx = 2 * sp + dx;
+          if (ry >= 7 || sx >= 7) continue;
           for (int c = 0; c < 3; ++c)
-            for (int co = 0; co < co_n; ++co)
-              w2[((size_t)r * 64 + sx * 16 + c) * co_n + co] = w.v[(((size_t)r * 3 + sx) * 3 + c) * co_n + co];
-      ConvLayer L;
-      L.kh = 3; L.kw = 1; L.cin = 64; L.cout = co_n; L.stride = 1; L.rate = 1; L.act = ACT_RELU;
-      conv_layer_upload(L, w2.data(), nullptr, b.v.data());
-      e->layers[p + "#pack"] = L;
-    }
-    {
-      const HostTensor& g = W(e, s + "/conv_4_3_norm/gamma");
+            for (int co = 0; co < 64; ++co)
+              w2[((size_t)rp * 64 + sp * 16 + dy * 6 + dx * 3 + c) * 64 + co] = w.v[(((size_t)ry * 7 + sx) * 3 + c) * 64 + co];
+        }
+  std::vector<float> sc(64), bi(64);
+  LUMI_CUDA_CHECK(cudaMemcpy(sc.data(), base.scale, 64 * sizeof(float), cudaMemcpyDeviceToHost));
+  LUMI_CUDA_CHECK(cudaMemcpy(bi.data(), base.bias, 64 * sizeof(float), cudaMemcpyDeviceToHost));
+  ConvLayer L;
+  L.kh = 4; L.kw = 1; L.cin = 64; L.cout = 64; L.stride = 1; L.rate = 1; L.act = base.act;
+  conv_layer_upload(L, w2.data(), sc.data(), bi.data());
+  r.conv = L;
+}
+
+// tensor-core form of SSD's conv1_1 (3x3 over 3 channels): one filter row = 4 pixels x 16 ch = one K=64 slice
+// (kh=3, kw=1, cin=64) over the padded 16-channel staging written by launch_pack_c3
+void make_conv1_1_pack(lumi_engine* e, Layer& r) {
+  const HostTensor& w = W(e, r.scopes[0] + "/weights");
+  const HostTensor& b = W(e, r.scopes[0] + "/biases");
+  const int co_n = (int)w.shape[3];
+  LUMI_REQUIRE(w.shape[0] == 3 && w.shape[1] == 3 && w.shape[2] == 3, "conv1_1 must be 3x3x3");
+  std::vector<float> w2((size_t)3 * 64 * co_n, 0.f);
+  for (int ry = 0; ry < 3; ++ry)
+    for (int sx = 0; sx < 3; ++sx)
+      for (int c = 0; c < 3; ++c)
+        for (int co = 0; co < co_n; ++co)
+          w2[((size_t)ry * 64 + sx * 16 + c) * co_n + co] = w.v[(((size_t)ry * 3 + sx) * 3 + c) * co_n + co];
+  ConvLayer L;
+  L.kh = 3; L.kw = 1; L.cin = 64; L.cout = co_n; L.stride = 1; L.rate = 1; L.act = ACT_RELU;
+  conv_layer_upload(L, w2.data(), nullptr, b.v.data());
+  r.conv = L;
+}
+
+void build_layers(lumi_engine* e) {
+  for (Layer& r : e->net) {
+    if (r.kind == LK_CONV_BN) make_conv_bn(e, r);
+    else if (r.kind == LK_CONV_BIAS) make_conv_bias(e, r);
+    else if (r.kind == LK_PREACT) make_preact(e, r);
+    else if (r.kind == LK_STEM_S2D) make_stem_s2d(e, r);
+    else if (r.kind == LK_CONV1_1_PACK) make_conv1_1_pack(e, r);
+    else if (r.kind == LK_GAMMA) {
+      const HostTensor& g = W(e, r.scopes[0] + "/gamma");
       float* d = nullptr;
       LUMI_CUDA_CHECK(cudaMalloc(&d, g.v.size() * sizeof(float)));
       LUMI_CUDA_CHECK(cudaMemcpy(d, g.v.data(), g.v.size() * sizeof(float), cudaMemcpyHostToDevice));
-      e->dev_vecs["gamma"] = d;
-    }
-    for (const Extra& x : SSD_EXTRAS) {
-      const std::string p = s + "/extra_feature_layers/" + x.name;
-      make_conv_bias(e, p, {p + "/w"}, {p + "/b"}, x.stride, x.rate, ACT_RELU);
-    }
-    for (int i = 0; i < 6; ++i) {
-      const std::string n = "ssd/MultiBox_" + std::to_string(i);
-      make_conv_bias(e, n, {n + "_offsets_conv/w", n + "_classes_conv/w"}, {n + "_offsets_conv/b", n + "_classes_conv/b"},
-                     1, 1, ACT_NONE);
+      e->dev_vecs[r.key] = d;
     }
   }
 }
@@ -808,19 +811,17 @@ PreAct preact_of(lumi_engine* e, const std::string& unit, bool keep_x) {
   return pa;
 }
 
-// padding: 0 VALID, 1 SAME, 2 slim conv2d_same (explicit pad + VALID when stride > 1)
-Act run_conv(Ctx& cx, const std::string& key, Act in, int padding, const Act* res, int res_stride, float** out_f32,
+Act run_conv(Ctx& cx, const std::string& key, Act in, const Act* res, int res_stride, float** out_f32,
              const long* view_pitch = nullptr, double algorithmic_flops = -1.0, PreAct* pre = nullptr) {
-  auto it = cx.e->layers.find(key);
-  if (it == cx.e->layers.end()) throw Error(LUMI_ESTATE, "layer '" + key + "' missing (internal)");
-  const ConvLayer& L = it->second;
+  const Layer& R = layer(cx.e, key);
+  const ConvLayer& L = R.conv;
   ConvIO io;
   io.in = in;
   int ho, wo, pt = 0, pl = 0;
-  if (padding == 1 || (padding == 2 && L.stride == 1)) {
+  if (R.padding == PAD_SAME || (R.padding == PAD_CONV2D_SAME && L.stride == 1)) {
     tf_same(in.h, L.kh, L.stride, L.rate, ho, pt);
     tf_same(in.w, L.kw, L.stride, L.rate, wo, pl);
-  } else if (padding == 2) {
+  } else if (R.padding == PAD_CONV2D_SAME) {
     const int keff = L.kh + (L.kh - 1) * (L.rate - 1);
     pt = pl = (keff - 1) / 2;
     ho = (in.h + (keff - 1) - keff) / L.stride + 1;
@@ -882,38 +883,24 @@ Act run_pool(Ctx& cx, Act in, int k, int stride, bool same, const PreAct* pre = 
   return out;
 }
 
-// slim bottleneck_v1; `stop` (a UnitPart) returns that collected conv output instead of the unit's
-Act bottleneck(Ctx& cx, const std::string& s, Act x, int depth, int stop = UP_UNIT) {
-  if (stop == UP_SHORTCUT) return run_conv(cx, s + "/shortcut", x, 1, nullptr, 1, nullptr);
-  Act shortcut = x;
-  int res_stride = 1;
-  if (stop == UP_UNIT) {
-    res_stride = cx.e->layers.at(s + "/conv2").stride;
-    if (x.c != depth) { shortcut = run_conv(cx, s + "/shortcut", x, 1, nullptr, 1, nullptr); res_stride = 1; }
-  }
-  Act r = run_conv(cx, s + "/conv1", x, 1, nullptr, 1, nullptr);
-  if (stop == UP_CONV1) return r;
-  r = run_conv(cx, s + "/conv2", r, 2, nullptr, 1, nullptr);
-  if (stop == UP_CONV2) return r;
-  return run_conv(cx, s + "/conv3", r, 1, stop == UP_UNIT ? &shortcut : nullptr, res_stride, nullptr);
-}
-
 // slim bottleneck_v2 on (x, p = relu(BN_preact(x))); x may be absent when the unit projects its shortcut from p.
+// A slim bottleneck_v1 unit is the same computation with p = x and no `next`.
 // conv3 writes what the next unit reads, from `next` (nullptr: the endpoint, x only): p always, and x as well when
-// that unit's shortcut is the identity (its depth equals this unit's).  `stop` as in bottleneck().
+// that unit's shortcut is the identity (its depth equals this unit's).  `stop` (a UnitPart) returns that collected
+// conv output instead of the unit's.
 Act bottleneck_v2(Ctx& cx, const std::string& s, Act x, Act p, int depth, PreAct* next, int stop = UP_UNIT) {
-  if (stop == UP_SHORTCUT) return run_conv(cx, s + "/shortcut", p, 1, nullptr, 1, nullptr);
+  if (stop == UP_SHORTCUT) return run_conv(cx, s + "/shortcut", p, nullptr, 1, nullptr);
   Act shortcut = x;
   int res_stride = 1;
   if (stop == UP_UNIT) {
-    res_stride = cx.e->layers.at(s + "/conv2").stride;   // subsample(x, stride)
-    if (p.c != depth) { shortcut = run_conv(cx, s + "/shortcut", p, 1, nullptr, 1, nullptr); res_stride = 1; }
+    res_stride = layer(cx.e, s + "/conv2").stride;   // subsample(x, stride)
+    if (p.c != depth) { shortcut = run_conv(cx, s + "/shortcut", p, nullptr, 1, nullptr); res_stride = 1; }
   }
-  Act r = run_conv(cx, s + "/conv1", p, 1, nullptr, 1, nullptr);
+  Act r = run_conv(cx, s + "/conv1", p, nullptr, 1, nullptr);
   if (stop == UP_CONV1) return r;
-  r = run_conv(cx, s + "/conv2", r, 2, nullptr, 1, nullptr);
+  r = run_conv(cx, s + "/conv2", r, nullptr, 1, nullptr);
   if (stop == UP_CONV2) return r;
-  return run_conv(cx, s + "/conv3", r, 1, stop == UP_UNIT ? &shortcut : nullptr, res_stride, nullptr, nullptr, -1.0,
+  return run_conv(cx, s + "/conv3", r, stop == UP_UNIT ? &shortcut : nullptr, res_stride, nullptr, nullptr, -1.0,
                   next);
 }
 
@@ -964,11 +951,11 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
     Act view = x2;                      // Toeplitz view: pixel (y, x) -> the 64 contiguous fp16 starting at x2[y][x]
     view.w = wo; view.c = 64;
     const long pitch[3] = {16, (long)(wo + 3) * 16, (long)(ho + 3) * (wo + 3) * 16};
-    x = run_conv(cx, root + "/conv1#s2d", view, 0, nullptr, 1, nullptr, pitch, 2.0 * n * ho * wo * 147.0 * 64.0);
+    x = run_conv(cx, root + "/conv1#s2d", view, nullptr, 1, nullptr, pitch, 2.0 * n * ho * wo * 147.0 * 64.0);
   } else {
     x = cx.act(n, h, w, 3);
     if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_u8_to_act(images, cx.img_f32, x, RGB_MEANS, cx.st); }  // base_network.py:153-177
-    x = run_conv(cx, root + "/conv1", x, 2, nullptr, 1, nullptr);        // conv2d_same(64, 7, stride 2) + BN + relu
+    x = run_conv(cx, root + "/conv1", x, nullptr, 1, nullptr);           // conv2d_same(64, 7, stride 2) + BN + relu
   }                                                                      // (v2: + bias, no activation)
   const Endpoint& ep = e->ep;
   if (ep.block < 0) {
@@ -978,7 +965,7 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
     for (int b = 0; b <= ep.block; ++b)
       for (int u = 0; u < units[b]; ++u) {
         const bool at_ep = b == ep.block && u == ep.unit;
-        x = bottleneck(cx, unit_scope(e, b, u), x, BASE_DEPTH[b] * 4, at_ep ? ep.part : UP_UNIT);
+        x = bottleneck_v2(cx, unit_scope(e, b, u), x, x, BASE_DEPTH[b] * 4, nullptr, at_ep ? ep.part : UP_UNIT);
         if (at_ep) break;
       }
   } else {
@@ -1010,9 +997,9 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
   cx.tap_f32("all_anchors", e->d_anchors, na, 4, 1, 1);
 
   // RPN (rpn.py:136-180): 3x3 conv + act, fused 1x1 heads [cls 2A | bbox 4A], softmax fused into the decode
-  Act rf = run_conv(cx, "fasterrcnn/rpn/conv", fmap, 1, nullptr, 1, nullptr);
+  Act rf = run_conv(cx, "fasterrcnn/rpn/conv", fmap, nullptr, 1, nullptr);
   float* heads = nullptr;
-  run_conv(cx, "fasterrcnn/rpn/heads", rf, 1, nullptr, 1, &heads);
+  run_conv(cx, "fasterrcnn/rpn/heads", rf, nullptr, 1, &heads);
   const int hc = 6 * e->A;
   cx.tap_f32("rpn_heads", heads, n, fh * fw, hc, 1);
 
@@ -1072,7 +1059,8 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
     feat = pooled;
     if (e->tail)                                                         // truncated_base_network.py:56-95
       for (int u = 0; u < 3; ++u)
-        feat = bottleneck(cx, root + "/block4/unit_" + std::to_string(u + 1) + "/bottleneck_v1", feat, 2048);
+        feat = bottleneck_v2(cx, root + "/block4/unit_" + std::to_string(u + 1) + "/bottleneck_v1", feat, feat, 2048,
+                             nullptr);
     if (e->use_mean) {
       Act m = cx.act(feat.n, 1, 1, feat.c);
       if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_HEAD_MISC); launch_spatial_mean(feat, m, cx.st); }
@@ -1083,9 +1071,9 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
   }
   cx.tap_act("rcnn_features", feat);
   for (size_t i = 0; i < e->fc_sizes.size(); ++i)
-    feat = run_conv(cx, "fasterrcnn/rcnn/fc_" + std::to_string(i), feat, 1, nullptr, 1, nullptr);
+    feat = run_conv(cx, "fasterrcnn/rcnn/fc_" + std::to_string(i), feat, nullptr, 1, nullptr);
   float* fc = nullptr;
-  run_conv(cx, "fasterrcnn/rcnn/heads", feat, 1, nullptr, 1, &fc);
+  run_conv(cx, "fasterrcnn/rcnn/heads", feat, nullptr, 1, &fc);
   const int C = e->num_classes, fcw = 5 * C + 1;
   float* cls_prob = cx.f32((size_t)n * post * (C + 1));
   if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_HEAD_MISC); launch_softmax_rows(fc, cls_prob, n * post, C + 1, fcw, cx.st); }
@@ -1182,7 +1170,7 @@ void forward_ssd(Ctx& cx, const void* images, int n, int h, int w) {
     Act view = x2;
     view.w = w; view.c = 64;
     const long pitch[3] = {16, (long)(w + 3) * 16, (long)(h + 2) * (w + 3) * 16};
-    x = run_conv(cx, s + "/vgg_16/conv1/conv1_1#pack", view, 0, nullptr, 1, nullptr, pitch, 2.0 * n * h * w * 27.0 * 64.0);
+    x = run_conv(cx, s + "/vgg_16/conv1/conv1_1#pack", view, nullptr, 1, nullptr, pitch, 2.0 * n * h * w * 27.0 * 64.0);
   } else {
     x = cx.act(n, h, w, 3);
     if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_u8_to_act(images, cx.img_f32, x, nullptr, cx.st); }  // no mean subtraction (quirk Q7)
@@ -1190,8 +1178,8 @@ void forward_ssd(Ctx& cx, const void* images, int n, int h, int w) {
   Act fmaps[6];
   for (int b = 0; b < 5; ++b) {
     for (int r = (b == 0 && c11_tc) ? 1 : 0; r < VGG_REPS[b]; ++r)
-      x = run_conv(cx, s + "/vgg_16/" + VGG_NAMES[b] + "/" + VGG_NAMES[b] + "_" + std::to_string(r + 1), x, 1, nullptr,
-                   1, nullptr);
+      x = run_conv(cx, s + "/vgg_16/" + VGG_NAMES[b] + "/" + VGG_NAMES[b] + "_" + std::to_string(r + 1), x, nullptr, 1,
+                   nullptr);
     if (b == 3) {                                                         // conv4_3 -> l2norm x gamma
       Act nrm = cx.act(x.n, x.h, x.w, x.c);
       if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_HEAD_MISC); launch_l2norm_scale(x, nrm, e->dev_vecs.at("gamma"), 1e-12f, cx.st); }
@@ -1203,7 +1191,7 @@ void forward_ssd(Ctx& cx, const void* images, int n, int h, int w) {
   const std::string ex = s + "/extra_feature_layers/";
   int fi = 1;
   for (int i = 0; i < 10; ++i) {
-    x = run_conv(cx, ex + SSD_EXTRAS[i].name, x, SSD_EXTRAS[i].valid ? 0 : 1, nullptr, 1, nullptr);
+    x = run_conv(cx, ex + SSD_EXTRAS[i].name, x, nullptr, 1, nullptr);
     if (i == 1 || i == 3 || i == 5 || i == 7 || i == 9) fmaps[fi++] = x;
   }
   const int C1 = e->num_classes + 1, total = e->ssd_total_anchors;
@@ -1213,7 +1201,7 @@ void forward_ssd(Ctx& cx, const void* images, int n, int h, int w) {
   for (int i = 0; i < 6; ++i) {
     cx.tap_act("fmap_" + std::to_string(i), fmaps[i]);
     float* head = nullptr;
-    Act o = run_conv(cx, "ssd/MultiBox_" + std::to_string(i), fmaps[i], 1, nullptr, 1, &head);
+    Act o = run_conv(cx, "ssd/MultiBox_" + std::to_string(i), fmaps[i], nullptr, 1, &head);
     const int A = e->ssd_app[i], cells = o.h * o.w, per_cell = A * (4 + C1);
     if (!cx.dry) {
       ProfScope ps(cx.e, cx.dry, PC_HEAD_MISC);
@@ -1329,6 +1317,7 @@ int lumi_create(const char* cfg_json, int device, int max_batch, int max_h, int 
   eng->device = device; eng->max_batch = max_batch; eng->max_h = max_h; eng->max_w = max_w;
   parse_config(eng.get());
   if (eng->type == "ssd") compute_ssd_anchors(eng.get());
+  build_net(eng.get());
   build_specs(eng.get());
   int ndev = lumi_device_count();
   if (ndev <= 0) throw Error(LUMI_ECUDA, "no CUDA device visible: the luminoth_b200 engine has no CPU fallback");
