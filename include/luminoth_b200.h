@@ -225,6 +225,12 @@ int lumi_op_roi_pool_batched(const float* fmap, int n, int fh, int fw, int c, co
  * for pooled features that did not fuse the mean: x [r,h,w,c] fp32 on DEVICE (split into planes first), y [r,c]. */
 int lumi_op_spatial_mean(const float* x, int r, int h, int w, int c, float* y, void* stream);
 
+/* SSD's conv4_3 normalisation, tf.nn.l2_normalize over channels x gamma (ssd/feature_extractor.py:62-76), through
+ * split planes as the engine runs it: y = x / sqrt(max(sum_c x^2, eps)) * gamma[c].  x, y [n,h,w,c] fp32 and gamma
+ * [c] on DEVICE.  The output planes start out as NaN, so an element the kernel skips reads back as NaN. */
+int lumi_op_l2norm_scale(const float* x, int n, int h, int w, int c, const float* gamma, float eps, float* y,
+                         void* stream);
+
 /* Softmax over the first cols entries of each of rows rows of x (in_stride floats apart, >= cols); y [rows,cols]
  * dense.  The engine reads the C + 1 class logits out of fc rows 5C + 1 wide.  DEVICE pointers. */
 int lumi_op_softmax_rows(const float* x, int rows, int cols, int in_stride, float* y, void* stream);

@@ -305,6 +305,23 @@ int lumi_op_spatial_mean(const float* x, int r, int h, int w, int c, float* y, v
   OP_END
 }
 
+int lumi_op_l2norm_scale(const float* x, int n, int h, int w, int c, const float* gamma, float eps, float* y,
+                         void* stream) {
+  OP_BEGIN
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  LUMI_REQUIRE(n > 0 && h > 0 && w > 0 && c > 0, "l2norm_scale: sizes must be positive");
+  LUMI_REQUIRE(gamma, "l2norm_scale: gamma is required");
+  ActBuf in(n, h, w, c), out(n, h, w, c);
+  launch_f32_to_act(x, in.a, st);
+  LUMI_CUDA_CHECK(cudaMemsetAsync(out.a.hi, 0xFF, out.a.numel() * sizeof(__half), st));
+  LUMI_CUDA_CHECK(cudaMemsetAsync(out.a.lo, 0xFF, out.a.numel() * sizeof(__half), st));
+  launch_l2norm_scale(in.a, out.a, gamma, eps, st);
+  launch_act_to_f32(out.a, y, st);
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
+  return LUMI_OK;
+  OP_END
+}
+
 int lumi_op_softmax_rows(const float* x, int rows, int cols, int in_stride, float* y, void* stream) {
   OP_BEGIN
   cudaStream_t st = static_cast<cudaStream_t>(stream);

@@ -1,4 +1,4 @@
-"""SSD300 inference forward (oracle only).
+"""SSD inference forward at the configured fixed size (oracle only).
 
 ``luminoth/models/ssd/ssd.py:37-195`` (heads, softmax, anchors) and
 ``luminoth/models/ssd/proposal.py:41-171`` (per-class filter -> decode ->
@@ -60,7 +60,8 @@ def ssd_proposal(cls_prob, loc_pred, all_anchors, im_shape, num_classes, pcfg, v
 
 
 def forward(image, wts, config, dtype=np.float32):
-    """``SSD._build`` inference; image (300,300,3) raw 0..255 (dtype=float64: see fasterrcnn.forward)."""
+    """``SSD._build`` inference; image (fixed_height, fixed_width, 3) raw 0..255, uint8 or float (dtype=float64: see
+    fasterrcnn.forward)."""
     m = config['model']
     ip = config['dataset']['image_preprocessing']
     image_shape = [ip['fixed_height'], ip['fixed_width'], 3]     # ssd.py:30-31,63

@@ -16,7 +16,7 @@ VGG_CFG = [('conv1', 2, 64), ('conv2', 2, 128), ('conv3', 3, 256),
 
 
 def ssd_feature_maps(images, wts, scope='ssd/ssd_feature_extractor'):
-    """images (N,300,300,3) raw 0..255 -> OrderedDict of the 6 feature maps."""
+    """images (N,H,W,3) raw 0..255, any fixed size -> OrderedDict of the 6 feature maps."""
     v = scope + '/vgg_16'
     x = images
     conv4_3 = None

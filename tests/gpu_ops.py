@@ -102,6 +102,16 @@ def spatial_mean(x):
     return y.cpu().numpy()
 
 
+def l2norm_scale(x, gamma, eps=1e-12):
+    """x [n, h, w, c], gamma [c] -> x / sqrt(max(sum_c x^2, eps)) * gamma through the split planes, [n, h, w, c]."""
+    lib = _lib()
+    n, h, w, c = x.shape
+    xd, gd = _dev(x, np.float32), _dev(np.asarray(gamma).reshape(-1), np.float32)
+    y = torch.empty((n, h, w, c), dtype=torch.float32, device='cuda')
+    _check(lib.lumi_op_l2norm_scale(_p(xd), n, h, w, c, _p(gd), float(eps), _p(y), None))
+    return y.cpu().numpy()
+
+
 def softmax_rows(x, cols):
     """x [rows, in_stride] -> softmax of the first cols entries of each row, [rows, cols]."""
     lib = _lib()

@@ -180,30 +180,47 @@ def test_ssd_stages_and_detections(impl):
     for i in range(2):
         k = int(counts[i])
         assert box_dev(piped[0][i, :k], piped[2][i, :k], boxes[i, :k], labels[i, :k]) <= 2e-3
-    loc = eng.get_tensor('loc_pred'); prob = eng.get_tensor('cls_prob'); anchors = eng.get_tensor('all_anchors')
-    for i in range(2):
-        ref = ossd.forward(imgs[i], wts, cfg)
-        tru = ossd.forward(imgs[i], wts, cfg, dtype=np.float64)
+    ssd_parity('ssd/%s' % impl, eng, imgs, wts, cfg, (boxes, scores, labels, counts))
+    eng.close()
+
+
+def ssd_parity(key, eng, imgs, wts, cfg, out):
+    """The taps and detections `out` of the engine's last call on imgs, made with debug taps on, against the oracle
+    image by image: anchors bit-equal, feature maps, loc_pred, cls_prob and detections within the float bound."""
+    boxes, scores, labels, counts = out
+    n = len(imgs)
+    nc1 = cfg['model']['network']['num_classes'] + 1
+    loc, prob, anchors = eng.get_tensor('loc_pred'), eng.get_tensor('cls_prob'), eng.get_tensor('all_anchors')
+    fmaps = [eng.get_tensor('fmap_%d' % j) for j in range(6)]
+    total = anchors.shape[0]
+    assert anchors.shape == (total, 4) and loc.shape == (n, total, 4) and prob.shape == (n, total, nc1)
+    for i in range(n):
+        ref = ossd.forward(imgs[i], wts, cfg)                           # fp32 CPU oracle
+        tru = ossd.forward(imgs[i], wts, cfg, dtype=np.float64)         # exact-arithmetic yardstick
         np.testing.assert_array_equal(anchors, ref['all_anchors'])
         worst_e = worst_o = 0.0
-        for j, fm in enumerate(tru['feature_maps'].values()):
-            worst_e = max(worst_e, rel_err(eng.get_tensor('fmap_%d' % j)[i], fm[0]))
-            worst_o = max(worst_o, rel_err(list(ref['feature_maps'].values())[j][0], fm[0]))
+        for j, (fm_t, fm_r) in enumerate(zip(tru['feature_maps'].values(), ref['feature_maps'].values())):
+            assert fmaps[j][i].shape == fm_t.shape[1:], 'fmap_%d: %s vs %s' % (j, fmaps[j][i].shape, fm_t.shape[1:])
+            worst_e = max(worst_e, rel_err(fmaps[j][i], fm_t[0]))
+            worst_o = max(worst_o, rel_err(fm_r[0], fm_t[0]))
         e_loc, o_loc = rel_err(loc[i], tru['loc_pred']), rel_err(ref['loc_pred'], tru['loc_pred'])
-        e_pb = float(np.abs(prob[i] - tru['cls_prob']).max()); o_pb = float(np.abs(ref['cls_prob'] - tru['cls_prob']).max())
+        e_pb = float(np.abs(prob[i] - tru['cls_prob']).max())
+        o_pb = float(np.abs(ref['cls_prob'] - tru['cls_prob']).max())
         k = int(counts[i])
         tc_, rc_ = tru['classification_prediction'], ref['classification_prediction']
         e_det = box_dev(boxes[i, :k], labels[i, :k], tc_['objects'], tc_['labels'])
         o_det = box_dev(rc_['objects'], rc_['labels'], tc_['objects'], tc_['labels'])
-        _report('ssd/%s/img%d' % (impl, i), fmap_rel_engine=worst_e, fmap_rel_oracle32=worst_o, loc_rel_engine=e_loc,
+        e_p = float(np.abs(np.sort(scores[i, :k]) - np.sort(tc_['probs'])).max()) if k else 0.0
+        _report('%s/img%d' % (key, i), fmap_rel_engine=worst_e, fmap_rel_oracle32=worst_o, loc_rel_engine=e_loc,
                 loc_rel_oracle32=o_loc, prob_abs_engine=e_pb, prob_abs_oracle32=o_pb, detections_px_engine=e_det,
-                detections_px_oracle32=o_det, detections=k)
+                detections_px_oracle32=o_det, probs_abs_engine=e_p, detections=k, anchors=total)
+        assert k > 0, 'the comparison must not be vacuous'
         assert worst_e <= float_bound(worst_o, 5e-6), 'feature maps: %.2e vs %.2e' % (worst_e, worst_o)
-        assert e_loc <= float_bound(o_loc, 1e-5)
-        assert e_pb <= float_bound(o_pb, 2e-5)
+        assert e_loc <= float_bound(o_loc, 1e-5), 'loc: %.2e vs %.2e' % (e_loc, o_loc)
+        assert e_pb <= float_bound(o_pb, 2e-5), 'cls_prob: %.2e vs %.2e' % (e_pb, o_pb)
         assert e_det <= float_bound(o_det, 1e-3), 'detections: engine %.2e px vs oracle32 %.2e px' % (e_det, o_det)
+        assert e_p <= 2e-5
         assert (np.diff(scores[i, :k]) <= 0).all()
-    eng.close()
 
 
 def test_predictor_network_drop_in_schema():
@@ -398,11 +415,15 @@ def test_predictor_network_resized_images_match_the_reference_feed(shape):
     wts = synth.make_weights(cfg, seed=7)
     img = synth.make_images(1, shape[0], shape[1], seed=21)[0]
     net = PredictorNetwork(cfg, weights=wts)
-    got = net.predict_image(img)
-    ref = opredict.predict_image(img, wts, cfg)
+    match_reference(net.predict_image(img), opredict.predict_image(img, wts, cfg))
+    net.engine.close()
+
+
+def match_reference(got, ref):
+    """predict_image results against the oracle's: int(round(coord / scale)) can flip by one pixel when fp32 noise
+    (1e-3 px) meets a .5 boundary, so every detection is matched to an unused reference row of the same label within
+    1 px and 1e-4 in probability, and at least 97 % of them exactly."""
     assert len(got) == len(ref) and len(got) > 0
-    # int(round(coord / scale)) can flip by one pixel when fp32 noise (1e-3 px) meets a .5 boundary: match every
-    # detection to an unused reference row of the same label within 1 px and 1e-4 in probability
     free = list(ref)
     exact = 0
     for g in got:
@@ -413,7 +434,6 @@ def test_predictor_network_resized_images_match_the_reference_feed(shape):
         exact += best['bbox'] == g['bbox']
         free.remove(best)
     assert exact >= 0.97 * len(got)
-    net.engine.close()
 
 
 def test_full_size_batch_properties():
