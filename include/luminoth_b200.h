@@ -150,8 +150,11 @@ const char* lumi_op_last_error(void);      /* message of the last failed lumi_op
  * 6 / 7 2-CTA clusters multicasting the weight tile (7: + stream-K), 8 / 9 halo-patch kernels on 3x3 stride-1 layers
  * (9: + stream-K), 10 / 11 halo patches on 2-CTA clusters (11: + stream-K), 12 as 3 with the register epilogue, 13 the
  * SIMT kernel writing split planes (what the engine stores under conv_impl = simt), 14 / 15 as 3 on 128 x 256 tiles
- * (15: + stream-K; C_out padded to a multiple of 256 only).  Returns LUMI_EOVERFLOW when a split output (codes 3-15)
- * exceeds the split range, |x| > 65504. */
+ * (15: + stream-K; C_out padded to a multiple of 256 only).  Codes 1-12 run the engine's single-buffered mainloop;
+ * impl | 32 on them runs the double-buffered one (the engine's LUMI_CONV_PIPE=1), bit-identical by design.  16-19 run
+ * the layer as the engine launches it (auto stream-K, the engine's four-warpgroup bound and 128 x 256 tile rule):
+ * 16 split outputs on all SMs, 17 split outputs leaving the 8 SMs a pipelined half-batch leaves free, 18 / 19 the same
+ * with fp32 outputs.  Returns LUMI_EOVERFLOW when a split output (codes 3-17) exceeds the split range, |x| > 65504. */
 int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout,
                    int stride, int rate, int padding, const float* scale, const float* bias,
                    const float* residual, int act, int impl, float* y, int* ho, int* wo, void* stream);
@@ -160,7 +163,7 @@ int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wg
  * epilogue: p = relu(fmaf(x^, pre_scale[c], pre_bias[c])) where x^ is the output x as stored in its fp16x2 split
  * planes.  pre_scale / pre_bias [cout] on DEVICE.  y (x) and p are NHWC fp32 read back from the split planes; y may be
  * NULL to write p only; y and p both NULL is a shape query.  impl: 0 or 13 SIMT, or one of the split-output codes 3-7,
- * 12 (12: as 3 with the register epilogue).  Returns LUMI_EOVERFLOW when x or p exceeds the split range. */
+ * 12, 16, 17 (12: as 3 with the register epilogue; | 32 as for lumi_op_conv2d).  Returns LUMI_EOVERFLOW when x or p exceeds the split range. */
 int lumi_op_conv2d_preact(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout,
                           int stride, int rate, int padding, const float* scale, const float* bias,
                           const float* residual, int act, int impl, const float* pre_scale, const float* pre_bias,

@@ -37,6 +37,13 @@ void conv_workspace_free(ConvWorkspace& w);
 int device_sm_count();            // SMs of the CURRENT device
 constexpr int LUMI_MAX_DEVICES = 64;
 
+// The engine's default mainloop and four-warpgroup bound (DESIGN 7.2).  The stand-alone conv op runs the same, so the
+// per-kernel tests exercise the instances the engine launches.
+constexpr int CONV_PIPE_DEFAULT = 0;    // single-buffered slice accumulators (env LUMI_CONV_PIPE=1: double-buffered)
+constexpr int CONV_EPI16_DEFAULT = 16;  // four consumer warpgroups on split-output layers with <= 16 K slices per tile
+// SMs a persistent conv launch leaves free while the engine runs its two-stream half-batch pipeline
+constexpr int CONV_PIPELINE_SM_RESERVE = 8;
+
 struct ConvIO {
   Act in;
   Act out;                  // split-plane output (used when out_f32 == nullptr)
@@ -58,7 +65,7 @@ struct ConvIO {
   int cta2 = 0;                 // 2-CTA cluster kernel (weight tile multicast) on layers with at least this many K slices per tile (0 = never)
   int halo = 0;                 // halo-patch kernels on 3x3 stride-1 SAME layers without residual or fp32 output (0 never; on CTA pairs with cta2)
   int halo_tiles_pct = 150;     // ... while their M-tile count stays within this percentage of the generic kernel's
-  int pipe = 1;                 // 1: double-buffered slice accumulators (slice k + 1's MMAs overlap slice k's fold); 0: single (the engine's default, LUMI_CONV_PIPE)
+  int pipe = CONV_PIPE_DEFAULT; // 1: double-buffered slice accumulators (slice k + 1's MMAs overlap slice k's fold); 0: single
   int epi16 = 0;                // four-consumer-warpgroup (16 epilogue warps) kernel on layers with at most this many K slices per tile (0 = never)
   int wide = 16;                // 128 x 256 tiles on split-output layers with cout_pad % 256 == 0 and at least this many K slices per tile (0 = never)
   int wide_sm_pct = 50;         // ... while those tiles number at least this percentage of the SMs the launch may use

@@ -163,8 +163,8 @@ struct lumi_engine {
   int conv_cta2 = 0;            // env LUMI_CONV_2CTA: 2-CTA cluster kernel on layers with at least this many K slices per tile
   int conv_halo = 0;            // env LUMI_CONV_HALO: 1 = halo-patch kernels on the 3x3 stride-1 layers
   int conv_halo_pct = 150;      // env LUMI_CONV_HALO_PCT: ... while the M-tile count stays within this percentage of the generic kernel's
-  int conv_epi16 = 16;          // env LUMI_CONV_EPI16: four-warpgroup kernel on layers with at most this many K slices per tile
-  int conv_pipe = 0;            // env LUMI_CONV_PIPE: 1 = double-buffered slice accumulators in the conv mainloop (slower on R50, DESIGN 7.1)
+  int conv_epi16 = CONV_EPI16_DEFAULT;  // env LUMI_CONV_EPI16: four-warpgroup kernel on layers with at most this many K slices per tile
+  int conv_pipe = CONV_PIPE_DEFAULT;    // env LUMI_CONV_PIPE: 1 = double-buffered slice accumulators in the conv mainloop (slower on R50, DESIGN 7.1)
   int conv_epi_tma = 1;         // env LUMI_CONV_EPI_TMA: 1 = split outputs through the shared-memory slot epilogue, 0 = register epilogue
   uint8_t* d_images = nullptr; size_t images_cap = 0;
   float* d_boxes = nullptr; float* d_scores = nullptr; int* d_labels = nullptr; int* d_counts = nullptr;
@@ -957,6 +957,7 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
     if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_u8_to_act(images, cx.img_f32, x, RGB_MEANS, cx.st); }  // base_network.py:153-177
     x = run_conv(cx, root + "/conv1", x, nullptr, 1, nullptr);           // conv2d_same(64, 7, stride 2) + BN + relu
   }                                                                      // (v2: + bias, no activation)
+  cx.tap_act("stem", x);
   const Endpoint& ep = e->ep;
   if (ep.block < 0) {
     // the stem conv is the endpoint
@@ -1171,15 +1172,18 @@ void forward_ssd(Ctx& cx, const void* images, int n, int h, int w) {
     view.w = w; view.c = 64;
     const long pitch[3] = {16, (long)(w + 3) * 16, (long)(h + 2) * (w + 3) * 16};
     x = run_conv(cx, s + "/vgg_16/conv1/conv1_1#pack", view, nullptr, 1, nullptr, pitch, 2.0 * n * h * w * 27.0 * 64.0);
+    cx.tap_act("conv1_1", x);
   } else {
     x = cx.act(n, h, w, 3);
     if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_u8_to_act(images, cx.img_f32, x, nullptr, cx.st); }  // no mean subtraction (quirk Q7)
   }
   Act fmaps[6];
   for (int b = 0; b < 5; ++b) {
-    for (int r = (b == 0 && c11_tc) ? 1 : 0; r < VGG_REPS[b]; ++r)
+    for (int r = (b == 0 && c11_tc) ? 1 : 0; r < VGG_REPS[b]; ++r) {
       x = run_conv(cx, s + "/vgg_16/" + VGG_NAMES[b] + "/" + VGG_NAMES[b] + "_" + std::to_string(r + 1), x, nullptr, 1,
                    nullptr);
+      if (b == 0 && r == 0) cx.tap_act("conv1_1", x);
+    }
     if (b == 3) {                                                         // conv4_3 -> l2norm x gamma
       Act nrm = cx.act(x.n, x.h, x.w, x.c);
       if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_HEAD_MISC); launch_l2norm_scale(x, nrm, e->dev_vecs.at("gamma"), 1e-12f, cx.st); }
@@ -1507,7 +1511,7 @@ static int predict_impl(lumi_engine* e, const void* images, int esz, int images_
   if (e->type == "fasterrcnn") ensure_frcnn_anchors(e, h, w, e->stream);
   Ctx cx = make_ctx(e, false, 0);
   cx.img_f32 = esz == 4;
-  cx.sm_reserve = piped ? 8 : 0;
+  cx.sm_reserve = piped ? CONV_PIPELINE_SM_RESERVE : 0;
   if (piped) {
     LUMI_CUDA_CHECK(cudaEventRecord(e->ev_fork, e->stream));
     LUMI_CUDA_CHECK(cudaStreamWaitEvent(e->stream2, e->ev_fork, 0));

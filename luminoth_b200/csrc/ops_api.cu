@@ -33,6 +33,8 @@ struct ActBuf {
 
 int op_fail(const Error& e) { g_op_error = e.what(); return e.code; }
 
+constexpr int CONV_OP_PIPE = 32;   // impl flag of lumi_op_conv2d*: the double-buffered mainloop
+
 // The arguments of lumi_op_conv2d_io: those of lumi_op_conv2d, the residual's own resolution and sampling stride
 // (res_h <= 0: the output's, stride 1) and the pre-activation output of lumi_op_conv2d_preact (pre_scale == nullptr:
 // none; then y is required, else y == nullptr writes p only).
@@ -41,7 +43,10 @@ int op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, in
               int res_w, int res_stride, int act, int impl, const float* pre_scale, const float* pre_bias, float* y,
               float* p, int* ho_out, int* wo_out, cudaStream_t st) {
   const bool preact = pre_scale != nullptr;
-  LUMI_REQUIRE(impl >= 0 && impl <= 15, "conv2d: impl must be one of 0-15");
+  const bool pipe = (impl & CONV_OP_PIPE) != 0;
+  impl &= ~CONV_OP_PIPE;
+  LUMI_REQUIRE(impl >= 0 && impl <= 19, "conv2d: impl must be one of 0-19");
+  LUMI_REQUIRE(!pipe || (impl >= 1 && impl <= 12), "conv2d: impl | 32 (double-buffered mainloop) needs one of 1-12");
   ConvLayer L;
   L.kh = kh; L.kw = kw; L.cin = cin; L.cout = cout; L.stride = stride; L.rate = rate; L.act = act;
   const size_t nw = (size_t)kh * kw * cin * cout;
@@ -68,17 +73,23 @@ int op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, in
   LUMI_REQUIRE(preact ? (p && pre_bias) : (y && !p), "conv2d: bad output arguments");
   // 0: SIMT, fp32 outputs; 1 whole tiles, 2 stream-K forced (fp32 outputs written by the epilogue);
   // 3 / 4 / 5: the engine's inter-layer form -- fp16x2 split planes -- with two consumer warpgroups (3), the
-  // four-warpgroup short-K kernel allowed (4), and 4 + stream-K (5), all through the shared-memory slot epilogue;
-  // 6 / 7: the 2-CTA cluster kernel wherever it applies (7: + stream-K); 8-11: the halo-patch kernels (10, 11 on
-  // cluster pairs; 9, 11: + stream-K); 12: as 3 with the register epilogue; 13: SIMT writing split planes (the engine's
-  // conv_impl = simt); 14 / 15: as 3 on 128 x 256 tiles whatever the K-slice and tile counts (15: + stream-K), for layers with
-  // cout_pad % 256 == 0.  Codes 1-12 never take the 128 x 256 tile.  A pre-activation output is written in split planes
-  // only: SIMT (0 or 13), 3-7 or 12.
+  // four-warpgroup short-K kernel allowed up to the engine's CONV_EPI16_DEFAULT K slices (4), and 4 + stream-K (5), all
+  // through the shared-memory slot epilogue; 6 / 7: the 2-CTA cluster kernel wherever it applies (7: + stream-K); 8-11:
+  // the halo-patch kernels (10, 11 on cluster pairs; 9, 11: + stream-K); 12: as 3 with the register epilogue; 13: SIMT
+  // writing split planes (the engine's conv_impl = simt); 14 / 15: as 3 on 128 x 256 tiles whatever the K-slice and tile
+  // counts (15: + stream-K), for layers with cout_pad % 256 == 0.  Codes 1-12 never take the 128 x 256 tile, and run the
+  // engine's single-buffered mainloop; impl | 32 (CONV_OP_PIPE) on them runs the double-buffered one (LUMI_CONV_PIPE=1).
+  // 16-19: as the engine launches the layer, every switch at run_conv's default (auto stream-K on a workspace, the
+  // four-warpgroup bound, the 128 x 256 tile by its shape rule, slot epilogue, single-buffered, no 2-CTA or halo
+  // kernels): 16 split outputs on all SMs, 17 split outputs leaving CONV_PIPELINE_SM_RESERVE SMs free (a pipelined
+  // half-batch), 18 / 19 the same with fp32 outputs (the RPN and RCNN heads, the RCNN FC layers).  A pre-activation
+  // output is written in split planes only: SIMT (0 or 13), 3-7, 12, 16 or 17.
   const bool simt = impl == 0 || impl == 13;
-  const bool split = preact || impl >= 3;
+  const bool as_engine = impl >= 16;
+  const bool split = preact || (impl >= 3 && impl <= 17);
   if (preact)
-    LUMI_REQUIRE(simt || (impl >= 3 && impl <= 7) || impl == 12,
-                 "conv2d_preact: impl must be 0 or 13 (SIMT) or one of the split-output codes 3-7, 12");
+    LUMI_REQUIRE(simt || (impl >= 3 && impl <= 7) || impl == 12 || impl == 16 || impl == 17,
+                 "conv2d_preact: impl must be 0 or 13 (SIMT) or one of the split-output codes 3-7, 12, 16, 17");
   if (split) LUMI_REQUIRE(cout % 32 == 0, "conv2d: split outputs need cout % 32 == 0");
   ActBuf in(n, h, w, cin);
   launch_f32_to_act(x, in.a, st);
@@ -120,9 +131,17 @@ int op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, in
   struct SkGuard { ConvWorkspace& w; ~SkGuard() { conv_workspace_free(w); } } skg{sk};
   if (simt) {
     launch_conv_simt(L, io, st);
+  } else if (as_engine) {
+    io.epi16 = CONV_EPI16_DEFAULT;
+    io.sm_reserve = (impl == 17 || impl == 19) ? CONV_PIPELINE_SM_RESERVE : 0;
+    LUMI_REQUIRE(conv_tc_supported(L, io), "conv2d: this layer shape is not handled by the tensor-core kernel");
+    conv_workspace_create(sk);
+    io.sk = &sk;
+    launch_conv_tc(L, io, st);
   } else {
+    io.pipe = pipe ? 1 : 0;
     io.epi_tma = impl == 12 ? 0 : 1;
-    io.epi16 = (impl == 4 || impl == 5) ? 8 : 0;
+    io.epi16 = (impl == 4 || impl == 5) ? CONV_EPI16_DEFAULT : 0;
     io.cta2 = (impl == 6 || impl == 7 || impl == 10 || impl == 11) ? 1 : 0;
     io.halo = (impl >= 8 && impl <= 11) ? 1 : 0;
     io.halo_tiles_pct = 1000000;                    // test hook: whenever the shape allows

@@ -37,7 +37,9 @@ def conv2d(x, w, stride=1, rate=1, padding='SAME', scale=None, bias=None, residu
     rd = _dev(residual, np.float32) if residual is not None else None
     ho, wo = ctypes.c_int(), ctypes.c_int()
     im = {'simt': 0, 'tc': 1, 'tc_streamk': 2, 'tc_split': 3, 'tc_split_epi16': 4, 'tc_split_epi16_streamk': 5, 'tc_split_cta2': 6, 'tc_split_cta2_streamk': 7,
-          'tc_split_halo': 8, 'tc_split_halo_streamk': 9, 'tc_split_halo_cta2': 10, 'tc_split_halo_cta2_streamk': 11}[impl]
+          'tc_split_halo': 8, 'tc_split_halo_streamk': 9, 'tc_split_halo_cta2': 10, 'tc_split_halo_cta2_streamk': 11,
+          'tc_split_register': 12, 'simt_split': 13, 'tc_split_wide': 14, 'tc_split_wide_streamk': 15,
+          'engine': 16, 'engine_reserve': 17, 'engine_f32': 18, 'engine_f32_reserve': 19}[impl]
     _check(lib.lumi_op_conv2d(_p(xd), n, h, wd, cin, _p(wdv), kh, kw, cout, stride, rate, pad, _p(sd), _p(bd), _p(rd),
                               act, im, None, ctypes.byref(ho), ctypes.byref(wo), None))
     y = torch.empty((n, ho.value, wo.value, cout), dtype=torch.float32, device='cuda')

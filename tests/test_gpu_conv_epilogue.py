@@ -11,8 +11,9 @@ import pytest
 
 from test_gpu_kernels import CONV_CASES, _bn_fold, _ref_conv, assert_close
 
-# lumi_op_conv2d impl codes: split planes through the slot epilogue (two consumer warpgroups / four allowed /
-# four + stream-K), and the generic kernel with the register epilogue forced
+# lumi_op_conv2d impl codes: split planes through the slot epilogue (two consumer warpgroups / four allowed up to the
+# engine's 16 K slices / four + stream-K), and the generic kernel with the register epilogue forced; all run the
+# engine's single-buffered mainloop
 SLOT, SLOT_EPI16, SLOT_EPI16_STREAMK, REGISTER = 3, 4, 5, 12
 
 # name, n, h, w, cin, cout, k, stride, rate, padding, residual, act: the second 64-channel box of the tile is half

@@ -2,8 +2,10 @@
 
 Every case runs through `lumi_op_conv2d_io` on the SIMT kernel (impl 0: fp32 outputs, 13: split planes) and the
 tensor-core kernel (1 / 2: fp32 outputs, whole tiles / stream-K; 3 / 4 / 5: split planes through the slot epilogue,
-two consumer warpgroups / four allowed / four + stream-K; 12: the register epilogue; 6 / 7: 2-CTA clusters), and
-is compared with a float64 reference computed from the fp32 inputs.
+two consumer warpgroups / four allowed up to the engine's 16 K slices / four + stream-K; 12: the register epilogue;
+6 / 7: 2-CTA clusters), all on the engine's single-buffered mainloop, and is compared with a float64 reference
+computed from the fp32 inputs.  test_gpu_conv_engine_layers runs the engine's own launch (codes 16-19) of every
+production layer against the same bound, evaluated at sampled pixels (`reference(..., at=...)`).
 
 The bound
 ---------
@@ -102,25 +104,74 @@ def pack_exponent(w):
     return e, mx
 
 
-def reference(x, w, stride, padding, scale, bias, residual, res_stride, act, impl):
-    """float64 reference of the layer and the per-element bound of the module docstring."""
+def out_geometry(h, w, k, stride, rate, padding):
+    """(ho, wo, pad_top, pad_left) of the layer, as lumi_op_conv2d and the engine's run_conv derive them."""
+    keff = k + (k - 1) * (rate - 1)
+    if padding == 'SAME' or (padding == 'SLIM' and stride == 1):
+        ho, wo = -(-h // stride), -(-w // stride)
+        return ho, wo, max(0, (ho - 1) * stride + keff - h) // 2, max(0, (wo - 1) * stride + keff - w) // 2
+    if padding == 'SLIM':
+        p = (keff - 1) // 2
+        return (h - 1) // stride + 1, (w - 1) // stride + 1, p, p
+    return (h - keff) // stride + 1, (w - keff) // stride + 1, 0, 0
+
+
+def _sampled_sums(x, w, stride, padding, rate, at):
+    """float64 sum x w, sum |x||w|, sum |w| and sum |x| over the taps inside the map, at output pixels
+    at = (img, oy, ox): [P, C_out] each ([P, 1] for sum |x|).  Only the sampled input patches are gathered."""
+    n, h, wd, cin = x.shape
+    kh, kw, _, cout = w.shape
+    _, _, pt, pl = out_geometry(h, wd, kh, stride, rate, padding)
+    img, oy, ox = (np.asarray(a, np.int64) for a in at)
+    w64 = w.astype(f64).reshape(kh * kw, cin, cout)
+    aw = np.abs(w64)
+    acc = np.zeros((len(img), cout))
+    sxw = np.zeros((len(img), cout))
+    sw = np.zeros((len(img), cout))
+    sx = np.zeros((len(img), 1))
+    for t in range(kh * kw):
+        iy = oy * stride - pt + (t // kw) * rate
+        ix = ox * stride - pl + (t % kw) * rate
+        inside = (iy >= 0) & (iy < h) & (ix >= 0) & (ix < wd)
+        xt = x[img, iy.clip(0, h - 1), ix.clip(0, wd - 1)].astype(f64) * inside[:, None]
+        acc += xt @ w64[t]
+        axt = np.abs(xt)
+        sxw += axt @ aw[t]
+        sw += inside[:, None] * aw[t].sum(0)
+        sx += axt.sum(1, keepdims=True)
+    return acc, sxw, sw, sx
+
+
+def reference(x, w, stride, padding, scale, bias, residual, res_stride, act, impl, rate=1, at=None, k_fold=None):
+    """float64 reference of the layer and the per-element bound of the module docstring: at every output element
+    ([n, ho, wo, C_out]) or, with at = (img, oy, ox) index arrays, at those output pixels only ([P, C_out]).
+    k_fold: the K whose 64-deep slices the tensor-core kernel folds, when a packed layout runs more than kh kw C_in."""
     cout = w.shape[-1]
     s = np.ones(cout, f64) if scale is None else scale.astype(f64)
     b = np.zeros(cout, f64) if bias is None else bias.astype(f64)
-    acc = _conv64(x, w, stride, padding)
+    if at is None:
+        assert rate == 1
+        acc = _conv64(x, w, stride, padding)
+        ax, aw = np.abs(x.astype(f64)), np.abs(w.astype(f64))
+        sxw, sw = _conv64(ax, aw, stride, padding), _conv64(np.ones_like(ax), aw, stride, padding)
+        sx = _conv64(ax, np.ones(w.shape[:3] + (1,)), stride, padding)
+    else:
+        acc, sxw, sw, sx = _sampled_sums(x, w, stride, padding, rate, at)
     r = None
     if residual is not None:
-        r = residual.astype(f64)[:, ::res_stride, ::res_stride][:, :acc.shape[1], :acc.shape[2]]
+        if at is None:
+            r = residual.astype(f64)[:, ::res_stride, ::res_stride][:, :acc.shape[1], :acc.shape[2]]
+        else:
+            r = residual[at[0], np.asarray(at[1]) * res_stride, np.asarray(at[2]) * res_stride].astype(f64)
         assert r.shape == acc.shape
     ref = acc * s + b + (r if r is not None else 0.0)
     if act == 1:
         ref = np.maximum(ref, 0.0)
     elif act == 2:
         ref = np.clip(ref, 0.0, 6.0)
-    ax, aw = np.abs(x.astype(f64)), np.abs(w.astype(f64))
-    S = np.abs(s) * _conv64(ax, aw, stride, padding) + np.abs(b) + (np.abs(r) if r is not None else 0.0)
-    W = np.abs(s) * _conv64(np.ones_like(ax), aw, stride, padding)
-    K = w.shape[0] * w.shape[1] * w.shape[2]
+    S = np.abs(s) * sxw + np.abs(b) + (np.abs(r) if r is not None else 0.0)
+    W = np.abs(s) * sw
+    K = w.shape[0] * w.shape[1] * w.shape[2] if k_fold is None else k_fold
     if impl in (0, 13):
         alpha = 1.01 * (2.0 ** -22 * 2 + U * (K + 3))
         V = 0.0
@@ -128,7 +179,7 @@ def reference(x, w, stride, padding, scale, bias, residual, res_stride, act, imp
         alpha = 1.01 * (2.0 ** -22 * 12 + U * (math.ceil(K / 64) + 3))
         e, mx = pack_exponent(w)
         fw = 2.0 ** -25 * np.abs(s) * 2.0 ** -e.astype(f64) + 2.0 ** -150 * 2.0 ** e.astype(f64) * mx
-        V = fw * _conv64(ax, np.ones(w.shape[:3] + (1,)), stride, padding)
+        V = fw * sx
     delta = 2.0 ** -25 * (2 if r is not None else 1)
     return ref, alpha * S + 1.01 * 2.0 ** -25 * W + V + delta
 
