@@ -255,6 +255,12 @@ int act_from_name(const std::string& n) {
   throw Error(LUMI_EINVAL, "unsupported activation_function '" + n + "' (relu | relu6)");
 }
 
+// get_activation_function (utils/vars.py:80-88): null or '' is the identity; a missing key keeps the relu6 default
+int act_from_config(const JVal& c, const std::string& path) {
+  const std::string n = c.str_or_empty(path, "relu6");
+  return n.empty() ? ACT_NONE : act_from_name(n);
+}
+
 void compute_frcnn_anchor_ref(lumi_engine* e) {
   // utils/anchors.py:4-52 in float64, then truncation toward zero (fasterrcnn.py:299-302, quirk Q1)
   const double base = e->cfg.number("model.anchors.base_size", 256);
@@ -379,7 +385,7 @@ void parse_config(lumi_engine* e) {
     e->rpn_channels = (int)c.number("model.rpn.num_channels", 512);
     std::vector<double> ks = c.numbers("model.rpn.kernel_shape");
     if (ks.size() == 2) { e->rpn_kh = (int)ks[0]; e->rpn_kw = (int)ks[1]; }
-    e->rpn_act = act_from_name(c.str("model.rpn.activation_function", "relu6"));
+    e->rpn_act = act_from_config(c, "model.rpn.activation_function");
     RpnParams& r = e->rpn;
     r.pre_nms_top_n = (int)c.number("model.rpn.proposals.pre_nms_top_n", 12000);
     r.post_nms_top_n = (int)c.number("model.rpn.proposals.post_nms_top_n", 2000);
@@ -393,7 +399,7 @@ void parse_config(lumi_engine* e) {
     e->kmax = r.post_nms_top_n;
     if (e->with_rcnn) {
       for (double v : c.numbers("model.rcnn.layer_sizes")) e->fc_sizes.push_back((int)v);
-      e->fc_act = act_from_name(c.str("model.rcnn.activation_function", "relu6"));
+      e->fc_act = act_from_config(c, "model.rcnn.activation_function");
       e->use_mean = c.boolean("model.rcnn.use_mean", true);
       std::string mode = c.str("model.rcnn.roi.pooling_mode", "crop");
       std::transform(mode.begin(), mode.end(), mode.begin(), ::tolower);

@@ -51,6 +51,13 @@ struct JVal {
     if (v->t == Str) return v->s;
     throw std::runtime_error("config key '" + path + "' is not a string");
   }
+  // as str(), but a null value reads as the empty string: only a missing key takes the default
+  std::string str_or_empty(const std::string& path, const std::string& def) const {
+    const JVal* v = find(path);
+    if (!v) return def;
+    if (v->t == Null) return "";
+    return str(path, def);
+  }
   std::vector<double> numbers(const std::string& path) const {
     std::vector<double> out;
     const JVal* v = find(path);

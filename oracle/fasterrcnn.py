@@ -22,12 +22,20 @@ def cfg_get(cfg, path, default=None):
     return cur
 
 
+def activation(name):
+    """``utils/vars.py:80-88`` (get_activation_function): None or '' is the identity, else the tf.nn function of
+    that name (relu and relu6 here)."""
+    if not name:
+        return lambda a: a
+    return {'relu6': T.relu6, 'relu': T.relu}[name]
+
+
 # ---------------------------------------------------------------- RPN
-def rpn_head(fmap, wts, activation='relu6', scope='fasterrcnn/rpn'):
+def rpn_head(fmap, wts, act='relu6', scope='fasterrcnn/rpn'):
     """``rpn.py:67-90,136-170``: 3x3 conv(+bias) -> activation -> 1x1 cls (2A)
     and 1x1 bbox (4A) -> reshape(-1,2) softmax / reshape(-1,4)."""
     x = T.conv2d(fmap, wts[scope + '/conv/w'], 1, 'SAME', bias=wts[scope + '/conv/b'])
-    x = {'relu6': T.relu6, 'relu': T.relu}[activation](x)
+    x = activation(act)(x)
     cls = T.conv2d(x, wts[scope + '/cls_conv/w'], 1, 'VALID', bias=wts[scope + '/cls_conv/b'])
     box = T.conv2d(x, wts[scope + '/bbox_conv/w'], 1, 'VALID', bias=wts[scope + '/bbox_conv/b'])
     cls_score = cls.reshape(-1, 2)
@@ -108,7 +116,7 @@ def rcnn_head(pooled, wts, rcfg, arch, scope='fasterrcnn/rcnn', use_tail=True):
         else:
             feats = feats.reshape(0, feats.shape[-1])
     net = feats.reshape(feats.shape[0], -1)
-    act = {'relu6': T.relu6, 'relu': T.relu}[rcfg.get('activation_function', 'relu6')]
+    act = activation(rcfg.get('activation_function', 'relu6'))
     dt = net.dtype
     for i, _ in enumerate(rcfg.get('layer_sizes') or []):
         net = act(net @ wts['%s/fc_%d/w' % (scope, i)].astype(dt) + wts['%s/fc_%d/b' % (scope, i)].astype(dt))

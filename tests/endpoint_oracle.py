@@ -111,11 +111,18 @@ def fasterrcnn_forward(image, wts, config, dtype=np.float32):
     block4's variables, so it raises TF's ValueError on an endpoint that is not 1024 channels deep."""
     m = config['model']
     bn = m['base_network']
+    image = np.asarray(image, dtype)
+    fmap = trunk(image[None], wts, bn['architecture'], bn.get('endpoint'), bn.get('output_stride', 16))
+    return fasterrcnn_heads(fmap, image.shape[:2], wts, config)
+
+
+def fasterrcnn_heads(fmap, im_shape, wts, config):
+    """The stages of ``fasterrcnn_forward`` after the trunk, on its feature map ``fmap`` (1, h, w, c) of an image of
+    ``im_shape``: anchors, RPN, and with_rcnn the ROI pool, the RCNN head and the detections."""
+    m = config['model']
+    bn = m['base_network']
     arch = bn['architecture']
     use_tail = bn.get('use_tail', True)
-    image = np.asarray(image, dtype)
-    fmap = trunk(image[None], wts, arch, bn.get('endpoint'), bn.get('output_stride', 16))
-    im_shape = image.shape[:2]
     a = m['anchors']
     anchors = fasterrcnn_anchors(fmap.shape[1], fmap.shape[2], a['base_size'], a['ratios'], a['scales'], a['stride'])
     r = ofr.rpn_head(fmap, wts, m['rpn'].get('activation_function', 'relu6'))

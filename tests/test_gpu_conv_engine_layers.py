@@ -241,14 +241,18 @@ def _four_warpgroup(row):
 
 # ---------------------------------------------------------------------------------------------- host checks
 def test_sampled_bound_matches_the_full_bound():
-    """The sampled float64 reference and bound equal the full ones at every pixel (stride 1 / 2, every padding)."""
+    """The sampled float64 reference and bound equal the full ones at every pixel (stride 1 / 2, every padding,
+    square, non-square and even kernels)."""
     rng = np.random.default_rng(7)
     for k, stride, padding, res_stride in [(3, 1, 'SAME', 1), (3, 2, 'SLIM', 1), (1, 1, 'SAME', 2), (3, 1, 'VALID', 1),
-                                           (7, 2, 'SLIM', 1), (3, 2, 'SAME', 1)]:
+                                           (7, 2, 'SLIM', 1), (3, 2, 'SAME', 1), ((5, 3), 1, 'SAME', 1),
+                                           ((3, 5), 2, 'SAME', 1), ((1, 7), 1, 'VALID', 1), ((7, 1), 2, 'VALID', 1),
+                                           ((2, 2), 1, 'SAME', 1), ((4, 4), 2, 'SAME', 1), ((2, 2), 2, 'VALID', 1)]:
+        kh, kw = (k, k) if isinstance(k, int) else k
         x = rng.standard_normal((2, 11, 14, 8)).astype(f32)
-        w = rng.standard_normal((k, k, 8, 5)).astype(f32)
+        w = rng.standard_normal((kh, kw, 8, 5)).astype(f32)
         scale, bias = rng.uniform(0.5, 1.5, 5).astype(f32), rng.standard_normal(5).astype(f32)
-        ho, wo, _, _ = out_geometry(11, 14, k, stride, 1, padding)
+        ho, wo, _, _ = out_geometry(11, 14, kh, stride, 1, padding, kw=kw)
         res = rng.standard_normal((2, ho * res_stride, wo * res_stride, 5)).astype(f32)
         at = tuple(a.ravel() for a in np.meshgrid(np.arange(2), np.arange(ho), np.arange(wo), indexing='ij'))
         for impl in (0, ENGINE):

@@ -104,16 +104,18 @@ def pack_exponent(w):
     return e, mx
 
 
-def out_geometry(h, w, k, stride, rate, padding):
-    """(ho, wo, pad_top, pad_left) of the layer, as lumi_op_conv2d and the engine's run_conv derive them."""
+def out_geometry(h, w, k, stride, rate, padding, kw=None):
+    """(ho, wo, pad_top, pad_left) of the layer, as lumi_op_conv2d and the engine's run_conv derive them: a k x k
+    kernel, or k x kw (SLIM pads both sides by the kernel's height, as conv2d_same's square kernels need)."""
     keff = k + (k - 1) * (rate - 1)
+    kweff = keff if kw is None else kw + (kw - 1) * (rate - 1)
     if padding == 'SAME' or (padding == 'SLIM' and stride == 1):
         ho, wo = -(-h // stride), -(-w // stride)
-        return ho, wo, max(0, (ho - 1) * stride + keff - h) // 2, max(0, (wo - 1) * stride + keff - w) // 2
+        return ho, wo, max(0, (ho - 1) * stride + keff - h) // 2, max(0, (wo - 1) * stride + kweff - w) // 2
     if padding == 'SLIM':
         p = (keff - 1) // 2
         return (h - 1) // stride + 1, (w - 1) // stride + 1, p, p
-    return (h - keff) // stride + 1, (w - keff) // stride + 1, 0, 0
+    return (h - keff) // stride + 1, (w - kweff) // stride + 1, 0, 0
 
 
 def _sampled_sums(x, w, stride, padding, rate, at):
@@ -121,7 +123,7 @@ def _sampled_sums(x, w, stride, padding, rate, at):
     at = (img, oy, ox): [P, C_out] each ([P, 1] for sum |x|).  Only the sampled input patches are gathered."""
     n, h, wd, cin = x.shape
     kh, kw, _, cout = w.shape
-    _, _, pt, pl = out_geometry(h, wd, kh, stride, rate, padding)
+    _, _, pt, pl = out_geometry(h, wd, kh, stride, rate, padding, kw=kw)
     img, oy, ox = (np.asarray(a, np.int64) for a in at)
     w64 = w.astype(f64).reshape(kh * kw, cin, cout)
     aw = np.abs(w64)

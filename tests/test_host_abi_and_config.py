@@ -82,6 +82,38 @@ def test_parse_override_and_values():
     assert C.parse_override(None) == {}
 
 
+def test_empty_activation_function_is_the_identity():
+    """utils/vars.py:80-88 (get_activation_function): a None or '' activation_function is the identity in the oracle's
+    RPN and RCNN heads, relu and relu6 are tf.nn's.  The overrides `=None` and `=` reach the config as None and ''."""
+    from oracle import fasterrcnn as ofr
+    from oracle import tf_ops as T
+    rng = np.random.default_rng(3)
+    wts = {'fasterrcnn/rpn/conv/w': rng.standard_normal((3, 3, 8, 6)).astype(np.float32),
+           'fasterrcnn/rpn/conv/b': rng.standard_normal(6).astype(np.float32)}
+    for name, cout in (('cls_conv', 2), ('bbox_conv', 4)):
+        wts['fasterrcnn/rpn/%s/w' % name] = rng.standard_normal((1, 1, 6, cout)).astype(np.float32)
+        wts['fasterrcnn/rpn/%s/b' % name] = rng.standard_normal(cout).astype(np.float32)
+    fmap = (rng.standard_normal((1, 4, 5, 8)) * 4).astype(np.float32)
+    pre = T.conv2d(fmap, wts['fasterrcnn/rpn/conv/w'], 1, 'SAME', bias=wts['fasterrcnn/rpn/conv/b'])
+    assert pre.min() < 0 and pre.max() > 6
+    for act, want in ((None, pre), ('', pre), ('relu', np.maximum(pre, 0)), ('relu6', np.clip(pre, 0, 6))):
+        np.testing.assert_array_equal(ofr.rpn_head(fmap, wts, act)['rpn_feature'], want)
+    feats = (rng.standard_normal((3, 7, 7, 5)) * 4).astype(np.float32)
+    rcnn = {'fasterrcnn/rcnn/fc_0/w': rng.standard_normal((5, 4)).astype(np.float32),
+            'fasterrcnn/rcnn/fc_0/b': rng.standard_normal(4).astype(np.float32),
+            'fasterrcnn/rcnn/fc_classifier/w': rng.standard_normal((4, 3)).astype(np.float32),
+            'fasterrcnn/rcnn/fc_classifier/b': np.zeros(3, np.float32),
+            'fasterrcnn/rcnn/fc_bbox/w': rng.standard_normal((4, 8)).astype(np.float32),
+            'fasterrcnn/rcnn/fc_bbox/b': np.zeros(8, np.float32)}
+    fc = feats.mean(axis=(1, 2), dtype=np.float32) @ rcnn['fasterrcnn/rcnn/fc_0/w'] + rcnn['fasterrcnn/rcnn/fc_0/b']
+    assert fc.min() < 0
+    for act in (None, ''):
+        head = ofr.rcnn_head(feats, rcnn, {'layer_sizes': [4], 'activation_function': act}, 'resnet_v1_50')
+        np.testing.assert_array_equal(head['features'], fc)
+    cfg = C.default_config('fasterrcnn', ['model.rpn.activation_function=None', 'model.rcnn.activation_function='])
+    assert cfg.model.rpn.activation_function is None and cfg.model.rcnn.activation_function == ''
+
+
 def test_merge_into_type_check_and_replace():
     """utils/config.py:73-148"""
     base = C.Config({'a': 1, 'b': {'c': 2, 'd': 3}, 'e': None, 'opt': {'_replace': True, 'type': 'momentum', 'momentum': 0.9}})
