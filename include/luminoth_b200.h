@@ -55,7 +55,7 @@ int lumi_weight_info(lumi_engine* e, int index, const char** name, int64_t* shap
 int lumi_finalize(lumi_engine* e);
 
 /* Run the forward pass on n images of identical size h x w (already resized
- * like datasets/object_detection_dataset.py:71-83), RGB, NHWC.
+ * like datasets/object_detection_dataset.py:71-83; lumi_predict_resize takes them at their original sizes), RGB, NHWC.
  *   images      uint8 [n,h,w,3]; host pointer (images_on_device = 0, copied H2D inside)
  *               or device pointer (images_on_device = 1)
  *   boxes       float [n, kmax, 4]  (x1,y1,x2,y2) in resized-image pixels
@@ -73,6 +73,22 @@ int lumi_predict(lumi_engine* e, const void* images, int images_on_device, int n
  * as they are).  lumi_predict is the exact special case of integer-valued pixels. */
 int lumi_predict_f32(lumi_engine* e, const float* images, int images_on_device, int n, int h, int w,
                      float* boxes, float* scores, int32_t* labels, int32_t* counts, int outputs_on_device);
+
+/* Same call for n images of ANY sizes, resized inside the forward to one target size h x w: the TF 1.x bilinear resize
+ * of utils/image.py:38-147 (lumi_op_resize_bilinear), fused into the kernels that stage the input of the first conv,
+ * bit-identical to lumi_op_resize_bilinear followed by lumi_predict_f32.
+ *   images      n pointers, images[i] RGB [h0_i, w0_i, 3]; all uint8 (is_f32 = 0) or all float32 (1); all host
+ *               pointers (images_on_device = 0) or all device pointers (1)
+ *   sizes       int32 [n][2] host array {h0_i, w0_i}, each >= 1
+ * h x w is the size the caller's preprocessing gives the batch (predicting.target_size); boxes come back in its
+ * pixels.  The sources are packed into an engine-owned device buffer, host sources through an engine-owned pinned
+ * buffer inside the call, so host sources may be reused once the call returns.  Device sources are copied
+ * asynchronously on lumi_stream(e), after any work already queued there: the caller orders its writes of them before
+ * the call (e.g. an event the engine's stream waits on) and, with outputs_on_device = 1, must not overwrite them until
+ * that stream has passed the call.  The rest is as lumi_predict. */
+int lumi_predict_resize(lumi_engine* e, const void* const* images, const int32_t* sizes, int is_f32,
+                        int images_on_device, int n, int h, int w, float* boxes, float* scores, int32_t* labels,
+                        int32_t* counts, int outputs_on_device);
 
 int lumi_max_detections(lumi_engine* e);
 

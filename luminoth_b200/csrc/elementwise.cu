@@ -4,43 +4,13 @@
 
 namespace lumi {
 
-// uint8 RGB image -> (optionally mean-subtracted) fp16x2 planes.
-// base_network.py:153-177 (`inputs - [means]`, only for resnet*/vgg* architectures).
-template <typename PIX>
-__global__ void u8_to_act_kernel(const PIX* __restrict__ img, __half* __restrict__ hi, __half* __restrict__ lo,
-                                 size_t numel, int c, float m0, float m1, float m2) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= numel) return;
-  int ch = (int)(i % c);
-  float mean = ch == 0 ? m0 : (ch == 1 ? m1 : m2);
-  float v = __fsub_rn((float)img[i], mean);
-  __half h, l;
-  split_f32(v, h, l);
-  hi[i] = h; lo[i] = l;
-}
-void launch_u8_to_act(const void* img, bool img_f32, Act out, const float* means, cudaStream_t st) {
-  size_t n = out.numel();
-  if (!n) return;
-  float m0 = means ? means[0] : 0.f, m1 = means ? means[1] : 0.f, m2 = means ? means[2] : 0.f;
-  if (img_f32)
-    u8_to_act_kernel<float><<<(unsigned)cdiv64(n, 256), 256, 0, st>>>(static_cast<const float*>(img), out.hi, out.lo, n,
-                                                                      out.c, m0, m1, m2);
-  else
-    u8_to_act_kernel<uint8_t><<<(unsigned)cdiv64(n, 256), 256, 0, st>>>(static_cast<const uint8_t*>(img), out.hi,
-                                                                        out.lo, n, out.c, m0, m1, m2);
-  count_launch();
-  LUMI_CUDA_CHECK(cudaGetLastError());
-}
-
 // tf.image.resize_images(BILINEAR) of TF 1.x (legacy kernel: align_corners=False, src = dst * (in / out), no
 // half-pixel offset) -- luminoth/utils/image.py:94-97,139-142.  Same float32 operation order as the oracle
-// (tf_ops.resize_bilinear), no FMA contraction, so the result is bit-identical to it.
+// (tf_ops.resize_bilinear), no FMA contraction, so the result is bit-identical to it.  Pixel (y, x) of the h x w
+// output of the h0 x w0 HWC image src, hs = h0 / h and ws = w0 / w in float32.
 template <typename PIX>
-__global__ void resize_bilinear_kernel(const PIX* __restrict__ src, int h0, int w0, float* __restrict__ dst, int h, int w,
-                                       float hs, float ws) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (size_t)h * w) return;
-  const int x = (int)(i % w), y = (int)(i / w);
+__device__ __forceinline__ void bilinear_sample(const PIX* __restrict__ src, int h0, int w0, float hs, float ws, int y,
+                                                int x, float (&v)[3]) {
   const float fy = __fmul_rn((float)y, hs), fx = __fmul_rn((float)x, ws);
   const int y0 = (int)floorf(fy), x0 = (int)floorf(fx);
   const int y1 = min(y0 + 1, h0 - 1), x1 = min(x0 + 1, w0 - 1);
@@ -51,8 +21,18 @@ __global__ void resize_bilinear_kernel(const PIX* __restrict__ src, int h0, int 
     const float bl = (float)src[((size_t)y1 * w0 + x0) * 3 + c], br = (float)src[((size_t)y1 * w0 + x1) * 3 + c];
     const float top = __fadd_rn(tl, __fmul_rn(__fsub_rn(tr, tl), xl));
     const float bot = __fadd_rn(bl, __fmul_rn(__fsub_rn(br, bl), xl));
-    dst[i * 3 + c] = __fadd_rn(top, __fmul_rn(__fsub_rn(bot, top), yl));
+    v[c] = __fadd_rn(top, __fmul_rn(__fsub_rn(bot, top), yl));
   }
+}
+
+template <typename PIX>
+__global__ void resize_bilinear_kernel(const PIX* __restrict__ src, int h0, int w0, float* __restrict__ dst, int h, int w,
+                                       float hs, float ws) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)h * w) return;
+  float v[3];
+  bilinear_sample(src, h0, w0, hs, ws, (int)(i / w), (int)(i % w), v);
+  dst[i * 3] = v[0]; dst[i * 3 + 1] = v[1]; dst[i * 3 + 2] = v[2];
 }
 void launch_resize_bilinear(const void* src, bool src_f32, int h0, int w0, float* dst, int h, int w, cudaStream_t st) {
   if (!h || !w) return;
@@ -68,12 +48,73 @@ void launch_resize_bilinear(const void* src, bool src_f32, int h0, int w0, float
   LUMI_CUDA_CHECK(cudaGetLastError());
 }
 
+// Pixel sources of the input staging kernels: pixel (y, x) of image ni of the h x w batch the network sees.
+// DirectPixels: the batch itself, [n][h][w][3].
+template <typename PIX>
+struct DirectPixels {
+  const PIX* img;
+  int h, w;
+  __device__ __forceinline__ void load(int ni, int y, int x, float (&v)[3]) const {
+    const PIX* p = img + (((size_t)ni * h + y) * w + x) * 3;
+    v[0] = (float)p[0]; v[1] = (float)p[1]; v[2] = (float)p[2];
+  }
+};
+// ResizedPixels: image ni is the source table[ni] locates in `base`, resized to h x w on the fly -- the values
+// launch_resize_bilinear writes, so a fused staging is bit-identical to resize-then-stage.
+template <typename PIX>
+struct ResizedPixels {
+  const uint8_t* base;
+  const ResizeSrc* table;
+  __device__ __forceinline__ void load(int ni, int y, int x, float (&v)[3]) const {
+    const ResizeSrc t = table[ni];
+    bilinear_sample(reinterpret_cast<const PIX*>(base + t.off), t.h0, t.w0, t.hs, t.ws, y, x, v);
+  }
+};
+// Calls launch(pixels) with the source policy `src` describes.
+template <typename F>
+void with_pixels(const ImgSrc& src, int h, int w, F&& launch) {
+  if (src.table) {
+    const uint8_t* base = static_cast<const uint8_t*>(src.img);
+    if (src.f32) launch(ResizedPixels<float>{base, src.table});
+    else launch(ResizedPixels<uint8_t>{base, src.table});
+  } else {
+    if (src.f32) launch(DirectPixels<float>{static_cast<const float*>(src.img), h, w});
+    else launch(DirectPixels<uint8_t>{static_cast<const uint8_t*>(src.img), h, w});
+  }
+}
+
+// RGB image -> (optionally mean-subtracted) fp16x2 planes, one pixel per thread.
+// base_network.py:153-177 (`inputs - [means]`, only for resnet*/vgg* architectures).
+template <typename SRC>
+__global__ void u8_to_act_kernel(SRC src, __half* __restrict__ hi, __half* __restrict__ lo, int n, int h, int w,
+                                 float m0, float m1, float m2) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)n * h * w) return;
+  const int x = (int)(i % w), y = (int)((i / w) % h), ni = (int)(i / ((size_t)w * h));
+  float v[3];
+  src.load(ni, y, x, v);
+  split_f32(__fsub_rn(v[0], m0), hi[i * 3], lo[i * 3]);
+  split_f32(__fsub_rn(v[1], m1), hi[i * 3 + 1], lo[i * 3 + 1]);
+  split_f32(__fsub_rn(v[2], m2), hi[i * 3 + 2], lo[i * 3 + 2]);
+}
+void launch_u8_to_act(ImgSrc src, Act out, const float* means, cudaStream_t st) {
+  LUMI_REQUIRE(out.c == 3, "u8_to_act: the staged image has 3 channels");
+  const size_t total = (size_t)out.n * out.h * out.w;
+  if (!total) return;
+  const float m0 = means ? means[0] : 0.f, m1 = means ? means[1] : 0.f, m2 = means ? means[2] : 0.f;
+  with_pixels(src, out.h, out.w, [&](auto px) {
+    u8_to_act_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(px, out.hi, out.lo, out.n, out.h, out.w, m0, m1, m2);
+  });
+  count_launch();
+  LUMI_CUDA_CHECK(cudaGetLastError());
+}
+
 // Space-to-depth staging of the 7x7/2 stem (slim conv2d_same: zero pad 3/3 AFTER mean subtraction):
 // X2[n][Y][X][dy*6 + dx*3 + c] = xp[2Y+dy][2X+dx][c], xp = padded (image - mean); channels 12..15 = 0.
 // The stem then is a 4x4/1 VALID conv over X2 that the tensor-core kernel runs as 4 taps of K = 64.
-template <typename PIX>
-__global__ void stem_s2d_kernel(const PIX* __restrict__ img, __half* __restrict__ hi, __half* __restrict__ lo, int n,
-                                int h, int w, int h2, int w2, float m0, float m1, float m2) {
+template <typename SRC>
+__global__ void stem_s2d_kernel(SRC src, __half* __restrict__ hi, __half* __restrict__ lo, int n, int h, int w, int h2,
+                                int w2, float m0, float m1, float m2) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   size_t total = (size_t)n * h2 * w2;
   if (i >= total) return;
@@ -89,8 +130,9 @@ __global__ void stem_s2d_kernel(const PIX* __restrict__ img, __half* __restrict_
     for (int dx = 0; dx < 2; ++dx) {
       const int py = 2 * Y + dy - 3, px = 2 * X + dx - 3;
       if (py >= 0 && py < h && px >= 0 && px < w) {
-        const PIX* p = img + (((size_t)ni * h + py) * w + px) * 3;
-        const float v0 = __fsub_rn((float)p[0], m0), v1 = __fsub_rn((float)p[1], m1), v2 = __fsub_rn((float)p[2], m2);
+        float p[3];
+        src.load(ni, py, px, p);
+        const float v0 = __fsub_rn(p[0], m0), v1 = __fsub_rn(p[1], m1), v2 = __fsub_rn(p[2], m2);
         const int o = dy * 6 + dx * 3;
         split_f32(v0, ph[o], pl[o]); split_f32(v1, ph[o + 1], pl[o + 1]); split_f32(v2, ph[o + 2], pl[o + 2]);
       }
@@ -99,15 +141,13 @@ __global__ void stem_s2d_kernel(const PIX* __restrict__ img, __half* __restrict_
   uint4* ol = reinterpret_cast<uint4*>(lo + i * 16);
   oh[0] = vh[0]; oh[1] = vh[1]; ol[0] = vl[0]; ol[1] = vl[1];
 }
-void launch_stem_s2d(const void* img, bool img_f32, int n, int h, int w, Act x2, const float* means, cudaStream_t st) {
+void launch_stem_s2d(ImgSrc src, int n, int h, int w, Act x2, const float* means, cudaStream_t st) {
   size_t total = (size_t)n * x2.h * x2.w;
   if (!total) return;
-  if (img_f32)
-    stem_s2d_kernel<float><<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(static_cast<const float*>(img), x2.hi, x2.lo, n,
-                                                                         h, w, x2.h, x2.w, means[0], means[1], means[2]);
-  else
-    stem_s2d_kernel<uint8_t><<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(static_cast<const uint8_t*>(img), x2.hi, x2.lo,
-                                                                           n, h, w, x2.h, x2.w, means[0], means[1], means[2]);
+  with_pixels(src, h, w, [&](auto px) {
+    stem_s2d_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(px, x2.hi, x2.lo, n, h, w, x2.h, x2.w, means[0],
+                                                                  means[1], means[2]);
+  });
   count_launch();
   LUMI_CUDA_CHECK(cudaGetLastError());
 }
@@ -115,9 +155,9 @@ void launch_stem_s2d(const void* img, bool img_f32, int n, int h, int w, Act x2,
 // SSD conv1_1 (3x3, C_in = 3) staging for the tensor-core path: zero-padded image with 16-channel
 // pixels (3 real), so that the 64 contiguous fp16 starting at pixel (y, x) are the filter-row window
 // x-1 .. x+2 of row y-1 (the 4th pixel meets zero weights).  uint8 values are exact in fp16: lo = 0.
-template <typename PIX>
-__global__ void pack_c3_kernel(const PIX* __restrict__ img, __half* __restrict__ hi, __half* __restrict__ lo, int n,
-                               int h, int w, int h2, int w2) {
+template <typename SRC>
+__global__ void pack_c3_kernel(SRC src, __half* __restrict__ hi, __half* __restrict__ lo, int n, int h, int w, int h2,
+                               int w2) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   size_t total = (size_t)n * h2 * w2;
   if (i >= total) return;
@@ -129,24 +169,22 @@ __global__ void pack_c3_kernel(const PIX* __restrict__ img, __half* __restrict__
   for (int j = 0; j < 16; ++j) { ph[j] = __float2half_rn(0.f); pl[j] = __float2half_rn(0.f); }
   const int py = Y - 1, px = X - 1;
   if (py >= 0 && py < h && px >= 0 && px < w) {
-    const PIX* p = img + (((size_t)ni * h + py) * w + px) * 3;
+    float p[3];
+    src.load(ni, py, px, p);
     // uint8 pixels are exact in fp16 (lo = 0); resized float pixels keep their low part
-    split_f32((float)p[0], ph[0], pl[0]); split_f32((float)p[1], ph[1], pl[1]); split_f32((float)p[2], ph[2], pl[2]);
+    split_f32(p[0], ph[0], pl[0]); split_f32(p[1], ph[1], pl[1]); split_f32(p[2], ph[2], pl[2]);
   }
   uint4* oh = reinterpret_cast<uint4*>(hi + i * 16);
   uint4* ol = reinterpret_cast<uint4*>(lo + i * 16);
   oh[0] = vh[0]; oh[1] = vh[1];
   ol[0] = vl[0]; ol[1] = vl[1];
 }
-void launch_pack_c3(const void* img, bool img_f32, int n, int h, int w, Act x2, cudaStream_t st) {
+void launch_pack_c3(ImgSrc src, int n, int h, int w, Act x2, cudaStream_t st) {
   size_t total = (size_t)n * x2.h * x2.w;
   if (!total) return;
-  if (img_f32)
-    pack_c3_kernel<float><<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(static_cast<const float*>(img), x2.hi, x2.lo, n, h,
-                                                                        w, x2.h, x2.w);
-  else
-    pack_c3_kernel<uint8_t><<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(static_cast<const uint8_t*>(img), x2.hi, x2.lo,
-                                                                          n, h, w, x2.h, x2.w);
+  with_pixels(src, h, w, [&](auto px) {
+    pack_c3_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(px, x2.hi, x2.lo, n, h, w, x2.h, x2.w);
+  });
   count_launch();
   LUMI_CUDA_CHECK(cudaGetLastError());
 }

@@ -167,6 +167,11 @@ struct lumi_engine {
   int conv_pipe = CONV_PIPE_DEFAULT;    // env LUMI_CONV_PIPE: 1 = double-buffered slice accumulators in the conv mainloop (slower on R50, DESIGN 7.1)
   int conv_epi_tma = 1;         // env LUMI_CONV_EPI_TMA: 1 = split outputs through the shared-memory slot epilogue, 0 = register epilogue
   uint8_t* d_images = nullptr; size_t images_cap = 0;
+  // lumi_predict_resize: the packed sources (device arena and its pinned host staging) and their table
+  uint8_t* d_src = nullptr; size_t src_cap = 0;
+  uint8_t* h_src = nullptr; size_t h_src_cap = 0;
+  ResizeSrc* d_resize_tab = nullptr;             // [max_batch]
+  cudaEvent_t ev_src[2] = {nullptr, nullptr};    // after each half's upload from h_src (h_src is reused once they pass)
   float* d_boxes = nullptr; float* d_scores = nullptr; int* d_labels = nullptr; int* d_counts = nullptr;
   int* d_prop_counts = nullptr;
   float* d_records = nullptr;   // caller-owned device buffer [max_batch][1 + 6*kmax] (lumi_set_record_output) or null
@@ -174,11 +179,11 @@ struct lumi_engine {
   int planned_n = 0, planned_h = 0, planned_w = 0;
   // CUDA graphs: one captured graph per (half-)batch forward, keyed by everything baked into its nodes
   struct GraphKey {
-    int half, n, h, w, esz, img_off, conv_impl, streamk, reserve;
+    int half, n, h, w, esz, resize, img_off, conv_impl, streamk, reserve;
     const void* records;
     bool operator<(const GraphKey& o) const {
-      return std::tie(half, n, h, w, esz, img_off, conv_impl, streamk, reserve, records) <
-             std::tie(o.half, o.n, o.h, o.w, o.esz, o.img_off, o.conv_impl, o.streamk, o.reserve, o.records);
+      return std::tie(half, n, h, w, esz, resize, img_off, conv_impl, streamk, reserve, records) <
+             std::tie(o.half, o.n, o.h, o.w, o.esz, o.resize, o.img_off, o.conv_impl, o.streamk, o.reserve, o.records);
     }
   };
   struct GraphEntry { cudaGraphExec_t exec = nullptr; int launches = 0; int seen = 0; };
@@ -205,6 +210,9 @@ struct lumi_engine {
     cudaFree(d_anchor_ref); cudaFree(d_final_keys); cudaFree(d_ssd_anchors);
     for (auto& kv : anchor_grids) cudaFree(kv.second);
     cudaFree(arena.base); cudaFree(arena2.base); cudaFree(d_final_keys2); cudaFree(d_overflow); cudaFree(d_images);
+    cudaFree(d_src); cudaFree(d_resize_tab);
+    if (h_src) cudaFreeHost(h_src);
+    for (auto ev : ev_src) if (ev) cudaEventDestroy(ev);
     if (ev_fork) cudaEventDestroy(ev_fork);
     if (ev_join) cudaEventDestroy(ev_join);
     if (stream2) cudaStreamDestroy(stream2);
@@ -748,6 +756,7 @@ struct Ctx {
   ConvWorkspace* sk = nullptr;  // stream-K scratch of this stream
   bool taps = true;             // record debug taps (first half only)
   bool img_f32 = false;         // input pixels are float32 (resized images) instead of uint8
+  const ResizeSrc* resize = nullptr;  // per-image source table of a fused resize (lumi_predict_resize), else null
   int sm_reserve = 0;           // SMs the persistent conv launches of this forward leave to the other stream
   Act act(int n, int h, int w, int c) {
     Act a; a.n = n; a.h = h; a.w = w; a.c = c;
@@ -757,6 +766,7 @@ struct Ctx {
     return a;
   }
   float* f32(size_t count) { return (float*)arena->alloc(count * sizeof(float), dry); }
+  ImgSrc pixels(const void* images) const { return ImgSrc{images, img_f32, resize}; }
   void tap_f32(const std::string& name, const float* p, int64_t a, int64_t b, int64_t c, int64_t d) {
     if (!taps) return;
     Tap t; t.ptr = p; t.kind = 0; t.shape[0] = a; t.shape[1] = b; t.shape[2] = c; t.shape[3] = d;
@@ -953,14 +963,14 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
     // stem on the tensor cores: mean-subtract + zero-pad + space-to-depth staging, then 4 taps of K=64
     const int ho = (h + 6 - 7) / 2 + 1, wo = (w + 6 - 7) / 2 + 1;
     Act x2 = cx.act(n, ho + 3, wo + 3, 16);
-    if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_stem_s2d(images, cx.img_f32, n, h, w, x2, RGB_MEANS, cx.st); }
+    if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_stem_s2d(cx.pixels(images), n, h, w, x2, RGB_MEANS, cx.st); }
     Act view = x2;                      // Toeplitz view: pixel (y, x) -> the 64 contiguous fp16 starting at x2[y][x]
     view.w = wo; view.c = 64;
     const long pitch[3] = {16, (long)(wo + 3) * 16, (long)(ho + 3) * (wo + 3) * 16};
     x = run_conv(cx, root + "/conv1#s2d", view, nullptr, 1, nullptr, pitch, 2.0 * n * ho * wo * 147.0 * 64.0);
   } else {
     x = cx.act(n, h, w, 3);
-    if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_u8_to_act(images, cx.img_f32, x, RGB_MEANS, cx.st); }  // base_network.py:153-177
+    if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_u8_to_act(cx.pixels(images), x, RGB_MEANS, cx.st); }  // base_network.py:153-177
     x = run_conv(cx, root + "/conv1", x, nullptr, 1, nullptr);           // conv2d_same(64, 7, stride 2) + BN + relu
   }                                                                      // (v2: + bias, no activation)
   cx.tap_act("stem", x);
@@ -1173,7 +1183,7 @@ void forward_ssd(Ctx& cx, const void* images, int n, int h, int w) {
   if (c11_tc) {
     // conv1_1 on the tensor cores: zero-padded 16-channel staging, Toeplitz view, 3 filter rows of K=64
     Act x2 = cx.act(n, h + 2, w + 3, 16);
-    if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_pack_c3(images, cx.img_f32, n, h, w, x2, cx.st); }   // no mean subtraction (quirk Q7)
+    if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_pack_c3(cx.pixels(images), n, h, w, x2, cx.st); }   // no mean subtraction (quirk Q7)
     Act view = x2;
     view.w = w; view.c = 64;
     const long pitch[3] = {16, (long)(w + 3) * 16, (long)(h + 2) * (w + 3) * 16};
@@ -1181,7 +1191,7 @@ void forward_ssd(Ctx& cx, const void* images, int n, int h, int w) {
     cx.tap_act("conv1_1", x);
   } else {
     x = cx.act(n, h, w, 3);
-    if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_u8_to_act(images, cx.img_f32, x, nullptr, cx.st); }  // no mean subtraction (quirk Q7)
+    if (!cx.dry) { ProfScope ps(cx.e, cx.dry, PC_PREP); launch_u8_to_act(cx.pixels(images), x, nullptr, cx.st); }  // no mean subtraction (quirk Q7)
   }
   Act fmaps[6];
   for (int b = 0; b < 5; ++b) {
@@ -1440,7 +1450,7 @@ int lumi_finalize(lumi_engine* e) {
 static void run_forward(lumi_engine* e, Ctx& cx, int half, const void* images, int n, int h, int w, int esz) {
   const bool graphable = e->use_graphs && !e->profile && !e->debug_taps;
   if (!graphable) { forward(cx, images, n, h, w); return; }
-  lumi_engine::GraphKey key{half, n, h, w, esz, cx.img_off, e->conv_impl, e->conv_streamk, cx.sm_reserve, e->d_records};
+  lumi_engine::GraphKey key{half, n, h, w, esz, cx.resize != nullptr, cx.img_off, e->conv_impl, e->conv_streamk, cx.sm_reserve, e->d_records};
   lumi_engine::GraphEntry& ent = e->graphs[key];
   if (ent.exec) {
     LUMI_CUDA_CHECK(cudaGraphLaunch(ent.exec, cx.st));
@@ -1471,14 +1481,94 @@ static void run_forward(lumi_engine* e, Ctx& cx, int half, const void* images, i
   e->graph_replays++;
 }
 
-static int predict_impl(lumi_engine* e, const void* images, int esz, int images_on_device, int n, int h, int w,
-                        float* boxes, float* scores, int* labels, int* counts, int outputs_on_device) {
+// The pixels of one predict call: n images of the batch's size h x w in one dense [n,h,w,3] buffer (sources == null),
+// or n sources of any sizes, sources[i] of sizes[2i] x sizes[2i+1], that the staging kernels resize to h x w.
+struct PredictInput {
+  const void* images = nullptr;
+  const void* const* sources = nullptr;
+  const int32_t* sizes = nullptr;
+  int esz = 1;                  // bytes per channel value: 1 uint8, 4 float32
+  int on_device = 0;
+};
+
+// One copy of a half-batch's upload; with `pack`, the host source is first copied from there into src (pinned), so
+// the packing of the next image overlaps this one's transfer.
+struct Upload { void* dst; const void* src; size_t bytes; cudaMemcpyKind kind; const void* pack = nullptr; };
+
+// Device buffer of at least `need` bytes; growing it drops the graphs, whose nodes point into the old buffer.
+static void ensure_device_buffer(lumi_engine* e, uint8_t*& buf, size_t& cap, size_t need) {
+  if (need <= cap) return;
+  e->drop_graphs();
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+  if (e->stream2) LUMI_CUDA_CHECK(cudaStreamSynchronize(e->stream2));
+  cudaFree(buf);
+  buf = nullptr; cap = 0;
+  LUMI_CUDA_CHECK(cudaMalloc(&buf, need));
+  cap = need;
+}
+
+static size_t round16(size_t b) { return (b + 15) / 16 * 16; }
+
+// lumi_predict_resize's staging: packs the n sources in batch order, 16 B aligned, into the device arena e->d_src,
+// writes their table rows, and lists the copies of images [0, nA) in up[0] and of [nA, n) in up[1].  The table rows
+// and host sources go through the pinned buffer e->h_src, which is rewritten only after the last upload from it;
+// the host sources are packed into it as their half is uploaded.
+static void stage_resize(lumi_engine* e, const PredictInput& in, int n, int nA, int h, int w,
+                         std::vector<Upload> (&up)[2]) {
+  std::vector<size_t> off(n + 1, 0);
+  for (int i = 0; i < n; ++i) off[i + 1] = off[i] + round16((size_t)in.sizes[2 * i] * in.sizes[2 * i + 1] * 3 * in.esz);
+  ensure_device_buffer(e, e->d_src, e->src_cap, off[n]);
+  if (!e->d_resize_tab) {
+    LUMI_CUDA_CHECK(cudaMalloc(&e->d_resize_tab, (size_t)e->max_batch * sizeof(ResizeSrc)));
+    for (auto& ev : e->ev_src) LUMI_CUDA_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  }
+  const size_t tab_bytes = round16((size_t)n * sizeof(ResizeSrc));
+  const size_t pinned = tab_bytes + (in.on_device ? 0 : off[n]);
+  for (auto ev : e->ev_src) LUMI_CUDA_CHECK(cudaEventSynchronize(ev));
+  if (pinned > e->h_src_cap) {
+    if (e->h_src) cudaFreeHost(e->h_src);
+    e->h_src = nullptr; e->h_src_cap = 0;
+    LUMI_CUDA_CHECK(cudaHostAlloc((void**)&e->h_src, pinned, cudaHostAllocDefault));
+    e->h_src_cap = pinned;
+  }
+  ResizeSrc* rows = reinterpret_cast<ResizeSrc*>(e->h_src);
+  uint8_t* host_src = e->h_src + tab_bytes;
+  for (int i = 0; i < n; ++i) {
+    const int h0 = in.sizes[2 * i], w0 = in.sizes[2 * i + 1];
+    rows[i] = ResizeSrc{(long long)off[i], h0, w0, (float)h0 / (float)h, (float)w0 / (float)w};  // as launch_resize_bilinear
+  }
+  const int bounds[3] = {0, nA, n};
+  for (int k = 0; k < 2; ++k) {
+    const int b = bounds[k], t = bounds[k + 1];
+    if (b == t) continue;
+    up[k].push_back({e->d_resize_tab + b, rows + b, (size_t)(t - b) * sizeof(ResizeSrc), cudaMemcpyHostToDevice});
+    for (int i = b; i < t; ++i) {
+      const size_t bytes = (size_t)in.sizes[2 * i] * in.sizes[2 * i + 1] * 3 * in.esz;
+      if (in.on_device) up[k].push_back({e->d_src + off[i], in.sources[i], bytes, cudaMemcpyDeviceToDevice});
+      else up[k].push_back({e->d_src + off[i], host_src + off[i], bytes, cudaMemcpyHostToDevice, in.sources[i]});
+    }
+  }
+}
+
+static int predict_impl(lumi_engine* e, const PredictInput& in, int n, int h, int w, float* boxes, float* scores,
+                        int* labels, int* counts, int outputs_on_device) {
   if (!e) return LUMI_EINVAL;
   LUMI_API_BEGIN
   if (!e->finalized) throw Error(LUMI_ESTATE, "lumi_predict before lumi_finalize");
-  LUMI_REQUIRE(images && boxes && scores && labels && counts, "lumi_predict: null buffer");
+  const bool resize = in.sources != nullptr;
+  LUMI_REQUIRE((in.images || resize) && boxes && scores && labels && counts, "lumi_predict: null buffer");
   LUMI_REQUIRE(n > 0 && n <= e->max_batch, "lumi_predict: batch size exceeds max_batch");
   LUMI_REQUIRE(h > 0 && w > 0, "lumi_predict: empty image");
+  if (resize) {
+    LUMI_REQUIRE(in.sizes, "lumi_predict_resize: null sizes");
+    for (int i = 0; i < n; ++i) {
+      const int h0 = in.sizes[2 * i], w0 = in.sizes[2 * i + 1];
+      LUMI_REQUIRE(h0 >= 1 && w0 >= 1, "lumi_predict_resize: source image " + std::to_string(i) + " is " +
+                                           std::to_string(h0) + " x " + std::to_string(w0) + ", sizes must be >= 1");
+      LUMI_REQUIRE((long long)h0 * w0 < (1LL << 30), "lumi_predict_resize: source image too large");
+      LUMI_REQUIRE(in.sources[i], "lumi_predict_resize: null source image " + std::to_string(i));
+    }
+  }
   LUMI_CUDA_CHECK(cudaSetDevice(e->device));
   ensure_image_capacity(e, h, w);
   // software pipelining: two half-batches on two streams (off while profiling / tapping intermediates)
@@ -1493,30 +1583,40 @@ static int predict_impl(lumi_engine* e, const void* images, int esz, int images_
     if (piped) ensure_arena(e, e->arena2, need_bytes);
     e->planned_n = plan_key; e->planned_h = h; e->planned_w = w;
   }
-  const uint8_t* dimg = static_cast<const uint8_t*>(images);
-  const size_t img_bytes = (size_t)n * h * w * 3 * esz;
-  const size_t bytes_a = (size_t)nA * h * w * 3 * esz;
-  // graphs read their pixels from the engine's own staging buffer (a caller's device pointer changes per call)
-  const bool graphs_on = e->use_graphs && !e->profile && !e->debug_taps;
-  const bool stage = !images_on_device || graphs_on;
-  if (stage) {
-    if (img_bytes > e->images_cap) {
-      e->drop_graphs();
-      LUMI_CUDA_CHECK(cudaStreamSynchronize(e->stream));
-      if (e->stream2) LUMI_CUDA_CHECK(cudaStreamSynchronize(e->stream2));
-      cudaFree(e->d_images);
-      e->d_images = nullptr; e->images_cap = 0;
-      LUMI_CUDA_CHECK(cudaMalloc(&e->d_images, img_bytes));
-      e->images_cap = img_bytes;
+  // what each half uploads on its own stream, and where its forward reads its pixels
+  std::vector<Upload> up[2];
+  const uint8_t *img_a, *img_b;
+  if (resize) {
+    stage_resize(e, in, n, nA, h, w, up);
+    img_a = img_b = e->d_src;                      // the table rows hold the offsets
+  } else {
+    const size_t img_bytes = (size_t)n * h * w * 3 * in.esz;
+    const size_t bytes_a = (size_t)nA * h * w * 3 * in.esz;
+    // graphs read their pixels from the engine's own staging buffer (a caller's device pointer changes per call)
+    const bool graphs_on = e->use_graphs && !e->profile && !e->debug_taps;
+    const uint8_t* dimg = static_cast<const uint8_t*>(in.images);
+    if (!in.on_device || graphs_on) {
+      ensure_device_buffer(e, e->d_images, e->images_cap, img_bytes);
+      const cudaMemcpyKind kind = in.on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+      up[0].push_back({e->d_images, dimg, bytes_a, kind});
+      if (nB) up[1].push_back({e->d_images + bytes_a, dimg + bytes_a, img_bytes - bytes_a, kind});
+      dimg = e->d_images;
     }
-    dimg = e->d_images;
+    img_a = dimg; img_b = dimg + bytes_a;
   }
-  const cudaMemcpyKind up = images_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+  auto upload = [&](int half, cudaStream_t st) {
+    for (const Upload& u : up[half]) {
+      if (u.pack) std::memcpy(const_cast<void*>(u.src), u.pack, u.bytes);
+      LUMI_CUDA_CHECK(cudaMemcpyAsync(u.dst, u.src, u.bytes, u.kind, st));
+    }
+    if (resize) LUMI_CUDA_CHECK(cudaEventRecord(e->ev_src[half], st));
+  };
   g_launch_count = 0;
   e->graph_replays = 0;
   if (e->type == "fasterrcnn") ensure_frcnn_anchors(e, h, w, e->stream);
   Ctx cx = make_ctx(e, false, 0);
-  cx.img_f32 = esz == 4;
+  cx.img_f32 = in.esz == 4;
+  cx.resize = resize ? e->d_resize_tab : nullptr;
   cx.sm_reserve = piped ? CONV_PIPELINE_SM_RESERVE : 0;
   if (piped) {
     LUMI_CUDA_CHECK(cudaEventRecord(e->ev_fork, e->stream));
@@ -1524,20 +1624,19 @@ static int predict_impl(lumi_engine* e, const void* images, int esz, int images_
     Ctx cb = make_ctx(e, false, 1);
     cb.img_off = nA;
     cb.img_f32 = cx.img_f32;
+    cb.resize = resize ? e->d_resize_tab + nA : nullptr;
     cb.sm_reserve = cx.sm_reserve;
-    // each half uploads its own images on its own stream: the second half's H2D overlaps the first half's kernels
-    if (stage) {
-      LUMI_CUDA_CHECK(cudaMemcpyAsync(e->d_images, images, bytes_a, up, e->stream));
-      LUMI_CUDA_CHECK(cudaMemcpyAsync(e->d_images + bytes_a, static_cast<const uint8_t*>(images) + bytes_a,
-                                      img_bytes - bytes_a, up, e->stream2));
-    }
-    run_forward(e, cx, 0, dimg, nA, h, w, esz);
-    run_forward(e, cb, 1, dimg + bytes_a, nB, h, w, esz);
+    // each half uploads its own images (and table rows) on its own stream, before its forward or graph launch: the
+    // second half's host work and H2D overlap the first half's kernels
+    upload(0, e->stream);
+    run_forward(e, cx, 0, img_a, nA, h, w, in.esz);
+    upload(1, e->stream2);
+    run_forward(e, cb, 1, img_b, nB, h, w, in.esz);
     LUMI_CUDA_CHECK(cudaEventRecord(e->ev_join, e->stream2));
     LUMI_CUDA_CHECK(cudaStreamWaitEvent(e->stream, e->ev_join, 0));
   } else {
-    if (stage) LUMI_CUDA_CHECK(cudaMemcpyAsync(e->d_images, images, img_bytes, up, e->stream));
-    run_forward(e, cx, 0, dimg, n, h, w, esz);
+    upload(0, e->stream);
+    run_forward(e, cx, 0, img_a, n, h, w, in.esz);
   }
   e->launches = g_launch_count;
   const size_t k = (size_t)e->kmax;
@@ -1561,12 +1660,26 @@ static int predict_impl(lumi_engine* e, const void* images, int esz, int images_
 
 int lumi_predict(lumi_engine* e, const void* images, int images_on_device, int n, int h, int w, float* boxes,
                  float* scores, int* labels, int* counts, int outputs_on_device) {
-  return predict_impl(e, images, 1, images_on_device, n, h, w, boxes, scores, labels, counts, outputs_on_device);
+  PredictInput in;
+  in.images = images; in.esz = 1; in.on_device = images_on_device;
+  return predict_impl(e, in, n, h, w, boxes, scores, labels, counts, outputs_on_device);
 }
 
 int lumi_predict_f32(lumi_engine* e, const float* images, int images_on_device, int n, int h, int w, float* boxes,
                      float* scores, int* labels, int* counts, int outputs_on_device) {
-  return predict_impl(e, images, 4, images_on_device, n, h, w, boxes, scores, labels, counts, outputs_on_device);
+  PredictInput in;
+  in.images = images; in.esz = 4; in.on_device = images_on_device;
+  return predict_impl(e, in, n, h, w, boxes, scores, labels, counts, outputs_on_device);
+}
+
+int lumi_predict_resize(lumi_engine* e, const void* const* images, const int32_t* sizes, int is_f32,
+                        int images_on_device, int n, int h, int w, float* boxes, float* scores, int* labels,
+                        int* counts, int outputs_on_device) {
+  if (!e) return LUMI_EINVAL;
+  if (!images) return fail(e, LUMI_EINVAL, "lumi_predict_resize: null images");
+  PredictInput in;
+  in.sources = images; in.sizes = sizes; in.esz = is_f32 ? 4 : 1; in.on_device = images_on_device;
+  return predict_impl(e, in, n, h, w, boxes, scores, labels, counts, outputs_on_device);
 }
 
 int lumi_max_detections(lumi_engine* e) { return e ? e->kmax : 0; }

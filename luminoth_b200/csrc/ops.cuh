@@ -5,12 +5,26 @@
 namespace lumi {
 
 // ---- format conversion / preprocessing (elementwise.cu)
-void launch_u8_to_act(const void* img, bool img_f32, Act out, const float* means /*3 or nullptr*/, cudaStream_t st);
+// One source image of a fused resize: its first byte at `off` in the source buffer, h0 x w0 RGB pixels, resized to the
+// batch's h x w with the scale factors hs = (float)h0 / h, ws = (float)w0 / w (as launch_resize_bilinear computes them).
+struct ResizeSrc {
+  long long off;
+  int h0, w0;
+  float hs, ws;
+};
+// The pixels the input staging kernels read: with table == nullptr, img is the batch itself [n][h][w][3]; otherwise
+// image i of the batch is table[i]'s source in img, bilinearly resized on the fly.  f32: float32 pixels, else uint8.
+struct ImgSrc {
+  const void* img;
+  bool f32;
+  const ResizeSrc* table;
+};
+void launch_u8_to_act(ImgSrc src, Act out /*(n,h,w,3)*/, const float* means /*3 or nullptr*/, cudaStream_t st);
 void launch_f32_to_act(const float* x, Act out, cudaStream_t st);
 // x2: (n, Ho+3, Wo+3, 16) space-to-depth staging of the 7x7/2 stem input (see elementwise.cu)
-void launch_stem_s2d(const void* img, bool img_f32, int n, int h, int w, Act x2, const float* means, cudaStream_t st);
+void launch_stem_s2d(ImgSrc src, int n, int h, int w, Act x2, const float* means, cudaStream_t st);
 void launch_resize_bilinear(const void* src, bool src_f32, int h0, int w0, float* dst, int h, int w, cudaStream_t st);
-void launch_pack_c3(const void* img, bool img_f32, int n, int h, int w, Act x2 /*(n,h+2,w+3,16)*/, cudaStream_t st);
+void launch_pack_c3(ImgSrc src, int n, int h, int w, Act x2 /*(n,h+2,w+3,16)*/, cudaStream_t st);
 void launch_act_to_f32(Act in, float* y, cudaStream_t st);
 // pre_scale / pre_bias [c] (both or neither): out = relu(BN(max)) instead of the max (see elementwise.cu)
 void launch_max_pool(Act in, Act out, int k, int stride, int pad_t, int pad_l, cudaStream_t st,

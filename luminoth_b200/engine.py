@@ -40,6 +40,8 @@ SIGNATURES = {
                                     ctypes.c_int]),
     'lumi_predict_f32': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]),
+    'lumi_predict_resize': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 5 +
+                            [ctypes.c_void_p] * 4 + [ctypes.c_int]),
     'lumi_max_detections': (ctypes.c_int, [ctypes.c_void_p]),
     'lumi_set_record_output': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
     'lumi_stream': (ctypes.c_void_p, [ctypes.c_void_p]),
@@ -266,6 +268,66 @@ class Engine(object):
             rc = fn(self._h, ctypes.c_void_p(ptr), int(on_dev), n, h, w,
                     boxes.ctypes.data_as(ctypes.c_void_p), scores.ctypes.data_as(ctypes.c_void_p),
                     labels.ctypes.data_as(ctypes.c_void_p), counts.ctypes.data_as(ctypes.c_void_p), 0)
+            if rc != LUMI_OK:
+                _raise(rc, self._lib.lumi_last_error(self._h))
+        return boxes, scores, labels, counts
+
+    def predict_resize(self, images, h, w):
+        """Like ``predict_raw`` for a list of (h0, w0, 3) images of any sizes, resized to h x w inside the forward
+        (``lumi_predict_resize``): bit-identical to ``lumi_op_resize_bilinear`` per image followed by ``predict_raw``
+        on the float32 batch.  The images are all numpy arrays (host path) or all CUDA torch tensors (device path),
+        and all uint8 or all float32 (numpy arrays of other dtypes are read as float32).  CUDA tensors must be on the
+        engine's device and may be non-contiguous (they are copied); the engine reads them after the work queued so far
+        on torch's current stream of that device, which is what wrote them.  Returns numpy (boxes [n,K,4] in h x w
+        pixels, scores [n,K], labels [n,K], counts [n])."""
+        images = list(images)
+        n = len(images)
+        if n == 0:
+            raise ValueError('predict_resize: no images')
+        on_dev = [not isinstance(im, np.ndarray) for im in images]
+        if any(on_dev) != all(on_dev):
+            raise ValueError('predict_resize: the images must be all numpy arrays or all CUDA tensors')
+        if on_dev[0]:
+            import torch
+            for im in images:
+                if not im.is_cuda or im.dtype not in (torch.uint8, torch.float32):
+                    raise ValueError('predict_resize: device images must be CUDA uint8 or float32 tensors')
+                if im.device.index != self.device:
+                    raise ValueError('predict_resize: image on %s, the engine runs on cuda:%d' % (im.device, self.device))
+            f32 = [im.dtype == torch.float32 for im in images]
+            srcs = [im.contiguous() for im in images]
+            ptrs = [s.data_ptr() for s in srcs]
+        else:
+            f32 = [im.dtype != np.uint8 for im in images]
+            srcs = [np.ascontiguousarray(im, dtype=np.float32 if f else np.uint8) for im, f in zip(images, f32)]
+            ptrs = [s.ctypes.data for s in srcs]
+        if any(f32) != all(f32):
+            raise ValueError('predict_resize: the images of one call must share a dtype (uint8 or float32)')
+        for s in srcs:
+            if len(s.shape) != 3 or s.shape[2] != 3:
+                raise ValueError('predict_resize: images must be (h0, w0, 3) RGB')
+        ptr_arr = (ctypes.c_void_p * n)(*ptrs)
+        sizes = np.array([s.shape[:2] for s in srcs], np.int32)
+        k = self.max_detections
+        boxes = np.empty((n, k, 4), np.float32)
+        scores = np.empty((n, k), np.float32)
+        labels = np.empty((n, k), np.int32)
+        counts = np.empty((n,), np.int32)
+        with self._lock:
+            if on_dev[0]:
+                # the engine's streams do not follow torch's: make its stream wait for the work torch has queued on
+                # the device's current stream (the caller's writes of the images, the copies of .contiguous()); the
+                # call returns synchronised, so srcs outlive the engine's reads
+                dev = torch.device('cuda', self.device)
+                ready = torch.cuda.Event()
+                ready.record(torch.cuda.current_stream(dev))
+                torch.cuda.ExternalStream(self.stream, device=dev).wait_event(ready)
+            rc = self._lib.lumi_predict_resize(self._h, ptr_arr, sizes.ctypes.data_as(ctypes.c_void_p), int(f32[0]),
+                                               int(on_dev[0]), n, int(h), int(w),
+                                               boxes.ctypes.data_as(ctypes.c_void_p),
+                                               scores.ctypes.data_as(ctypes.c_void_p),
+                                               labels.ctypes.data_as(ctypes.c_void_p),
+                                               counts.ctypes.data_as(ctypes.c_void_p), 0)
             if rc != LUMI_OK:
                 _raise(rc, self._lib.lumi_last_error(self._h))
         return boxes, scores, labels, counts

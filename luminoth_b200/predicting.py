@@ -6,13 +6,14 @@ rounded to 4 decimals).  ``predict_batch(images)`` is the batched extension
 (the reference is hard-wired to batch 1, ``fasterrcnn.py:101-103``).
 
 What changed underneath: graph build + ``session.run`` is one call into the
-sm_90a engine (``lumi_predict`` / ``lumi_predict_f32``).  The aspect-preserving
+sm_90a engine (``lumi_predict`` / ``lumi_predict_resize``).  The aspect-preserving
 resize of ``datasets/object_detection_dataset.py:71-83`` / ``utils/image.py:38-147``
-runs on the GPU (``lumi_op_resize_bilinear``, bit-identical to the TF1 legacy
-bilinear kernel); only its size arithmetic (float32, like the reference) stays on
-the host.  Images of different sizes in one ``predict_batch`` call are bucketed by
-their preprocessed size, each bucket runs as one batched engine call, and the
-results come back in the caller's order.
+runs inside the engine's forward (``lumi_predict_resize`` samples the TF1 legacy
+bilinear kernel, bit-identically, in the kernels that stage the first conv's input);
+only its size arithmetic (float32, like the reference) stays on the host.  Images
+of different sizes in one ``predict_batch`` call are bucketed by their
+preprocessed size, each bucket runs as one batched engine call, and the results
+come back in the caller's order.
 """
 import json
 import math
@@ -64,7 +65,7 @@ def target_size(shape, config):
 
 def preprocess_image(image, config):
     """Inference preprocessing on the host (numpy); returns (float32 image, scale_factor).  The product path
-    resizes on the GPU (``PredictorNetwork._resize_on_device``); this restatement is its cross-check."""
+    resizes inside the engine (``Engine.predict_resize``); this restatement is its cross-check."""
     image = np.asarray(image)
     if image.ndim != 3 or image.shape[2] != 3:
         raise ValueError('expected an (H, W, 3) RGB image')
@@ -181,29 +182,14 @@ class PredictorNetwork(object):
             for s in range(0, len(idxs), self.engine.max_batch):
                 chunk = idxs[s:s + self.engine.max_batch]
                 if untouched:   # integer pixels, no resize: the uint8 entry point (the benchmark shapes)
-                    batch = np.stack([images[i] for i in chunk])
-                else:           # the reference feeds the resized FLOAT image (predicting.py:110-112)
-                    batch = self._resize_on_device([images[i] for i in chunk], nh, nw)
-                boxes, scores, labels, counts = self.engine.predict_raw(batch)
+                    res = self.engine.predict_raw(np.stack([images[i] for i in chunk]))
+                else:           # the reference feeds the resized FLOAT image (predicting.py:110-112): resized in
+                    srcs = [images[i] for i in chunk]     # the engine's input staging, one call per chunk
+                    if any(im.dtype != np.uint8 for im in srcs):
+                        srcs = [im.astype(np.float32, copy=False) for im in srcs]   # uint8 -> float32 is exact
+                    res = self.engine.predict_resize(srcs, nh, nw)
+                boxes, scores, labels, counts = res
                 for j, i in enumerate(chunk):
                     k = int(counts[j])
                     out[i] = (boxes[j, :k].copy(), labels[j, :k].copy(), scores[j, :k].copy(), sizes[i][2])
         return out
-
-    def _resize_on_device(self, images, nh, nw):
-        """``resize_image`` / ``resize_image_fixed`` (utils/image.py:38-147) on the GPU: legacy TF bilinear kernel,
-        bit-identical to the float32 host restatement; returns a CUDA float32 tensor [n, nh, nw, 3]."""
-        import ctypes
-        import torch
-        lib = self.engine._lib
-        dev = torch.device('cuda', self.engine.device)
-        batch = torch.empty((len(images), nh, nw, 3), dtype=torch.float32, device=dev)
-        for i, im in enumerate(images):
-            is_f32 = im.dtype != np.uint8
-            src = torch.from_numpy(np.ascontiguousarray(im, dtype=np.float32 if is_f32 else np.uint8)).to(dev)
-            rc = lib.lumi_op_resize_bilinear(ctypes.c_void_p(src.data_ptr()), int(is_f32), im.shape[0], im.shape[1],
-                                             ctypes.c_void_p(batch[i].data_ptr()), nh, nw, None)
-            if rc != 0:
-                raise RuntimeError(lib.lumi_op_last_error().decode())
-        torch.cuda.synchronize(dev)
-        return batch
