@@ -90,6 +90,18 @@ int lumi_predict_resize(lumi_engine* e, const void* const* images, const int32_t
                         int images_on_device, int n, int h, int w, float* boxes, float* scores, int32_t* labels,
                         int32_t* counts, int outputs_on_device);
 
+/* lumi_predict_resize with one target size per image: source i is resized to targets[i] = {th_i, tw_i} (int32 [n][2]
+ * host array, each >= 1), and its boxes come back in th_i x tw_i pixels.  Every image runs in one forward, at the top
+ * left of a canvas of the largest target height and width (it may exceed max_h x max_w; the workspace grows).  Each
+ * image's results are those of the call with that image alone: the staging and a band clear ahead of every windowed
+ * conv give it the zero padding it has alone, and pool1, the RPN, the ROI pool and the detections use its own size.
+ * When every target is equal this is lumi_predict_resize (same kernels, same bytes).  Faster R-CNN only: SSD takes the
+ * call only when every target is its fixed size.  A network with a layer whose padding would differ between an image
+ * and the canvas returns LUMI_EINVAL.  The rest is as lumi_predict_resize. */
+int lumi_predict_sizes(lumi_engine* e, const void* const* images, const int32_t* sizes, const int32_t* targets,
+                       int is_f32, int images_on_device, int n, float* boxes, float* scores, int32_t* labels,
+                       int32_t* counts, int outputs_on_device);
+
 int lumi_max_detections(lumi_engine* e);
 
 /* Multi-GPU detection exchange (SURVEY 8e; the reference has no counterpart -- it predicts one image at a time,

@@ -54,17 +54,22 @@ template <typename PIX>
 struct DirectPixels {
   const PIX* img;
   int h, w;
+  __device__ __forceinline__ bool inside(int, int, int) const { return true; }
   __device__ __forceinline__ void load(int ni, int y, int x, float (&v)[3]) const {
     const PIX* p = img + (((size_t)ni * h + y) * w + x) * 3;
     v[0] = (float)p[0]; v[1] = (float)p[1]; v[2] = (float)p[2];
   }
 };
-// ResizedPixels: image ni is the source table[ni] locates in `base`, resized to h x w on the fly -- the values
-// launch_resize_bilinear writes, so a fused staging is bit-identical to resize-then-stage.
-template <typename PIX>
+// ResizedPixels: image ni is the source table[ni] locates in `base`, resized to its target on the fly -- the values
+// launch_resize_bilinear writes, so a fused staging is bit-identical to resize-then-stage.  PACKED: the batch is a
+// canvas, and only the pixels inside image ni's target th x tw are the image's.
+template <typename PIX, bool PACKED>
 struct ResizedPixels {
   const uint8_t* base;
   const ResizeSrc* table;
+  __device__ __forceinline__ bool inside(int ni, int y, int x) const {
+    return !PACKED || (y < table[ni].th && x < table[ni].tw);
+  }
   __device__ __forceinline__ void load(int ni, int y, int x, float (&v)[3]) const {
     const ResizeSrc t = table[ni];
     bilinear_sample(reinterpret_cast<const PIX*>(base + t.off), t.h0, t.w0, t.hs, t.ws, y, x, v);
@@ -75,8 +80,13 @@ template <typename F>
 void with_pixels(const ImgSrc& src, int h, int w, F&& launch) {
   if (src.table) {
     const uint8_t* base = static_cast<const uint8_t*>(src.img);
-    if (src.f32) launch(ResizedPixels<float>{base, src.table});
-    else launch(ResizedPixels<uint8_t>{base, src.table});
+    if (src.packed) {
+      if (src.f32) launch(ResizedPixels<float, true>{base, src.table});
+      else launch(ResizedPixels<uint8_t, true>{base, src.table});
+    } else {
+      if (src.f32) launch(ResizedPixels<float, false>{base, src.table});
+      else launch(ResizedPixels<uint8_t, false>{base, src.table});
+    }
   } else {
     if (src.f32) launch(DirectPixels<float>{static_cast<const float*>(src.img), h, w});
     else launch(DirectPixels<uint8_t>{static_cast<const uint8_t*>(src.img), h, w});
@@ -91,6 +101,12 @@ __global__ void u8_to_act_kernel(SRC src, __half* __restrict__ hi, __half* __res
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)n * h * w) return;
   const int x = (int)(i % w), y = (int)((i / w) % h), ni = (int)(i / ((size_t)w * h));
+  if (!src.inside(ni, y, x)) {                    // canvas padding: the image's zero padding after mean subtraction
+    const __half z = __float2half_rn(0.f);
+    hi[i * 3] = hi[i * 3 + 1] = hi[i * 3 + 2] = z;
+    lo[i * 3] = lo[i * 3 + 1] = lo[i * 3 + 2] = z;
+    return;
+  }
   float v[3];
   src.load(ni, y, x, v);
   split_f32(__fsub_rn(v[0], m0), hi[i * 3], lo[i * 3]);
@@ -129,7 +145,7 @@ __global__ void stem_s2d_kernel(SRC src, __half* __restrict__ hi, __half* __rest
 #pragma unroll
     for (int dx = 0; dx < 2; ++dx) {
       const int py = 2 * Y + dy - 3, px = 2 * X + dx - 3;
-      if (py >= 0 && py < h && px >= 0 && px < w) {
+      if (py >= 0 && py < h && px >= 0 && px < w && src.inside(ni, py, px)) {
         float p[3];
         src.load(ni, py, px, p);
         const float v0 = __fsub_rn(p[0], m0), v1 = __fsub_rn(p[1], m1), v2 = __fsub_rn(p[2], m2);
@@ -168,7 +184,7 @@ __global__ void pack_c3_kernel(SRC src, __half* __restrict__ hi, __half* __restr
 #pragma unroll
   for (int j = 0; j < 16; ++j) { ph[j] = __float2half_rn(0.f); pl[j] = __float2half_rn(0.f); }
   const int py = Y - 1, px = X - 1;
-  if (py >= 0 && py < h && px >= 0 && px < w) {
+  if (py >= 0 && py < h && px >= 0 && px < w && src.inside(ni, py, px)) {
     float p[3];
     src.load(ni, py, px, p);
     // uint8 pixels are exact in fp16 (lo = 0); resized float pixels keep their low part
@@ -243,12 +259,16 @@ void launch_act_to_f32(Act in, float* y, cudaStream_t st) {
 // Padded cells are ignored (TF pads with -inf).
 // PRE: writes p = relu(fmaf(m^, pre_scale[c], pre_bias[c])) instead of the max m, with m^ = m as split and rejoined
 // (the batch norm follows the max: a negative gamma does not commute with it).
-template <bool PRE>
+// PACKED: image ni of a canvas batch -- its own input extent and SAME front padding (tab, in_stride), and 0 past its
+// own output extent.
+template <bool PRE, bool PACKED>
 __global__ void max_pool_kernel(const __half* __restrict__ ihi, const __half* __restrict__ ilo,
                                 __half* __restrict__ ohi, __half* __restrict__ olo, int n, int h, int w, int c,
                                 int ho, int wo, int k, int stride, int pad_t, int pad_l,
-                                const float* __restrict__ pre_scale, const float* __restrict__ pre_bias) {
+                                const float* __restrict__ pre_scale, const float* __restrict__ pre_bias,
+                                const ResizeSrc* __restrict__ tab, int in_stride) {
   const int cv = c >> 3;
+  const int hc = h, wc = w;                       // the input's layout; h x w: the extent the window may read
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   size_t total = (size_t)n * ho * wo * cv;
   if (i >= total) return;
@@ -257,6 +277,20 @@ __global__ void max_pool_kernel(const __half* __restrict__ ihi, const __half* __
   int ox = (int)(p % wo);
   int oy = (int)((p / wo) % ho);
   int ni = (int)(p / ((size_t)wo * ho));
+  if constexpr (PACKED) {
+    const int th = tab[ni].th, tw = tab[ni].tw;
+    h = (th + in_stride - 1) / in_stride;
+    w = (tw + in_stride - 1) / in_stride;
+    const int oh = (h + stride - 1) / stride, ow = (w + stride - 1) / stride;
+    if (oy >= oh || ox >= ow) {
+      const size_t ooff = p * c + (size_t)c8 * 8;
+      *reinterpret_cast<uint4*>(ohi + ooff) = make_uint4(0u, 0u, 0u, 0u);
+      *reinterpret_cast<uint4*>(olo + ooff) = make_uint4(0u, 0u, 0u, 0u);
+      return;
+    }
+    pad_t = max((oh - 1) * stride + k - h, 0) / 2;
+    pad_l = max((ow - 1) * stride + k - w, 0) / 2;
+  }
   float best[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) best[j] = -INFINITY;
@@ -266,7 +300,7 @@ __global__ void max_pool_kernel(const __half* __restrict__ ihi, const __half* __
     for (int s = 0; s < k; ++s) {
       int ix = ox * stride + s - pad_l;
       if (ix < 0 || ix >= w) continue;
-      size_t off = (((size_t)ni * h + iy) * w + ix) * c + (size_t)c8 * 8;
+      size_t off = (((size_t)ni * hc + iy) * wc + ix) * c + (size_t)c8 * 8;
       uint4 vh = *reinterpret_cast<const uint4*>(ihi + off);
       uint4 vl = *reinterpret_cast<const uint4*>(ilo + off);
       const __half* ph = reinterpret_cast<const __half*>(&vh);
@@ -291,17 +325,61 @@ __global__ void max_pool_kernel(const __half* __restrict__ ihi, const __half* __
   *reinterpret_cast<uint4*>(olo + ooff) = ol;
 }
 void launch_max_pool(Act in, Act out, int k, int stride, int pad_t, int pad_l, cudaStream_t st,
-                     const float* pre_scale, const float* pre_bias) {
+                     const float* pre_scale, const float* pre_bias, const ResizeSrc* tab, int in_stride) {
   LUMI_REQUIRE(in.c % 8 == 0 && in.c == out.c && in.n == out.n, "max_pool: C must be a multiple of 8");
   LUMI_REQUIRE(!pre_scale == !pre_bias, "max_pool: pre_scale and pre_bias go together");
+  LUMI_REQUIRE(!tab || in_stride > 0, "max_pool: a packed batch needs the input stride");
   size_t total = (size_t)out.n * out.h * out.w * (out.c / 8);
   if (!total) return;
-  if (pre_scale)
-    max_pool_kernel<true><<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(
-        in.hi, in.lo, out.hi, out.lo, in.n, in.h, in.w, in.c, out.h, out.w, k, stride, pad_t, pad_l, pre_scale, pre_bias);
-  else
-    max_pool_kernel<false><<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(
-        in.hi, in.lo, out.hi, out.lo, in.n, in.h, in.w, in.c, out.h, out.w, k, stride, pad_t, pad_l, nullptr, nullptr);
+  const unsigned grid = (unsigned)cdiv64(total, 256);
+  auto go = [&](auto kernel) {
+    kernel<<<grid, 256, 0, st>>>(in.hi, in.lo, out.hi, out.lo, in.n, in.h, in.w, in.c, out.h, out.w, k, stride, pad_t,
+                                 pad_l, pre_scale, pre_bias, tab, in_stride);
+  };
+  if (tab) {
+    if (pre_scale) go(max_pool_kernel<true, true>);
+    else go(max_pool_kernel<false, true>);
+  } else {
+    if (pre_scale) go(max_pool_kernel<true, false>);
+    else go(max_pool_kernel<false, false>);
+  }
+  count_launch();
+  LUMI_CUDA_CHECK(cudaGetLastError());
+}
+
+// Band clear of a packed batch: along each axis, image ni's valid outputs of the conv read input cells up to
+// max_read = (out - 1) * stride - pad + k_eff - 1, out = ceil(ext / stride) (SAME and conv2d_same alike), ext = the
+// image's extent ceil(t / in_stride).  Cells [ext, min(max_read + 1, canvas)) are the zero padding the image has alone;
+// the canvas holds other values there.  Grid (., n): the first bh * w pixels are the candidate rows ext .. ext+bh-1, the
+// next h * bw the candidate columns; 8 channels per thread.
+__global__ void band_clear_kernel(__half* __restrict__ hi, __half* __restrict__ lo, int h, int w, int c,
+                                  const ResizeSrc* __restrict__ tab, int in_stride, int keff_h, int keff_w, int stride,
+                                  int pad_t, int pad_l, int bh, int bw) {
+  const int ni = blockIdx.y, cv = c >> 3;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t rows = (size_t)bh * w * cv;
+  if (i >= rows + (size_t)h * bw * cv) return;
+  const int ext_h = (tab[ni].th + in_stride - 1) / in_stride, ext_w = (tab[ni].tw + in_stride - 1) / in_stride;
+  const int end_h = min(((ext_h + stride - 1) / stride - 1) * stride - pad_t + keff_h, h);
+  const int end_w = min(((ext_w + stride - 1) / stride - 1) * stride - pad_l + keff_w, w);
+  const int c8 = (int)(i % cv);
+  int y, x;
+  if (i < rows) { const size_t p = i / cv; y = ext_h + (int)(p / w); x = (int)(p % w); if (y >= end_h) return; }
+  else { const size_t p = (i - rows) / cv; y = (int)(p / bw); x = ext_w + (int)(p % bw); if (x >= end_w) return; }
+  const size_t off = (((size_t)ni * h + y) * w + x) * c + (size_t)c8 * 8;
+  *reinterpret_cast<uint4*>(hi + off) = make_uint4(0u, 0u, 0u, 0u);
+  *reinterpret_cast<uint4*>(lo + off) = make_uint4(0u, 0u, 0u, 0u);
+}
+void launch_band_clear(Act a, const ResizeSrc* tab, int in_stride, int kh, int kw, int stride, int rate, int pad_t,
+                       int pad_l, cudaStream_t st) {
+  LUMI_REQUIRE(a.c % 8 == 0 && tab && in_stride > 0, "band_clear: C must be a multiple of 8 (internal)");
+  const int keff_h = kh + (kh - 1) * (rate - 1), keff_w = kw + (kw - 1) * (rate - 1);
+  // (out - 1) * stride <= ext - 1, so the band is at most k_eff - 1 - pad cells wide
+  const int bh = keff_h - 1 - pad_t > 0 ? keff_h - 1 - pad_t : 0, bw = keff_w - 1 - pad_l > 0 ? keff_w - 1 - pad_l : 0;
+  const size_t total = ((size_t)bh * a.w + (size_t)a.h * bw) * (a.c / 8);
+  if (!total || !a.n) return;
+  band_clear_kernel<<<dim3((unsigned)cdiv64(total, 256), a.n), 256, 0, st>>>(a.hi, a.lo, a.h, a.w, a.c, tab, in_stride,
+                                                                             keff_h, keff_w, stride, pad_t, pad_l, bh, bw);
   count_launch();
   LUMI_CUDA_CHECK(cudaGetLastError());
 }

@@ -179,11 +179,12 @@ struct lumi_engine {
   int planned_n = 0, planned_h = 0, planned_w = 0;
   // CUDA graphs: one captured graph per (half-)batch forward, keyed by everything baked into its nodes
   struct GraphKey {
-    int half, n, h, w, esz, resize, img_off, conv_impl, streamk, reserve;
+    int half, n, h, w, esz, resize, packed, img_off, conv_impl, streamk, reserve;
     const void* records;
     bool operator<(const GraphKey& o) const {
-      return std::tie(half, n, h, w, esz, resize, img_off, conv_impl, streamk, reserve, records) <
-             std::tie(o.half, o.n, o.h, o.w, o.esz, o.resize, o.img_off, o.conv_impl, o.streamk, o.reserve, o.records);
+      return std::tie(half, n, h, w, esz, resize, packed, img_off, conv_impl, streamk, reserve, records) <
+             std::tie(o.half, o.n, o.h, o.w, o.esz, o.resize, o.packed, o.img_off, o.conv_impl, o.streamk, o.reserve,
+                      o.records);
     }
   };
   struct GraphEntry { cudaGraphExec_t exec = nullptr; int launches = 0; int seen = 0; };
@@ -757,6 +758,12 @@ struct Ctx {
   bool taps = true;             // record debug taps (first half only)
   bool img_f32 = false;         // input pixels are float32 (resized images) instead of uint8
   const ResizeSrc* resize = nullptr;  // per-image source table of a fused resize (lumi_predict_resize), else null
+  // A packed batch (lumi_predict_sizes): image i sits at the top left of the h x w canvas, resize[i] holds its size.
+  // fstride: the feature stride of the trunk map the next run_conv reads (0 where nothing is packed: the stem, which
+  // the staging pads, and the ROI tail); run_conv clears each image's band ahead of a windowed conv there.
+  bool packed = false;
+  int fstride = 0;
+  const int32_t* targets = nullptr;   // host [n][2] targets of the whole call: the padding check of a dry forward
   int sm_reserve = 0;           // SMs the persistent conv launches of this forward leave to the other stream
   Act act(int n, int h, int w, int c) {
     Act a; a.n = n; a.h = h; a.w = w; a.c = c;
@@ -766,7 +773,7 @@ struct Ctx {
     return a;
   }
   float* f32(size_t count) { return (float*)arena->alloc(count * sizeof(float), dry); }
-  ImgSrc pixels(const void* images) const { return ImgSrc{images, img_f32, resize}; }
+  ImgSrc pixels(const void* images) const { return ImgSrc{images, img_f32, resize, packed}; }
   void tap_f32(const std::string& name, const float* p, int64_t a, int64_t b, int64_t c, int64_t d) {
     if (!taps) return;
     Tap t; t.ptr = p; t.kind = 0; t.shape[0] = a; t.shape[1] = b; t.shape[2] = c; t.shape[3] = d;
@@ -847,6 +854,28 @@ Act run_conv(Ctx& cx, const std::string& key, Act in, const Act* res, int res_st
     wo = tf_valid(in.w, L.kw, L.stride, L.rate);
   }
   LUMI_REQUIRE(ho > 0 && wo > 0, "conv '" + key + "': input too small");
+  if (cx.packed && cx.fstride > 0) {
+    // Every image at the top left of the canvas gives the same outputs as alone only where the layer pads the front
+    // of each image as it pads the canvas (true of every conv the Faster R-CNN trunk and RPN have; pool1 is per image)
+    const int keff_h = L.kh + (L.kh - 1) * (L.rate - 1), keff_w = L.kw + (L.kw - 1) * (L.rate - 1);
+    for (int i = 0; cx.targets && i < in.n; ++i) {
+      const int ih = cdiv(cx.targets[2 * i], cx.fstride), iw = cdiv(cx.targets[2 * i + 1], cx.fstride);
+      int oh_i, ow_i, pt_i = (keff_h - 1) / 2, pl_i = (keff_w - 1) / 2;
+      if (R.padding == PAD_SAME || (R.padding == PAD_CONV2D_SAME && L.stride == 1)) {
+        tf_same(ih, L.kh, L.stride, L.rate, oh_i, pt_i);
+        tf_same(iw, L.kw, L.stride, L.rate, ow_i, pl_i);
+      } else if (R.padding == PAD_VALID) {
+        pt_i = pl_i = 0;
+      }
+      if (pt_i != pt || pl_i != pl)
+        throw Error(LUMI_EINVAL, "lumi_predict_sizes: conv '" + key + "' pads image " + std::to_string(i) +
+                                     " unlike the canvas; predict these sizes in separate calls");
+    }
+    if (!cx.dry && L.kh * L.kw > 1) {
+      ProfScope ps(cx.e, cx.dry, PC_PREP, 0.0, "band_clear");
+      launch_band_clear(in, cx.resize, cx.fstride, L.kh, L.kw, L.stride, L.rate, pt, pl, cx.st);
+    }
+  }
   io.pad_t = pt; io.pad_l = pl; io.ho = ho; io.wo = wo;
   Act out; out.n = in.n; out.h = ho; out.w = wo; out.c = L.cout;
   if (out_f32) {
@@ -894,7 +923,8 @@ Act run_pool(Ctx& cx, Act in, int k, int stride, bool same, const PreAct* pre = 
   Act out = cx.act(in.n, ho, wo, in.c);
   if (!cx.dry) {
     ProfScope ps(cx.e, cx.dry, PC_POOL);
-    launch_max_pool(in, out, k, stride, pt, pl, cx.st, pre ? pre->scale : nullptr, pre ? pre->bias : nullptr);
+    launch_max_pool(in, out, k, stride, pt, pl, cx.st, pre ? pre->scale : nullptr, pre ? pre->bias : nullptr,
+                    cx.packed ? cx.resize : nullptr, cx.fstride);  // packed: each image's own SAME padding
   }
   return out;
 }
@@ -906,6 +936,7 @@ Act run_pool(Ctx& cx, Act in, int k, int stride, bool same, const PreAct* pre = 
 // conv output instead of the unit's.
 Act bottleneck_v2(Ctx& cx, const std::string& s, Act x, Act p, int depth, PreAct* next, int stop = UP_UNIT) {
   if (stop == UP_SHORTCUT) return run_conv(cx, s + "/shortcut", p, nullptr, 1, nullptr);
+  const int fstride = cx.fstride;
   Act shortcut = x;
   int res_stride = 1;
   if (stop == UP_UNIT) {
@@ -915,6 +946,7 @@ Act bottleneck_v2(Ctx& cx, const std::string& s, Act x, Act p, int depth, PreAct
   Act r = run_conv(cx, s + "/conv1", p, nullptr, 1, nullptr);
   if (stop == UP_CONV1) return r;
   r = run_conv(cx, s + "/conv2", r, nullptr, 1, nullptr);
+  cx.fstride = fstride * layer(cx.e, s + "/conv2").stride;
   if (stop == UP_CONV2) return r;
   return run_conv(cx, s + "/conv3", r, stop == UP_UNIT ? &shortcut : nullptr, res_stride, nullptr, nullptr, -1.0,
                   next);
@@ -974,11 +1006,13 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
     x = run_conv(cx, root + "/conv1", x, nullptr, 1, nullptr);           // conv2d_same(64, 7, stride 2) + BN + relu
   }                                                                      // (v2: + bias, no activation)
   cx.tap_act("stem", x);
+  if (cx.packed) cx.fstride = 2;
   const Endpoint& ep = e->ep;
   if (ep.block < 0) {
     // the stem conv is the endpoint
   } else if (!v2) {
     x = run_pool(cx, x, 3, 2, true);                                     // pool1 3x3/2 SAME
+    if (cx.packed) cx.fstride = 4;
     for (int b = 0; b <= ep.block; ++b)
       for (int u = 0; u < units[b]; ++u) {
         const bool at_ep = b == ep.block && u == ep.unit;
@@ -989,6 +1023,7 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
     // block1/unit_1 projects from its preact: the stem's pool emits only p = relu(BN(pool1))
     const PreAct first = preact_of(e, unit_scope(e, 0, 0), false);
     Act p = run_pool(cx, x, 3, 2, true, &first);
+    if (cx.packed) cx.fstride = 4;
     x = Act();
     for (int b = 0; b <= ep.block; ++b)
       for (int u = 0; u < units[b]; ++u) {
@@ -1014,7 +1049,9 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
   cx.tap_f32("all_anchors", e->d_anchors, na, 4, 1, 1);
 
   // RPN (rpn.py:136-180): 3x3 conv + act, fused 1x1 heads [cls 2A | bbox 4A], softmax fused into the decode
+  if (cx.packed) cx.fstride = ep.stride;
   Act rf = run_conv(cx, "fasterrcnn/rpn/conv", fmap, nullptr, 1, nullptr);
+  cx.fstride = 0;
   float* heads = nullptr;
   run_conv(cx, "fasterrcnn/rpn/heads", rf, nullptr, 1, &heads);
   const int hc = 6 * e->A;
@@ -1023,6 +1060,7 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
   RpnParams rp = e->rpn;
   rp.na = na; rp.im_h = (float)h; rp.im_w = (float)w; rp.logits = 1;
   rp.cls_stride = hc; rp.cls_off = 0; rp.box_stride = hc; rp.box_off = 2 * e->A;
+  if (cx.packed) { rp.tab = cx.resize; rp.feat_stride = ep.stride; rp.grid_w = fw; }
   const int post = rp.post_nms_top_n;
   float* proposals = cx.f32((size_t)n * post * 4);
   float* pscores = cx.f32((size_t)n * post);
@@ -1069,7 +1107,8 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
     ProfScope ps(cx.e, cx.dry, PC_ROI, bytes);
     launch_act_to_f32(fmap, fmap_f32, cx.st);
     launch_roi_pool(fmap_f32, fmap.n, fmap.h, fmap.w, fmap.c, proposals, prop_counts, post, (float)h, (float)w,
-                    e->pooled_h, e->pooled_w, pooled, fuse_mean ? feat : Act(), cx.st);
+                    e->pooled_h, e->pooled_w, pooled, fuse_mean ? feat : Act(), cx.st, -1,
+                    cx.packed ? cx.resize : nullptr, ep.stride);
   }
   if (need_pooled) cx.tap_act("roi_pool", pooled);
   if (!fuse_mean) {
@@ -1099,6 +1138,7 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
   DetParams dp = e->det;
   dp.r = post; dp.im_h = (float)h; dp.im_w = (float)w;
   dp.prob_stride = C + 1; dp.delta_stride = fcw;
+  if (cx.packed) dp.tab = cx.resize;
   if (!cx.dry) {
     ProfScope ps(cx.e, cx.dry, PC_DET_POST);
     NmsWorkspace wsd = ws_view(e->ws_det, io * C);
@@ -1450,7 +1490,8 @@ int lumi_finalize(lumi_engine* e) {
 static void run_forward(lumi_engine* e, Ctx& cx, int half, const void* images, int n, int h, int w, int esz) {
   const bool graphable = e->use_graphs && !e->profile && !e->debug_taps;
   if (!graphable) { forward(cx, images, n, h, w); return; }
-  lumi_engine::GraphKey key{half, n, h, w, esz, cx.resize != nullptr, cx.img_off, e->conv_impl, e->conv_streamk, cx.sm_reserve, e->d_records};
+  lumi_engine::GraphKey key{half, n, h, w, esz, cx.resize != nullptr, cx.packed, cx.img_off, e->conv_impl,
+                            e->conv_streamk, cx.sm_reserve, e->d_records};
   lumi_engine::GraphEntry& ent = e->graphs[key];
   if (ent.exec) {
     LUMI_CUDA_CHECK(cudaGraphLaunch(ent.exec, cx.st));
@@ -1487,6 +1528,8 @@ struct PredictInput {
   const void* images = nullptr;
   const void* const* sources = nullptr;
   const int32_t* sizes = nullptr;
+  const int32_t* targets = nullptr;   // packed batch (lumi_predict_sizes): image i resized to targets[2i] x [2i+1]
+                                      // at the top left of the h x w canvas; null: every image is h x w
   int esz = 1;                  // bytes per channel value: 1 uint8, 4 float32
   int on_device = 0;
 };
@@ -1535,7 +1578,8 @@ static void stage_resize(lumi_engine* e, const PredictInput& in, int n, int nA, 
   uint8_t* host_src = e->h_src + tab_bytes;
   for (int i = 0; i < n; ++i) {
     const int h0 = in.sizes[2 * i], w0 = in.sizes[2 * i + 1];
-    rows[i] = ResizeSrc{(long long)off[i], h0, w0, (float)h0 / (float)h, (float)w0 / (float)w};  // as launch_resize_bilinear
+    const int th = in.targets ? in.targets[2 * i] : h, tw = in.targets ? in.targets[2 * i + 1] : w;
+    rows[i] = ResizeSrc{(long long)off[i], h0, w0, (float)h0 / (float)th, (float)w0 / (float)tw, th, tw};  // as launch_resize_bilinear
   }
   const int bounds[3] = {0, nA, n};
   for (int k = 0; k < 2; ++k) {
@@ -1555,7 +1599,7 @@ static int predict_impl(lumi_engine* e, const PredictInput& in, int n, int h, in
   if (!e) return LUMI_EINVAL;
   LUMI_API_BEGIN
   if (!e->finalized) throw Error(LUMI_ESTATE, "lumi_predict before lumi_finalize");
-  const bool resize = in.sources != nullptr;
+  const bool resize = in.sources != nullptr, packed = in.targets != nullptr;
   LUMI_REQUIRE((in.images || resize) && boxes && scores && labels && counts, "lumi_predict: null buffer");
   LUMI_REQUIRE(n > 0 && n <= e->max_batch, "lumi_predict: batch size exceeds max_batch");
   LUMI_REQUIRE(h > 0 && w > 0, "lumi_predict: empty image");
@@ -1582,6 +1626,11 @@ static int predict_impl(lumi_engine* e, const PredictInput& in, int n, int h, in
     ensure_arena(e, e->arena, need_bytes);
     if (piped) ensure_arena(e, e->arena2, need_bytes);
     e->planned_n = plan_key; e->planned_h = h; e->planned_w = w;
+  }
+  if (packed) {                                    // every layer's padding per image against the canvas's (host only)
+    Ctx chk = make_ctx(e, true, 0);
+    chk.taps = false; chk.packed = true; chk.targets = in.targets;
+    forward(chk, nullptr, n, h, w);
   }
   // what each half uploads on its own stream, and where its forward reads its pixels
   std::vector<Upload> up[2];
@@ -1617,6 +1666,7 @@ static int predict_impl(lumi_engine* e, const PredictInput& in, int n, int h, in
   Ctx cx = make_ctx(e, false, 0);
   cx.img_f32 = in.esz == 4;
   cx.resize = resize ? e->d_resize_tab : nullptr;
+  cx.packed = packed;
   cx.sm_reserve = piped ? CONV_PIPELINE_SM_RESERVE : 0;
   if (piped) {
     LUMI_CUDA_CHECK(cudaEventRecord(e->ev_fork, e->stream));
@@ -1625,6 +1675,7 @@ static int predict_impl(lumi_engine* e, const PredictInput& in, int n, int h, in
     cb.img_off = nA;
     cb.img_f32 = cx.img_f32;
     cb.resize = resize ? e->d_resize_tab + nA : nullptr;
+    cb.packed = packed;
     cb.sm_reserve = cx.sm_reserve;
     // each half uploads its own images (and table rows) on its own stream, before its forward or graph launch: the
     // second half's host work and H2D overlap the first half's kernels
@@ -1680,6 +1731,33 @@ int lumi_predict_resize(lumi_engine* e, const void* const* images, const int32_t
   PredictInput in;
   in.sources = images; in.sizes = sizes; in.esz = is_f32 ? 4 : 1; in.on_device = images_on_device;
   return predict_impl(e, in, n, h, w, boxes, scores, labels, counts, outputs_on_device);
+}
+
+int lumi_predict_sizes(lumi_engine* e, const void* const* images, const int32_t* sizes, const int32_t* targets,
+                       int is_f32, int images_on_device, int n, float* boxes, float* scores, int* labels, int* counts,
+                       int outputs_on_device) {
+  if (!e) return LUMI_EINVAL;
+  if (!images) return fail(e, LUMI_EINVAL, "lumi_predict_sizes: null images");
+  if (!targets) return fail(e, LUMI_EINVAL, "lumi_predict_sizes: null targets");
+  if (n <= 0 || n > e->max_batch) return fail(e, LUMI_EINVAL, "lumi_predict_sizes: batch size exceeds max_batch");
+  int hc = 0, wc = 0;
+  bool uniform = true;
+  for (int i = 0; i < n; ++i) {
+    const int th = targets[2 * i], tw = targets[2 * i + 1];
+    if (th < 1 || tw < 1)
+      return fail(e, LUMI_EINVAL, "lumi_predict_sizes: target " + std::to_string(i) + " is " + std::to_string(th) +
+                                      " x " + std::to_string(tw) + ", targets must be >= 1");
+    uniform = uniform && th == targets[0] && tw == targets[1];
+    hc = std::max(hc, th); wc = std::max(wc, tw);
+  }
+  PredictInput in;
+  in.sources = images; in.sizes = sizes; in.esz = is_f32 ? 4 : 1; in.on_device = images_on_device;
+  if (!uniform) {                                  // one h x w target is lumi_predict_resize itself
+    if (e->type != "fasterrcnn")
+      return fail(e, LUMI_EINVAL, "lumi_predict_sizes: SSD runs at its fixed size only");
+    in.targets = targets;
+  }
+  return predict_impl(e, in, n, hc, wc, boxes, scores, labels, counts, outputs_on_device);
 }
 
 int lumi_max_detections(lumi_engine* e) { return e ? e->kmax : 0; }

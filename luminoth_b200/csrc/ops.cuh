@@ -5,19 +5,24 @@
 namespace lumi {
 
 // ---- format conversion / preprocessing (elementwise.cu)
-// One source image of a fused resize: its first byte at `off` in the source buffer, h0 x w0 RGB pixels, resized to the
-// batch's h x w with the scale factors hs = (float)h0 / h, ws = (float)w0 / w (as launch_resize_bilinear computes them).
+// One source image of a fused resize: its first byte at `off` in the source buffer, h0 x w0 RGB pixels, resized to its
+// target th x tw with the scale factors hs = (float)h0 / th, ws = (float)w0 / tw (as launch_resize_bilinear computes
+// them).  A uniform batch has th x tw = the batch's h x w; a packed batch (lumi_predict_sizes) places each image at the
+// top left of its h x w canvas, and the per-image kernels below read th x tw from this one table.
 struct ResizeSrc {
   long long off;
   int h0, w0;
   float hs, ws;
+  int th, tw;
 };
 // The pixels the input staging kernels read: with table == nullptr, img is the batch itself [n][h][w][3]; otherwise
 // image i of the batch is table[i]'s source in img, bilinearly resized on the fly.  f32: float32 pixels, else uint8.
+// packed: pixels outside image i's th x tw are the zero padding (0 after the mean subtraction).
 struct ImgSrc {
   const void* img;
   bool f32;
   const ResizeSrc* table;
+  bool packed;
 };
 void launch_u8_to_act(ImgSrc src, Act out /*(n,h,w,3)*/, const float* means /*3 or nullptr*/, cudaStream_t st);
 void launch_f32_to_act(const float* x, Act out, cudaStream_t st);
@@ -27,8 +32,16 @@ void launch_resize_bilinear(const void* src, bool src_f32, int h0, int w0, float
 void launch_pack_c3(ImgSrc src, int n, int h, int w, Act x2 /*(n,h+2,w+3,16)*/, cudaStream_t st);
 void launch_act_to_f32(Act in, float* y, cudaStream_t st);
 // pre_scale / pre_bias [c] (both or neither): out = relu(BN(max)) instead of the max (see elementwise.cu)
+// tab (packed batch, SAME padding only): image i's input extent is ceil(tab[i].th / in_stride) x ceil(tw / in_stride)
+// and its front padding the one SAME gives that extent; outputs past its own output extent are 0
 void launch_max_pool(Act in, Act out, int k, int stride, int pad_t, int pad_l, cudaStream_t st,
-                     const float* pre_scale = nullptr, const float* pre_bias = nullptr);
+                     const float* pre_scale = nullptr, const float* pre_bias = nullptr,
+                     const ResizeSrc* tab = nullptr, int in_stride = 0);
+// Packed batch: zeros the rows and columns of `a` past image i's extent ceil(tab[i].th / in_stride) (and tw) that a
+// conv (kh x kw, stride, rate, front padding pad_t / pad_l) reads from image i's valid outputs -- the zero padding
+// that image has when it runs alone.
+void launch_band_clear(Act a, const ResizeSrc* tab, int in_stride, int kh, int kw, int stride, int rate, int pad_t,
+                       int pad_l, cudaStream_t st);
 void launch_l2norm_scale(Act in, Act out, const float* gamma, float eps, cudaStream_t st);
 void launch_spatial_mean(Act in, Act out, cudaStream_t st);               // (R,h,w,C) -> (R,1,1,C)
 void launch_softmax_rows(const float* x, float* y, int rows, int cols, int in_stride, cudaStream_t st);
@@ -39,8 +52,11 @@ void launch_frcnn_anchors(const int* ref /*A x 4*/, int A, int fh, int fw, int s
 // and/or mean (nimg*rmax, 1, 1, C) = tf.reduce_mean over the pooled cells (either may be an empty Act).
 // fmap_f32: fp32 NHWC copy of the feature map (n, fh, fw, c).  kernel: one of the ROI_* instance codes below, or -1
 // for roi_kernel(c, ph, pw); a code whose shape preconditions fail throws LUMI_EINVAL.
+// tab (packed batch): image i is tab[i].th x tw with a ceil(th / feat_stride) x ceil(tw / feat_stride) feature grid at
+// the top left of the fh x fw map; its rois are normalised and sampled on that grid (im_h / im_w are then unused).
 void launch_roi_pool(const float* fmap_f32, int n, int fh, int fw, int c, const float* rois, const int* counts, int rmax,
-                     float im_h, float im_w, int ph, int pw, Act out, Act mean, cudaStream_t st, int kernel = -1);
+                     float im_h, float im_w, int ph, int pw, Act out, Act mean, cudaStream_t st, int kernel = -1,
+                     const ResizeSrc* tab = nullptr, int feat_stride = 0);
 // Every kernel instance launch_roi_pool can start: the row-walk kernel at 6 / 5 / 4 resident CTAs per SM, the
 // column-walk kernel at 4 / 8 channels per lane, and the round-1 cell kernel roi_pool_kernel<CPL, RB, NW>.
 enum {
@@ -95,6 +111,10 @@ struct RpnParams {
   int filter_outside, clip_after_nms, apply_nms;
   int logits;             // 1: cls input holds logits (softmax fused), 0: probabilities
   int cls_stride, cls_off, box_stride, box_off;  // per-anchor-cell channel layout of the fused head output
+  // packed batch (or nullptr): image i is tab[i].th x tw, its anchors those of the cells inside its
+  // ceil(th / feat_stride) x ceil(tw / feat_stride) grid at the top left of the grid_w cells wide canvas grid
+  const ResizeSrc* tab;
+  int feat_stride, grid_w;
 };
 // cls/box: per image [na/A cells][channels]; anchors [na][4] float. Outputs per image [post_nms_top_n].
 void launch_rpn_proposals(const float* cls, const float* box, long img_stride_cls, long img_stride_box, int A,
@@ -109,6 +129,7 @@ struct DetParams {
   int shared_deltas;      // 1: deltas [r][4] shared by all classes (SSD), 0: [r][4*nc]
   int prob_stride;        // floats between consecutive rows of cls_prob (>= nc+1)
   int delta_stride;       // floats between consecutive rows of deltas
+  const ResizeSrc* tab;   // packed batch: image i is clipped to tab[i].th x tw instead of im_h x im_w (or nullptr)
 };
 size_t det_final_scratch_bytes(int nimg, int nc, int class_max);   // size of `final_keys` below
 // boxes_in [nimg][r][4] (or shared anchors when boxes_img_stride == 0), row_counts [nimg] or nullptr

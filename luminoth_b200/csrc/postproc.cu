@@ -941,8 +941,15 @@ __global__ void rpn_decode_kernel(const float* __restrict__ cls, const float* __
   const float4 an = reinterpret_cast<const float4*>(anchors)[i];
   float4 b = decode_box(an, bp[0], bp[1], bp[2], bp[3], 1.f, 1.f);
   bool ok = (score >= p.min_prob) && area_positive(b);
-  if (p.filter_outside) ok = ok && (an.x >= 0.f && an.y >= 0.f && an.z < p.im_w && an.w < p.im_h);
-  if (!p.clip_after_nms) b = clip_box(b, p.im_h, p.im_w);
+  float im_h = p.im_h, im_w = p.im_w;
+  if (p.tab) {             // packed batch: the image's own size, and only the cells of its own grid
+    const int th = p.tab[img].th, tw = p.tab[img].tw;
+    im_h = (float)th; im_w = (float)tw;
+    const int fh = (th + p.feat_stride - 1) / p.feat_stride, fw = (tw + p.feat_stride - 1) / p.feat_stride;
+    ok = ok && cell / p.grid_w < fh && cell % p.grid_w < fw;
+  }
+  if (p.filter_outside) ok = ok && (an.x >= 0.f && an.y >= 0.f && an.z < im_w && an.w < im_h);
+  if (!p.clip_after_nms) b = clip_box(b, im_h, im_w);
   const size_t o = (size_t)img * cap + i;
   keys[o] = ok ? score : -1.f;
   reinterpret_cast<float4*>(boxes)[o] = b;
@@ -950,8 +957,8 @@ __global__ void rpn_decode_kernel(const float* __restrict__ cls, const float* __
 
 __global__ void rpn_output_kernel(const float* __restrict__ sboxes, const float* __restrict__ sscores,
                                   const int* __restrict__ keep, const int* __restrict__ nkeep, int cap, int max_out,
-                                  int clip, float im_h, float im_w, float* __restrict__ proposals,
-                                  float* __restrict__ scores, int* __restrict__ counts) {
+                                  int clip, float im_h, float im_w, const ResizeSrc* __restrict__ tab,
+                                  float* __restrict__ proposals, float* __restrict__ scores, int* __restrict__ counts) {
   const int img = blockIdx.y;
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const int nk = nkeep[img];
@@ -963,7 +970,7 @@ __global__ void rpn_output_kernel(const float* __restrict__ sboxes, const float*
     const size_t src = (size_t)img * cap + keep[(size_t)img * max_out + j];
     b = reinterpret_cast<const float4*>(sboxes)[src];
     s = sscores[src];
-    if (clip) b = clip_box(b, im_h, im_w);
+    if (clip) b = tab ? clip_box(b, (float)tab[img].th, (float)tab[img].tw) : clip_box(b, im_h, im_w);
   }
   reinterpret_cast<float4*>(proposals)[(size_t)img * max_out + j] = b;
   scores[(size_t)img * max_out + j] = s;
@@ -999,7 +1006,7 @@ void launch_rpn_proposals(const float* cls, const float* box, long img_stride_cl
   run_nms(ws, nimg, thr, p.post_nms_top_n, st);
   dim3 g3(cdiv(p.post_nms_top_n, 256), nimg);
   rpn_output_kernel<<<g3, 256, 0, st>>>(ws.sboxes, ws.sscores, ws.keep, ws.nkeep, ws.ncap, p.post_nms_top_n,
-                                        p.clip_after_nms, p.im_h, p.im_w, proposals, scores, counts);
+                                        p.clip_after_nms, p.im_h, p.im_w, p.tab, proposals, scores, counts);
   count_launch();
   LUMI_CUDA_CHECK(cudaGetLastError());
 }
@@ -1026,7 +1033,7 @@ __global__ void det_decode_kernel(const float* __restrict__ boxes_in, long boxes
   const float* dp = deltas + row * p.delta_stride + (p.shared_deltas ? 0 : 4 * c);
   const float4 bin = reinterpret_cast<const float4*>(boxes_in)[(size_t)img * (boxes_img_stride / 4) + r];
   float4 b = decode_box(bin, dp[0], dp[1], dp[2], dp[3], p.var0, p.var1);
-  b = clip_box(b, p.im_h, p.im_w);
+  b = p.tab ? clip_box(b, (float)p.tab[img].th, (float)p.tab[img].tw) : clip_box(b, p.im_h, p.im_w);
   const bool ok = (prob >= p.min_prob) && area_positive(b);
   keys[o] = ok ? prob : -1.f;
   reinterpret_cast<float4*>(boxes)[o] = b;

@@ -17,12 +17,27 @@ struct RoiArgs {
   int n, fh, fw, c;
   const float* rois; const int* counts; int rmax;
   float im_h, im_w;
+  const ResizeSrc* tab;      // packed batch: image i is tab[i].th x tw on a ceil(th / feat_stride) x ... grid, or nullptr
+  int feat_stride;
   int crop_h, crop_w;        // 2*pw, 2*ph  (sic)
   __half* ohi; __half* olo;  // (n*rmax, crop_h/2, crop_w/2, c) or nullptr (mean only)
   __half* mhi; __half* mlo;  // optional fused tf.reduce_mean over the pooled cells: (n*rmax, c)
 };
 
 struct Samp { int lo, hi; float lerp; int ok; };    // one crop sample coordinate along y or x
+
+// The image size the rois of image img are normalised by, and its feature grid (D - 1 is the crop's last cell): the
+// batch's, or in a packed batch the image's own -- the map's row pitch stays a.fw.
+__device__ __forceinline__ void roi_geometry(const RoiArgs& a, int img, bool is_y, float& im, int& D) {
+  if (a.tab) {
+    const int t = is_y ? a.tab[img].th : a.tab[img].tw;
+    im = (float)t;
+    D = (t + a.feat_stride - 1) / a.feat_stride;
+  } else {
+    im = is_y ? a.im_h : a.im_w;
+    D = is_y ? a.fh : a.fw;
+  }
+}
 
 template <int CPL>
 __device__ __forceinline__ void load8f(const float* f, size_t off, float (&v)[CPL]) {
@@ -91,11 +106,13 @@ __global__ void __launch_bounds__(32 * NW, (CPL == 8 ? 2 : 3) * (8 / NW)) roi_po
     const bool is_y = ts < a.crop_h;
     const int k = is_y ? ts : ts - a.crop_h;
     const float* rb = a.rois + (size_t)row * 4;
+    float im; int D;
+    roi_geometry(a, row / a.rmax, is_y, im, D);
     // normalised box, TF order (y1,x1,y2,x2): divided by the IMAGE size (quirk Q3)
-    const float lo_n = is_y ? __fdiv_rn(rb[1], a.im_h) : __fdiv_rn(rb[0], a.im_w);
-    const float hi_n = is_y ? __fdiv_rn(rb[3], a.im_h) : __fdiv_rn(rb[2], a.im_w);
+    const float lo_n = __fdiv_rn(is_y ? rb[1] : rb[0], im);
+    const float hi_n = __fdiv_rn(is_y ? rb[3] : rb[2], im);
     const int crop = is_y ? a.crop_h : a.crop_w;
-    const float Dm1 = (float)((is_y ? a.fh : a.fw) - 1);
+    const float Dm1 = (float)(D - 1);
     const float step = crop > 1 ? __fdiv_rn(__fmul_rn(__fsub_rn(hi_n, lo_n), Dm1), (float)(crop - 1)) : 0.f;
     const float in = crop > 1 ? __fadd_rn(__fmul_rn(lo_n, Dm1), __fmul_rn((float)k, step))
                               : __fmul_rn(__fmul_rn(0.5f, __fadd_rn(lo_n, hi_n)), Dm1);
@@ -349,10 +366,12 @@ __global__ void __launch_bounds__(32 * WARPS) roi_pool_cols_kernel(const RoiArgs
       const bool is_y = lane < a.crop_h;
       const int k = is_y ? lane : lane - a.crop_h;
       const float* rb = a.rois + (size_t)row * 4;
-      const float lo_n = is_y ? __fdiv_rn(rb[1], a.im_h) : __fdiv_rn(rb[0], a.im_w);
-      const float hi_n = is_y ? __fdiv_rn(rb[3], a.im_h) : __fdiv_rn(rb[2], a.im_w);
+      float im; int D;
+      roi_geometry(a, img, is_y, im, D);
+      const float lo_n = __fdiv_rn(is_y ? rb[1] : rb[0], im);
+      const float hi_n = __fdiv_rn(is_y ? rb[3] : rb[2], im);
       const int crop = is_y ? a.crop_h : a.crop_w;
-      const float Dm1 = (float)((is_y ? a.fh : a.fw) - 1);
+      const float Dm1 = (float)(D - 1);
       const float step = crop > 1 ? __fdiv_rn(__fmul_rn(__fsub_rn(hi_n, lo_n), Dm1), (float)(crop - 1)) : 0.f;
       const float in = crop > 1 ? __fadd_rn(__fmul_rn(lo_n, Dm1), __fmul_rn((float)k, step))
                                 : __fmul_rn(__fmul_rn(0.5f, __fadd_rn(lo_n, hi_n)), Dm1);
@@ -580,10 +599,11 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) roi_pool_rows_kernel(const R
     const bool is_y = lane < a.crop_h;
     const int k = is_y ? lane : lane - a.crop_h;
     const float* rb = a.rois + (size_t)row * 4;
-    const float lo_n = is_y ? __fdiv_rn(rb[1], a.im_h) : __fdiv_rn(rb[0], a.im_w);
-    const float hi_n = is_y ? __fdiv_rn(rb[3], a.im_h) : __fdiv_rn(rb[2], a.im_w);
+    float im; int D;
+    roi_geometry(a, img, is_y, im, D);
+    const float lo_n = __fdiv_rn(is_y ? rb[1] : rb[0], im);
+    const float hi_n = __fdiv_rn(is_y ? rb[3] : rb[2], im);
     const int crop = is_y ? a.crop_h : a.crop_w;
-    const int D = is_y ? a.fh : a.fw;
     const float Dm1 = (float)(D - 1);
     const float step = crop > 1 ? __fdiv_rn(__fmul_rn(__fsub_rn(hi_n, lo_n), Dm1), (float)(crop - 1)) : 0.f;
     const float in = crop > 1 ? __fadd_rn(__fmul_rn(lo_n, Dm1), __fmul_rn((float)k, step))
@@ -677,7 +697,8 @@ int roi_kernel(int c, int ph, int pw) {
 }
 
 void launch_roi_pool(const float* fmap_f32, int n, int fh, int fw, int c, const float* rois, const int* counts, int rmax,
-                     float im_h, float im_w, int ph, int pw, Act out, Act mean, cudaStream_t st, int kernel) {
+                     float im_h, float im_w, int ph, int pw, Act out, Act mean, cudaStream_t st, int kernel,
+                     const ResizeSrc* tab, int feat_stride) {
   LUMI_REQUIRE(c % 8 == 0, "roi_pool: C must be a multiple of 8");
   LUMI_REQUIRE(ph >= 1 && pw >= 1 && 2 * (ph + pw) <= 64, "roi_pool: pooled size must be >= 1 with 2 * (ph + pw) <= 64");
   LUMI_REQUIRE(kernel >= -1 && kernel < ROI_KERNEL_COUNT, "roi_pool: kernel must be -1 or one of the codes 0-8");
@@ -688,6 +709,8 @@ void launch_roi_pool(const float* fmap_f32, int n, int fh, int fw, int c, const 
   RoiArgs a;
   a.fmap = fmap_f32; a.n = n; a.fh = fh; a.fw = fw; a.c = c;
   a.rois = rois; a.counts = counts; a.rmax = rmax; a.im_h = im_h; a.im_w = im_w;
+  LUMI_REQUIRE(!tab || feat_stride > 0, "roi_pool: a packed batch needs the feature stride");
+  a.tab = tab; a.feat_stride = feat_stride;
   a.crop_h = pw * 2; a.crop_w = ph * 2;      // roi_pool.py:77 passes [pooled_width*2, pooled_height*2]
   a.ohi = out.hi; a.olo = out.lo;
   a.mhi = mean.hi; a.mlo = mean.lo;

@@ -42,6 +42,8 @@ SIGNATURES = {
                                         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]),
     'lumi_predict_resize': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 5 +
                             [ctypes.c_void_p] * 4 + [ctypes.c_int]),
+    'lumi_predict_sizes': (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 4 +
+                           [ctypes.c_int]),
     'lumi_max_detections': (ctypes.c_int, [ctypes.c_void_p]),
     'lumi_set_record_output': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
     'lumi_stream': (ctypes.c_void_p, [ctypes.c_void_p]),
@@ -280,20 +282,34 @@ class Engine(object):
         engine's device and may be non-contiguous (they are copied); the engine reads them after the work queued so far
         on torch's current stream of that device, which is what wrote them.  Returns numpy (boxes [n,K,4] in h x w
         pixels, scores [n,K], labels [n,K], counts [n])."""
+        return self._predict_sources('predict_resize', images, None, int(h), int(w))
+
+    def predict_sizes(self, images, targets):
+        """``predict_resize`` with one target size per image (``lumi_predict_sizes``): images[i] is resized to
+        targets[i] = (h_i, w_i), every image runs in one forward at the top left of a canvas of the largest target
+        height and width, and its results equal those of ``predict_resize([images[i]], h_i, w_i)``.  Same argument
+        rules as ``predict_resize``; boxes come back in each image's own target pixels.  Faster R-CNN only (SSD takes
+        only its fixed size)."""
+        targets = np.array(targets, np.int32).reshape(-1, 2) if len(targets) else np.zeros((0, 2), np.int32)
+        return self._predict_sources('predict_sizes', images, targets, 0, 0)
+
+    def _predict_sources(self, name, images, targets, h, w):
         images = list(images)
         n = len(images)
         if n == 0:
-            raise ValueError('predict_resize: no images')
+            raise ValueError('%s: no images' % name)
+        if targets is not None and len(targets) != n:
+            raise ValueError('%s: %d images but %d targets' % (name, n, len(targets)))
         on_dev = [not isinstance(im, np.ndarray) for im in images]
         if any(on_dev) != all(on_dev):
-            raise ValueError('predict_resize: the images must be all numpy arrays or all CUDA tensors')
+            raise ValueError('%s: the images must be all numpy arrays or all CUDA tensors' % name)
         if on_dev[0]:
             import torch
             for im in images:
                 if not im.is_cuda or im.dtype not in (torch.uint8, torch.float32):
-                    raise ValueError('predict_resize: device images must be CUDA uint8 or float32 tensors')
+                    raise ValueError('%s: device images must be CUDA uint8 or float32 tensors' % name)
                 if im.device.index != self.device:
-                    raise ValueError('predict_resize: image on %s, the engine runs on cuda:%d' % (im.device, self.device))
+                    raise ValueError('%s: image on %s, the engine runs on cuda:%d' % (name, im.device, self.device))
             f32 = [im.dtype == torch.float32 for im in images]
             srcs = [im.contiguous() for im in images]
             ptrs = [s.data_ptr() for s in srcs]
@@ -302,10 +318,10 @@ class Engine(object):
             srcs = [np.ascontiguousarray(im, dtype=np.float32 if f else np.uint8) for im, f in zip(images, f32)]
             ptrs = [s.ctypes.data for s in srcs]
         if any(f32) != all(f32):
-            raise ValueError('predict_resize: the images of one call must share a dtype (uint8 or float32)')
+            raise ValueError('%s: the images of one call must share a dtype (uint8 or float32)' % name)
         for s in srcs:
             if len(s.shape) != 3 or s.shape[2] != 3:
-                raise ValueError('predict_resize: images must be (h0, w0, 3) RGB')
+                raise ValueError('%s: images must be (h0, w0, 3) RGB' % name)
         ptr_arr = (ctypes.c_void_p * n)(*ptrs)
         sizes = np.array([s.shape[:2] for s in srcs], np.int32)
         k = self.max_detections
@@ -313,6 +329,7 @@ class Engine(object):
         scores = np.empty((n, k), np.float32)
         labels = np.empty((n, k), np.int32)
         counts = np.empty((n,), np.int32)
+        outs = [a.ctypes.data_as(ctypes.c_void_p) for a in (boxes, scores, labels, counts)]
         with self._lock:
             if on_dev[0]:
                 # the engine's streams do not follow torch's: make its stream wait for the work torch has queued on
@@ -322,12 +339,12 @@ class Engine(object):
                 ready = torch.cuda.Event()
                 ready.record(torch.cuda.current_stream(dev))
                 torch.cuda.ExternalStream(self.stream, device=dev).wait_event(ready)
-            rc = self._lib.lumi_predict_resize(self._h, ptr_arr, sizes.ctypes.data_as(ctypes.c_void_p), int(f32[0]),
-                                               int(on_dev[0]), n, int(h), int(w),
-                                               boxes.ctypes.data_as(ctypes.c_void_p),
-                                               scores.ctypes.data_as(ctypes.c_void_p),
-                                               labels.ctypes.data_as(ctypes.c_void_p),
-                                               counts.ctypes.data_as(ctypes.c_void_p), 0)
+            sz = sizes.ctypes.data_as(ctypes.c_void_p)
+            if targets is None:
+                rc = self._lib.lumi_predict_resize(self._h, ptr_arr, sz, int(f32[0]), int(on_dev[0]), n, h, w, *outs, 0)
+            else:
+                rc = self._lib.lumi_predict_sizes(self._h, ptr_arr, sz, targets.ctypes.data_as(ctypes.c_void_p),
+                                                  int(f32[0]), int(on_dev[0]), n, *outs, 0)
             if rc != LUMI_OK:
                 _raise(rc, self._lib.lumi_last_error(self._h))
         return boxes, scores, labels, counts

@@ -342,7 +342,7 @@ def evaluate_dataset(network, config, dataset_split='val', batch_size=None, log=
 
 
 def evaluate(config, dataset_split='val', watch=False, from_global_step=None, max_detections=100, device=0,
-             max_batch=8, log=print, poll_seconds=5.0):
+             max_batch=8, log=print, poll_seconds=5.0, pack_sizes=False):
     """``lumi eval``: every (or, without ``watch``, the last) checkpoint of ``<job_dir>/<run_name>`` evaluated on the
     split; returns [{'global_step', 'metrics'}].  ``watch=True`` keeps polling for new checkpoints like the reference
     (:168-219)."""
@@ -366,7 +366,7 @@ def evaluate(config, dataset_split='val', watch=False, from_global_step=None, ma
         for checkpoint in checkpoints:
             log("Evaluating global_step {} using checkpoint '{}'".format(checkpoint['global_step'], checkpoint['file']))
             start = time.time()
-            network = PredictorNetwork(config, device=device, max_batch=max_batch,
+            network = PredictorNetwork(config, device=device, max_batch=max_batch, pack_sizes=pack_sizes,
                                        weights=lambda eng, f=checkpoint['file']: load_checkpoint_weights(eng, None, prefix=f))
             metrics, ap, _ar, total = evaluate_dataset(network, config, dataset_split, log=log)
             network.engine.close()
@@ -398,13 +398,14 @@ def main(argv=None):
     ap.add_argument('--max-detections', type=int, default=100)
     ap.add_argument('--device', type=int, default=0)
     ap.add_argument('--max-batch', type=int, default=8)
+    ap.add_argument('--pack-sizes', action='store_true', help='run images of different preprocessed sizes in one engine call, each at the top left of a shared canvas')
     args = ap.parse_args(argv)
     try:
         config = get_config(args.config_files, override_params=args.override_params)
     except KeyError:
         raise KeyError('model.type should be set on the custom config.')
     res = evaluate(config, args.dataset_split, args.watch, args.from_global_step, args.max_detections, args.device,
-                   args.max_batch)
+                   args.max_batch, pack_sizes=args.pack_sizes)
     print(json.dumps(res))
 
 

@@ -175,6 +175,7 @@ def main(argv=None):
     ap.add_argument('--only-class', '-k', action='append', default=None)
     ap.add_argument('--ignore-class', '-K', action='append', default=None)
     ap.add_argument('--max-batch', default=8, type=int, help='images / frames per engine call')
+    ap.add_argument('--pack-sizes', action='store_true', help='run images of different preprocessed sizes in one engine call, each at the top left of a shared canvas')
     ap.add_argument('--decode', default='pil', choices=['pil', 'nvjpeg'])
     ap.add_argument('--device', default=0, type=int)
     args = ap.parse_args(argv)
@@ -197,7 +198,7 @@ def main(argv=None):
     output = sys.stdout if args.output_path == '-' else open(args.output_path, 'w')
     if args.save_media_to:
         os.makedirs(args.save_media_to, exist_ok=True)
-    network = PredictorNetwork(config, device=args.device, max_batch=args.max_batch)
+    network = PredictorNetwork(config, device=args.device, max_batch=args.max_batch, pack_sizes=args.pack_sizes)
     image_files = [f for f in files if get_file_type(f) == 'image']
     echo = lambda m: print(m, file=sys.stderr)
     for path, objects in predict_images(network, image_files, args.only_class, args.ignore_class, args.save_media_to,

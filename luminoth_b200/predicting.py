@@ -13,7 +13,9 @@ bilinear kernel, bit-identically, in the kernels that stage the first conv's inp
 only its size arithmetic (float32, like the reference) stays on the host.  Images
 of different sizes in one ``predict_batch`` call are bucketed by their
 preprocessed size, each bucket runs as one batched engine call, and the results
-come back in the caller's order.
+come back in the caller's order.  With ``pack_sizes=True``, images of different
+preprocessed sizes share an engine call (``lumi_predict_sizes``), each at the top
+left of a common canvas, with the results of separate calls.
 """
 import json
 import math
@@ -90,6 +92,39 @@ def format_predictions(objects, labels, probs, scale_factor, class_labels=None):
                   key=lambda x: x['prob'], reverse=True)
 
 
+# Packing (``pack_sizes=True``) starts a new engine call when the images of the current one would cover less than this
+# share of their canvas (n x largest height x largest width): the canvas positions outside the images cost conv time.
+PACK_FILL = 0.75
+
+
+def size_groups(targets, max_batch):
+    """Today's grouping: indices bucketed by identical target (h, w) in first-seen order, each bucket cut into
+    chunks of ``max_batch``."""
+    buckets = {}
+    for i, t in enumerate(targets):
+        buckets.setdefault(tuple(t), []).append(i)
+    return [idxs[s:s + max_batch] for idxs in buckets.values() for s in range(0, len(idxs), max_batch)]
+
+
+def pack_groups(targets, max_batch, fill=PACK_FILL):
+    """Groups for packed calls: indices sorted by orientation (landscape or square first, then portrait), then by
+    height and width, cut into groups of at most ``max_batch`` that end where adding the next image would bring the
+    group's fill (sum of image areas over n x canvas height x canvas width) below ``fill``."""
+    order = sorted(range(len(targets)), key=lambda i: (targets[i][0] > targets[i][1], targets[i][0], targets[i][1], i))
+    groups, cur, area, hc, wc = [], [], 0, 0, 0
+    for i in order:
+        h, w = targets[i]
+        nh, nw, na = max(hc, h), max(wc, w), area + h * w
+        if cur and (len(cur) == max_batch or na < fill * (len(cur) + 1) * nh * nw):
+            groups.append(cur)
+            cur, area, nh, nw, na = [], 0, h, w, h * w
+        cur.append(i)
+        area, hc, wc = na, nh, nw
+    if cur:
+        groups.append(cur)
+    return groups
+
+
 def load_checkpoint_weights(engine, job_dir, prefix=None):
     """The ``Saver.restore`` of ``predicting.py:51-63`` without TensorFlow: reads the latest Saver-V2 bundle under
     ``job_dir`` and returns {tf variable name: array} for exactly the variables the engine's plan uses (optimizer
@@ -123,8 +158,9 @@ class PredictorNetwork(object):
     used for testing" branch (``predicting.py:64-72``).
     """
 
-    def __init__(self, config, weights=None, device=0, max_batch=1):
+    def __init__(self, config, weights=None, device=0, max_batch=1, pack_sizes=False):
         self.class_labels = None
+        self.pack_sizes = bool(pack_sizes)
         if config.dataset.dir:
             classes_file = os.path.join(config.dataset.dir, 'classes.json')
             if os.path.exists(classes_file):
@@ -173,23 +209,28 @@ class PredictorNetwork(object):
             if im.ndim != 3 or im.shape[2] != 3:
                 raise ValueError('expected an (H, W, 3) RGB image')
         sizes = [target_size(im.shape, self.config) for im in images]
-        buckets = {}                                     # (nh, nw) -> indices, first-seen order
-        for i, (nh, nw, _) in enumerate(sizes):
-            buckets.setdefault((nh, nw), []).append(i)
+        targets = [(nh, nw) for nh, nw, _ in sizes]
+        if self.pack_sizes:
+            groups = pack_groups(targets, self.engine.max_batch)
+        else:
+            groups = size_groups(targets, self.engine.max_batch)
+        touched = set(t for t, im in zip(targets, images) if im.dtype != np.uint8 or im.shape[:2] != t)
         out = [None] * len(images)
-        for (nh, nw), idxs in buckets.items():
-            untouched = all(images[i].dtype == np.uint8 and images[i].shape[:2] == (nh, nw) for i in idxs)
-            for s in range(0, len(idxs), self.engine.max_batch):
-                chunk = idxs[s:s + self.engine.max_batch]
-                if untouched:   # integer pixels, no resize: the uint8 entry point (the benchmark shapes)
-                    res = self.engine.predict_raw(np.stack([images[i] for i in chunk]))
-                else:           # the reference feeds the resized FLOAT image (predicting.py:110-112): resized in
-                    srcs = [images[i] for i in chunk]     # the engine's input staging, one call per chunk
-                    if any(im.dtype != np.uint8 for im in srcs):
-                        srcs = [im.astype(np.float32, copy=False) for im in srcs]   # uint8 -> float32 is exact
-                    res = self.engine.predict_resize(srcs, nh, nw)
-                boxes, scores, labels, counts = res
-                for j, i in enumerate(chunk):
-                    k = int(counts[j])
-                    out[i] = (boxes[j, :k].copy(), labels[j, :k].copy(), scores[j, :k].copy(), sizes[i][2])
+        for chunk in groups:
+            shapes = set(targets[i] for i in chunk)
+            srcs = [images[i] for i in chunk]
+            if len(shapes) == 1 and not shapes & touched:
+                # integer pixels, no resize: the uint8 entry point (the benchmark shapes)
+                res = self.engine.predict_raw(np.stack(srcs))
+            else:       # the reference feeds the resized FLOAT image (predicting.py:110-112): resized in the engine's
+                if any(im.dtype != np.uint8 for im in srcs):    # input staging, one call per group
+                    srcs = [im.astype(np.float32, copy=False) for im in srcs]   # uint8 -> float32 is exact
+                if len(shapes) == 1:
+                    res = self.engine.predict_resize(srcs, *targets[chunk[0]])
+                else:
+                    res = self.engine.predict_sizes(srcs, [targets[i] for i in chunk])
+            boxes, scores, labels, counts = res
+            for j, i in enumerate(chunk):
+                k = int(counts[j])
+                out[i] = (boxes[j, :k].copy(), labels[j, :k].copy(), scores[j, :k].copy(), sizes[i][2])
         return out

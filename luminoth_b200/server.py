@@ -104,7 +104,7 @@ class LumiServer(object):
     """The web application object: owns the network (loaded on a background thread) and the batcher."""
 
     def __init__(self, config, host='127.0.0.1', port=5000, device=0, max_batch=8, batch_window_ms=2.0, weights=None,
-                 network_factory=None):
+                 network_factory=None, pack_sizes=False):
         self.config = set_prediction_filters(config, 0.01, None)         # web.py:94-103
         self.network = None
         self.batcher = None
@@ -116,7 +116,8 @@ class LumiServer(object):
                     self.network = network_factory(self.config)
                 else:
                     from .predicting import PredictorNetwork
-                    self.network = PredictorNetwork(self.config, weights=weights, device=device, max_batch=max_batch)
+                    self.network = PredictorNetwork(self.config, weights=weights, device=device, max_batch=max_batch,
+                                                    pack_sizes=pack_sizes)
                 self.batcher = MicroBatcher(self.network.predict_batch, max_batch, batch_window_ms)
             except Exception as e:               # noqa: BLE001 -- reported to every request (web.py:64-69 kills the server)
                 self.error = e
@@ -212,12 +213,14 @@ def main(argv=None):
     ap.add_argument('--port', default=5000, type=int)
     ap.add_argument('--device', default=0, type=int)
     ap.add_argument('--max-batch', default=8, type=int)
+    ap.add_argument('--pack-sizes', action='store_true', help='run images of different preprocessed sizes in one engine call, each at the top left of a shared canvas')
     ap.add_argument('--batch-window-ms', default=2.0, type=float)
     args = ap.parse_args(argv)
     config = get_config(args.config_files)
     if args.override_params:
         config = override_config_params(config, args.override_params)
-    srv = LumiServer(config, args.host, args.port, args.device, args.max_batch, args.batch_window_ms)
+    srv = LumiServer(config, args.host, args.port, args.device, args.max_batch, args.batch_window_ms,
+                     pack_sizes=args.pack_sizes)
     print('listening on http://{}:{}'.format(args.host, srv.port))
     try:
         srv.serve_forever()
