@@ -115,7 +115,7 @@ def rcnn_head(pooled, wts, rcfg, arch, scope='fasterrcnn/rcnn', use_tail=True):
             feats = feats.mean(axis=(1, 2), dtype=feats.dtype)
         else:
             feats = feats.reshape(0, feats.shape[-1])
-    net = feats.reshape(feats.shape[0], -1)
+    net = feats.reshape(feats.shape[0], int(np.prod(feats.shape[1:])))   # tf.contrib.layers.flatten: known inner size
     act = activation(rcfg.get('activation_function', 'relu6'))
     dt = net.dtype
     for i, _ in enumerate(rcfg.get('layer_sizes') or []):

@@ -445,6 +445,11 @@ def _bn_fold(wts, scope):
 def test_toeplitz_view_stem_matches_float64(n, h, w):
     """The stem conv (7x7/2 over image - mean as four K = 64 taps of the space-to-depth staging) per element at
     sampled pixels, K = 256 in the fold count."""
+    stem_against_float64(n, h, w)
+
+
+def stem_against_float64(n, h, w):
+    """The `stem` tap of a batch of n h x w images against float64 at sampled pixels; returns the largest err / bound."""
     from luminoth_b200 import synth
     from luminoth_b200.engine import Engine
     cfg = _frcnn_cfg()
@@ -463,7 +468,7 @@ def test_toeplitz_view_stem_matches_float64(n, h, w):
     x = imgs.astype(f32) - RGB_MEANS                                   # the engine's fp32 image - mean
     at = sample_pixels(n, ho, wo, 23)
     ref, bound = reference(x, wts[root + '/weights'], 2, 'SLIM', scale, bias, None, 1, RELU, ENGINE, at=at, k_fold=256)
-    check('stem %dx%dx%d (%d px)' % (n, h, w, len(at[0])), stem[at], ref, bound)
+    return check('stem %dx%dx%d (%d px)' % (n, h, w, len(at[0])), stem[at], ref, bound)
 
 
 @pytest.mark.gpu

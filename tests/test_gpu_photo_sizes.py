@@ -110,6 +110,10 @@ def test_photo_layer_table_geometry():
 def test_photo_launch_matches_float64(row):
     """Codes 16 / 17 (18 / 19 for fp32 outputs) against float64 at the sampled pixels (every border pixel of each
     image and one pixel in 16), held to the per-element bound of test_gpu_conv_numerics."""
+    launch_against_float64(row, 'photo_sizes/conv/')
+
+
+def launch_against_float64(row, report_prefix):
     inputs = _inputs(row)
     x, w, scale, bias, res, pre = inputs
     launch = Launch(row, inputs)
@@ -129,7 +133,7 @@ def test_photo_launch_matches_float64(row):
             worst = max(worst, check(tag, _gather(y, at), ref, bound))
         if p is not None:
             worst = max(worst, check(tag + '/p', _gather(p, at), pref, pbound))
-    _report('photo_sizes/conv/' + row.name, err_over_bound=worst)
+    _report(report_prefix + row.name, err_over_bound=worst)
 
 
 # ---------------------------------------------------------------------------------------------- GPU: end to end
@@ -150,14 +154,19 @@ def _engine(cfg, wts, n, h, w):
     return eng
 
 
-def _against_oracle(key, cfg, wts, src, hw, i, out, fmap, pcnt):
-    """Image i of a production call (out) against the fp32 and float64 oracle fed `src` resized to hw on the host;
-    fmap / pcnt: the feature map and proposal counts of a debug-taps run of the same call."""
+def oracle_pair(cfg, wts, src, hw):
+    """The fp32 and float64 oracle forward of `src` resized to hw on the host."""
     from oracle import fasterrcnn as ofr
     from oracle import tf_ops as T
     img = T.resize_bilinear(src.astype(np.float32), *hw)          # bit-identical to the engine's staging
-    ref = ofr.forward(img, wts, cfg)
-    tru = ofr.forward(img, wts, cfg, dtype=np.float64)
+    return ofr.forward(img, wts, cfg), ofr.forward(img, wts, cfg, dtype=np.float64)
+
+
+def _against_oracle(key, cfg, wts, src, hw, i, out, fmap, pcnt, oracle=None):
+    """Image i of a production call (out) against the fp32 and float64 oracle fed `src` resized to hw on the host
+    (or `oracle`, the oracle_pair of that image already evaluated); fmap / pcnt: the feature map and proposal counts
+    of a debug-taps run of the same call."""
+    ref, tru = oracle or oracle_pair(cfg, wts, src, hw)
     fm = fmap[i, :-(-hw[0] // STRIDE), :-(-hw[1] // STRIDE)]
     assert fm.shape == tru['conv_feature_map'][0].shape, (fm.shape, tru['conv_feature_map'].shape)
     extra = dict(image_index=i, target_h=hw[0], target_w=hw[1],

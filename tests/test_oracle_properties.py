@@ -4,8 +4,11 @@ reference's own tests cannot pin because the arithmetic lives in TensorFlow (SUR
 import math
 
 import numpy as np
+import pytest
 from hypothesis import given, settings, strategies as st
 
+from luminoth_b200 import default_config, synth
+from oracle import fasterrcnn as ofr
 from oracle import tf_ops as T
 
 SET = settings(max_examples=25, deadline=None)
@@ -148,3 +151,27 @@ def test_resize_bilinear_matches_scalar_kernel(H, W, nh, nw, seed):
             top = img[y0, x0] + (img[y0, x1] - img[y0, x0]) * (fx - x0)
             bot = img[y1, x0] + (img[y1, x1] - img[y1, x0]) * (fx - x0)
             np.testing.assert_allclose(got[y, x], top + (bot - top) * (fy - y0), rtol=1e-12, atol=1e-9)
+
+
+@pytest.mark.parametrize('arch,with_rcnn', [('resnet_v1_50', True), ('resnet_v1_101', True), ('resnet_v1_50', False)],
+                         ids=['r50', 'r101', 'r50_rpn_only'])
+def test_forward_on_an_image_without_proposals(arch, with_rcnn):
+    """With filter_outside_anchors no anchor (the smallest is 64 px high) lies inside an image under 55 px high, so a
+    40x640 image has no proposals.  The reference still runs its RCNN head on the empty list: tf.contrib.layers.flatten
+    reshapes with the known inner size (rcnn.py:192) and the forward returns no detections.  At 55 px the anchors of
+    the first row fit and the image has proposals again."""
+    cfg = default_config('fasterrcnn', ['model.base_network.architecture=' + arch, 'model.network.num_classes=20',
+                                        'model.rpn.proposals.post_nms_top_n=200',
+                                        'model.rcnn.proposals.min_prob_threshold=0.05',
+                                        'model.rpn.proposals.filter_outside_anchors=true',
+                                        'model.network.with_rcnn=%s' % str(with_rcnn).lower()])
+    wts = synth.make_weights(cfg, seed=1)
+    out = ofr.forward(synth.make_images(1, 40, 640, seed=2)[0], wts, cfg)
+    assert out['rpn_prediction']['proposals'].shape == (0, 4)
+    if with_rcnn:
+        det = out['classification_prediction']
+        assert det['objects'].shape == (0, 4) and len(det['labels']) == 0 and len(det['probs']) == 0
+        assert out['rcnn']['cls_prob'].shape == (0, 21) and out['rcnn']['bbox_offsets'].shape == (0, 80)
+    else:
+        assert 'classification_prediction' not in out
+    assert len(ofr.forward(synth.make_images(1, 55, 640, seed=2)[0], wts, cfg)['rpn_prediction']['proposals']) > 0
