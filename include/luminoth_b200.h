@@ -135,6 +135,12 @@ int lumi_set_conv_impl(lumi_engine* e, int impl);
  * are deterministic in every mode; modes differ in fp32 summation order only. */
 int lumi_set_conv_streamk(lumi_engine* e, int mode);
 
+/* SMs the engine's launch decisions count on: the persistent conv grids, the stream-K partition and whether stream-K
+ * runs, the 128 x 256 tile rule, the 2-CTA cluster pairs and the NMS mask grid.  0 (default) = the device's count; a
+ * larger value is capped at it (the grids only ever shrink).  What a GPU with fewer SMs (H100 PCIe, a MIG slice)
+ * would run, on this one.  Results are deterministic at every limit; limits differ in fp32 summation order only. */
+int lumi_set_sm_limit(lumi_engine* e, int sms);
+
 /* 1 (default): lumi_predict splits the batch in two halves that run on two streams, so the latency-bound
  * proposal / NMS kernels of one half overlap the convolutions of the other. 0: single stream. Results are
  * identical either way (images are independent). Off automatically while profiling or tapping. */
@@ -209,6 +215,16 @@ int lumi_op_conv2d_io(const float* x, int n, int h, int w, int cin, const float*
                       int stride, int rate, int padding, const float* scale, const float* bias, const float* residual,
                       int res_h, int res_w, int res_stride, int act, int impl, const float* pre_scale,
                       const float* pre_bias, float* y, float* p, int* ho, int* wo, void* stream);
+
+/* lumi_op_conv2d_io on a chosen schedule: sm_limit is the SM count the launch counts on (0: the device's; capped at
+ * it), as lumi_set_sm_limit sets it for an engine; launches >= 1 runs the conv that many times back to back on one
+ * stream-K workspace (each launch a new flag epoch, as the engine's eager launches) and returns the last output.
+ * A 2-CTA cluster kernel (codes 6, 7) with a budget below 2 SMs returns LUMI_EINVAL. */
+int lumi_op_conv2d_sched(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout,
+                         int stride, int rate, int padding, const float* scale, const float* bias, const float* residual,
+                         int res_h, int res_w, int res_stride, int act, int impl, const float* pre_scale,
+                         const float* pre_bias, int sm_limit, int launches, float* y, float* p, int* ho, int* wo,
+                         void* stream);
 
 /* The tensor-core weight packing of a conv layer, on HOST pointers and without any CUDA call.  w: TF layout
  * [kdim = kh*kw*cin][cout] fp32; scale [cout] or NULL (1).  Writes hi, lo: [cout][kdim] fp16 bit patterns of the split

@@ -1006,8 +1006,9 @@ int device_sm_count() {
   }
   return v;
 }
-static int sm_budget(int reserve) {
-  const int n = device_sm_count();
+int sm_budget(int reserve, int limit) {
+  int n = device_sm_count();
+  if (limit > 0 && limit < n) n = limit;
   return (reserve > 0 && reserve < n) ? n - reserve : n;
 }
 
@@ -1027,7 +1028,7 @@ void conv_workspace_free(ConvWorkspace& w) {
 }
 
 template <int BN, int STAGES, int NCWG, bool PAIR, bool HALO, bool PIPE, int SLOTS, bool PRE>
-static void launch_tc_cfg(const TcArgs& a, ConvWorkspace* sk, int streamk, int sm_reserve, cudaStream_t st) {
+static void launch_tc_cfg(const TcArgs& a, ConvWorkspace* sk, int streamk, int sms, cudaStream_t st) {
   using Cfg = TcCfg<BN, STAGES, NCWG, PAIR, HALO, SLOTS>;
   auto kernel = conv_tc_kernel<BN, STAGES, NCWG, PAIR, HALO, PIPE, SLOTS, PRE>;
   // cudaFuncSetAttribute is per device: one flag per (kernel instance, device)
@@ -1040,9 +1041,10 @@ static void launch_tc_cfg(const TcArgs& a, ConvWorkspace* sk, int streamk, int s
   }
   const long m_tiles = (long)a.tiles_w * a.tiles_h * a.tiles_n;
   const long total = (PAIR ? (m_tiles + 1) / 2 : m_tiles) * a.n_tiles;      // scheduling units (tiles or tile pairs)
-  const int sms = sm_budget(sm_reserve);
   int units_max = PAIR ? sms / 2 : sms;
   if (PAIR) {
+    LUMI_REQUIRE(units_max >= 1, "conv_tc: the 2-CTA cluster kernel needs a budget of at least 2 SMs, got " +
+                                     std::to_string(sms));
     // stream-K needs every cluster of the grid resident at once: never launch more pairs than can be co-scheduled
     static int max_clusters[LUMI_MAX_DEVICES] = {0};
     int mc = (dev >= 0 && dev < LUMI_MAX_DEVICES) ? __atomic_load_n(&max_clusters[dev], __ATOMIC_RELAXED) : 0;
@@ -1107,15 +1109,16 @@ static void launch_tc_cfg(const TcArgs& a, ConvWorkspace* sk, int streamk, int s
 // pre-activation output selects the PRE instances, which exist for the non-halo kernels only
 template <int BN, int STAGES, int NCWG = 2, bool PAIR = false, bool HALO = false, int SLOTS = 0>
 static void launch_tc(const TcArgs& a, const ConvIO& io, cudaStream_t st) {
+  const int sms = sm_budget(io.sm_reserve, io.sm_limit);
   if constexpr (!HALO) {
     if (io.pre.hi) {
-      if (io.pipe) launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, true, SLOTS, true>(a, io.sk, io.streamk, io.sm_reserve, st);
-      else launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, false, SLOTS, true>(a, io.sk, io.streamk, io.sm_reserve, st);
+      if (io.pipe) launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, true, SLOTS, true>(a, io.sk, io.streamk, sms, st);
+      else launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, false, SLOTS, true>(a, io.sk, io.streamk, sms, st);
       return;
     }
   }
-  if (io.pipe) launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, true, SLOTS, false>(a, io.sk, io.streamk, io.sm_reserve, st);
-  else launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, false, SLOTS, false>(a, io.sk, io.streamk, io.sm_reserve, st);
+  if (io.pipe) launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, true, SLOTS, false>(a, io.sk, io.streamk, sms, st);
+  else launch_tc_cfg<BN, STAGES, NCWG, PAIR, HALO, false, SLOTS, false>(a, io.sk, io.streamk, sms, st);
 }
 
 void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
@@ -1132,7 +1135,7 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
   // slower (DESIGN 7.1).  They are never halo or cluster-pair layers.
   const long wide_tiles = (long)cdiv(io.in.n, nb) * cdiv(io.ho, th) * cdiv(io.wo, tw) * (L.cout_pad / 256);
   const bool wide = io.wide && L.cout_pad % 256 == 0 && n_iters_all >= io.wide && !io.out_f32 && io.epi_tma &&
-                    !io.pre.hi && wide_tiles * 100 >= (long)sm_budget(io.sm_reserve) * io.wide_sm_pct;
+                    !io.pre.hi && wide_tiles * 100 >= (long)sm_budget(io.sm_reserve, io.sm_limit) * io.wide_sm_pct;
   const int bn = wide ? 256 : (L.cout_pad % 128 == 0) ? 128 : 64;
   // halo-patch kernels (3x3, stride 1, rate 1, SAME): tiles of th x 8 pixels of one image, th <= 16 chosen so that the
   // rows of the map split evenly.  They trade M-tile occupancy (th * 8 <= 128 rows, and the weights stream once per
@@ -1203,7 +1206,9 @@ void launch_conv_tc(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
     }
     // the wide tile: 2 x 96 KB stages + one slot (224 KB); a slice is twice the MMA work of a BN = 128 slice, so two
     // stages keep as much of it in flight as four do there
-    if (wide) launch_tc_cfg<256, 2, 2, false, false, false, 1, false>(a, io.sk, io.streamk, io.sm_reserve, st);
+    if (wide)
+      launch_tc_cfg<256, 2, 2, false, false, false, 1, false>(a, io.sk, io.streamk,
+                                                              sm_budget(io.sm_reserve, io.sm_limit), st);
     else if (epi16) launch_tc<128, 2, 4, false, false, 2>(a, io, st);
     else if (bn == 128) launch_tc<128, 3, 2, false, false, 1>(a, io, st);
     else launch_tc<64, 3, 2, false, false, 2>(a, io, st);

@@ -35,6 +35,9 @@ void conv_workspace_free(ConvWorkspace& w);
 // Per-device facts (SM count, opt-in dynamic shared memory of a kernel) are cached per CUDA device, never per
 // process: two engines on two devices, or on two threads, share no mutable launch state.
 int device_sm_count();            // SMs of the CURRENT device
+// SMs a persistent launch may occupy: min(limit, device count) (limit <= 0: the device count), less `reserve` when
+// the reserve leaves at least one SM
+int sm_budget(int reserve, int limit);
 constexpr int LUMI_MAX_DEVICES = 64;
 
 // The engine's default mainloop and four-warpgroup bound (DESIGN 7.2).  The stand-alone conv op runs the same, so the
@@ -71,6 +74,9 @@ struct ConvIO {
   int wide_sm_pct = 50;         // ... while those tiles number at least this percentage of the SMs the launch may use
   int epi_tma = 1;              // 1: split outputs of the generic kernel leave through the shared-memory slot epilogue (TMA); 0: register epilogue
   int sm_reserve = 0;           // SMs a persistent launch leaves free (the engine's two-stream pipeline sets 8)
+  // SMs the launch may count on before the reserve (0: the device's).  Never raises the budget above the device's
+  // count: the stream-K head CTA spins on flags of later CTAs, so every CTA of a persistent grid must be resident.
+  int sm_limit = 0;
   // Optional strided ("Toeplitz") view of the input for the tensor-core path: element pitches between
   // consecutive pixels / rows / images (0 = dense NHWC).  Used by the space-to-depth stem, where each
   // A row is the 64 contiguous fp16 of four horizontally adjacent 16-channel pixels.

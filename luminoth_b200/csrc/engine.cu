@@ -159,6 +159,7 @@ struct lumi_engine {
   int* d_overflow = nullptr;
   ConvWorkspace sk_ws[2];       // stream-K scratch, one per stream
   int conv_streamk = 1;         // 0 off, 1 auto, 2 whenever possible
+  int sm_limit = 0;             // lumi_set_sm_limit: SMs the launch decisions count on (0: the device's)
   // conv kernel variants; the defaults are the fastest setting measured on the Faster R-CNN R50 workload (DESIGN 7.2):
   int conv_cta2 = 0;            // env LUMI_CONV_2CTA: 2-CTA cluster kernel on layers with at least this many K slices per tile
   int conv_halo = 0;            // env LUMI_CONV_HALO: 1 = halo-patch kernels on the 3x3 stride-1 layers
@@ -179,12 +180,12 @@ struct lumi_engine {
   int planned_n = 0, planned_h = 0, planned_w = 0;
   // CUDA graphs: one captured graph per (half-)batch forward, keyed by everything baked into its nodes
   struct GraphKey {
-    int half, n, h, w, esz, resize, packed, img_off, conv_impl, streamk, reserve;
+    int half, n, h, w, esz, resize, packed, img_off, conv_impl, streamk, reserve, sm_limit;
     const void* records;
     bool operator<(const GraphKey& o) const {
-      return std::tie(half, n, h, w, esz, resize, packed, img_off, conv_impl, streamk, reserve, records) <
+      return std::tie(half, n, h, w, esz, resize, packed, img_off, conv_impl, streamk, reserve, sm_limit, records) <
              std::tie(o.half, o.n, o.h, o.w, o.esz, o.resize, o.packed, o.img_off, o.conv_impl, o.streamk, o.reserve,
-                      o.records);
+                      o.sm_limit, o.records);
     }
   };
   struct GraphEntry { cudaGraphExec_t exec = nullptr; int launches = 0; int seen = 0; };
@@ -791,9 +792,11 @@ struct Ctx {
   }
 };
 
-// problems [off, ...) of a batched NMS workspace (the second half-batch works on its own slice)
-NmsWorkspace ws_view(const NmsWorkspace& ws, int off) {
+// problems [off, ...) of a batched NMS workspace (the second half-batch works on its own slice), its grids sized for
+// the engine's SM budget
+NmsWorkspace ws_view(const NmsWorkspace& ws, int off, int sm_limit) {
   NmsWorkspace v = ws;
+  v.sm_limit = sm_limit;
   v.problems = ws.problems - off;
   v.keys = ws.keys + (size_t)off * ws.cap;
   v.boxes = ws.boxes + (size_t)off * ws.cap * 4;
@@ -896,6 +899,7 @@ Act run_conv(Ctx& cx, const std::string& key, Act in, const Act* res, int res_st
   io.sk = cx.sk;
   io.streamk = cx.e->conv_streamk;
   io.sm_reserve = cx.sm_reserve;
+  io.sm_limit = cx.e->sm_limit;
   io.cta2 = cx.e->conv_cta2;
   io.halo = cx.e->conv_halo;
   io.halo_tiles_pct = cx.e->conv_halo_pct;
@@ -1066,7 +1070,7 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
   float* pscores = cx.f32((size_t)n * post);
   if (!cx.dry) {
     LUMI_REQUIRE(na <= e->ws_rpn.cap, "image too large for the RPN workspace (max_h/max_w at lumi_create)");
-    NmsWorkspace wsr = ws_view(e->ws_rpn, io);
+    NmsWorkspace wsr = ws_view(e->ws_rpn, io, e->sm_limit);
     // algorithmic bytes (SURVEY 8d): decode N*(36 in + 20 out), sort N*4 + K*20, bitmask NMS K*16 + 2*K*ceil(K/64)*8 + P*4
     const double kk = std::min(na, rp.pre_nms_top_n);
     const double bytes = (double)n * (56.0 * na + 4.0 * na + 20.0 * kk + 16.0 * kk + 16.0 * kk * std::ceil(kk / 64.0) + 4.0 * post);
@@ -1141,7 +1145,7 @@ void forward_frcnn(Ctx& cx, const void* images, int n, int h, int w) {
   if (cx.packed) dp.tab = cx.resize;
   if (!cx.dry) {
     ProfScope ps(cx.e, cx.dry, PC_DET_POST);
-    NmsWorkspace wsd = ws_view(e->ws_det, io * C);
+    NmsWorkspace wsd = ws_view(e->ws_det, io * C, e->sm_limit);
     launch_class_detections(proposals, (long)post * 4, prop_counts, fc + (C + 1), cls_prob, n, dp, wsd, cx.final_keys,
                             out_boxes, out_labels, out_scores, out_counts, cx.st, out_records);
   }
@@ -1283,7 +1287,7 @@ void forward_ssd(Ctx& cx, const void* images, int n, int h, int w) {
   if (!cx.dry) {
     ProfScope ps(cx.e, cx.dry, PC_DET_POST);
     const int io = cx.img_off;
-    NmsWorkspace wsd = ws_view(e->ws_det, io * e->num_classes);
+    NmsWorkspace wsd = ws_view(e->ws_det, io * e->num_classes, e->sm_limit);
     launch_class_detections(e->d_ssd_anchors, 0, nullptr, loc, prob, n, dp, wsd, cx.final_keys,
                             e->d_boxes + (size_t)io * e->kmax * 4, e->d_labels + (size_t)io * e->kmax,
                             e->d_scores + (size_t)io * e->kmax, e->d_counts + io, cx.st,
@@ -1491,7 +1495,7 @@ static void run_forward(lumi_engine* e, Ctx& cx, int half, const void* images, i
   const bool graphable = e->use_graphs && !e->profile && !e->debug_taps;
   if (!graphable) { forward(cx, images, n, h, w); return; }
   lumi_engine::GraphKey key{half, n, h, w, esz, cx.resize != nullptr, cx.packed, cx.img_off, e->conv_impl,
-                            e->conv_streamk, cx.sm_reserve, e->d_records};
+                            e->conv_streamk, cx.sm_reserve, e->sm_limit, e->d_records};
   lumi_engine::GraphEntry& ent = e->graphs[key];
   if (ent.exec) {
     LUMI_CUDA_CHECK(cudaGraphLaunch(ent.exec, cx.st));
@@ -1819,6 +1823,13 @@ int lumi_set_conv_impl(lumi_engine* e, int impl) {
 int lumi_set_conv_streamk(lumi_engine* e, int mode) {
   if (!e || mode < 0 || mode > 2) return LUMI_EINVAL;
   e->conv_streamk = mode;
+  return LUMI_OK;
+}
+
+int lumi_set_sm_limit(lumi_engine* e, int sms) {
+  if (!e) return LUMI_EINVAL;
+  if (sms < 0) return fail(e, LUMI_EINVAL, "lumi_set_sm_limit: the SM limit must be >= 0 (0: the device's count)");
+  e->sm_limit = sms;
   return LUMI_OK;
 }
 

@@ -94,6 +94,7 @@ struct NmsWorkspace {
   unsigned int* cut_hist = nullptr;         // [P][4 digits][256]
   unsigned long long* cut_counts = nullptr; // [P][cut_blocks] (candidates above the k-th key << 32 | equal to it)
   int cut_blocks = 0;
+  int sm_limit = 0;             // SMs the NMS mask grid is sized for (0: the device's; see sm_budget)
 };
 void nms_workspace_alloc(NmsWorkspace& ws, int problems, int cap, int max_out, int ncap = 0);
 void nms_workspace_free(NmsWorkspace& ws);

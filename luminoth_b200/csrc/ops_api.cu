@@ -37,11 +37,14 @@ constexpr int CONV_OP_PIPE = 32;   // impl flag of lumi_op_conv2d*: the double-b
 
 // The arguments of lumi_op_conv2d_io: those of lumi_op_conv2d, the residual's own resolution and sampling stride
 // (res_h <= 0: the output's, stride 1) and the pre-activation output of lumi_op_conv2d_preact (pre_scale == nullptr:
-// none; then y is required, else y == nullptr writes p only).
+// none; then y is required, else y == nullptr writes p only), and the schedule of lumi_op_conv2d_sched: the SM budget
+// (0: the device's) and how many times the conv runs back to back on one stream-K workspace.
 int op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout, int stride,
               int rate, int padding, const float* scale, const float* bias, const float* residual, int res_h,
               int res_w, int res_stride, int act, int impl, const float* pre_scale, const float* pre_bias, float* y,
-              float* p, int* ho_out, int* wo_out, cudaStream_t st) {
+              float* p, int* ho_out, int* wo_out, int sm_limit, int launches, cudaStream_t st) {
+  LUMI_REQUIRE(sm_limit >= 0, "conv2d: sm_limit must be >= 0 (0: the device's SM count)");
+  LUMI_REQUIRE(launches >= 1, "conv2d: launches must be >= 1");
   const bool preact = pre_scale != nullptr;
   const bool pipe = (impl & CONV_OP_PIPE) != 0;
   impl &= ~CONV_OP_PIPE;
@@ -95,6 +98,7 @@ int op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, in
   launch_f32_to_act(x, in.a, st);
   ConvIO io;
   io.in = in.a; io.pad_t = pt; io.pad_l = pl; io.ho = ho; io.wo = wo; io.out_f32 = y;
+  io.sm_limit = sm_limit;
   std::unique_ptr<ActBuf> res;
   if (residual) {
     if (res_h <= 0) { res_h = ho; res_w = wo; res_stride = 1; }
@@ -130,14 +134,14 @@ int op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, in
   ConvWorkspace sk;
   struct SkGuard { ConvWorkspace& w; ~SkGuard() { conv_workspace_free(w); } } skg{sk};
   if (simt) {
-    launch_conv_simt(L, io, st);
+    for (int i = 0; i < launches; ++i) launch_conv_simt(L, io, st);
   } else if (as_engine) {
     io.epi16 = CONV_EPI16_DEFAULT;
     io.sm_reserve = (impl == 17 || impl == 19) ? CONV_PIPELINE_SM_RESERVE : 0;
     LUMI_REQUIRE(conv_tc_supported(L, io), "conv2d: this layer shape is not handled by the tensor-core kernel");
     conv_workspace_create(sk);
     io.sk = &sk;
-    launch_conv_tc(L, io, st);
+    for (int i = 0; i < launches; ++i) launch_conv_tc(L, io, st);
   } else {
     io.pipe = pipe ? 1 : 0;
     io.epi_tma = impl == 12 ? 0 : 1;
@@ -155,7 +159,7 @@ int op_conv2d(const float* x, int n, int h, int w, int cin, const float* wgt, in
       io.sk = &sk;
       io.streamk = 2;
     }
-    launch_conv_tc(L, io, st);
+    for (int i = 0; i < launches; ++i) launch_conv_tc(L, io, st);
   }
   if (xo) launch_act_to_f32(xo->a, y, st);
   if (po) launch_act_to_f32(po->a, p, st);
@@ -182,7 +186,7 @@ int lumi_op_conv2d(const float* x, int n, int h, int w, int cin, const float* wg
                    int impl, float* y, int* ho_out, int* wo_out, void* stream) {
   OP_BEGIN
   return op_conv2d(x, n, h, w, cin, wgt, kh, kw, cout, stride, rate, padding, scale, bias, residual, 0, 0, 1, act, impl,
-                   nullptr, nullptr, y, nullptr, ho_out, wo_out, static_cast<cudaStream_t>(stream));
+                   nullptr, nullptr, y, nullptr, ho_out, wo_out, 0, 1, static_cast<cudaStream_t>(stream));
   OP_END
 }
 
@@ -193,7 +197,7 @@ int lumi_op_conv2d_preact(const float* x, int n, int h, int w, int cin, const fl
   OP_BEGIN
   LUMI_REQUIRE(pre_scale && pre_bias, "conv2d_preact: pre_scale and pre_bias are required");
   return op_conv2d(x, n, h, w, cin, wgt, kh, kw, cout, stride, rate, padding, scale, bias, residual, 0, 0, 1, act, impl,
-                   pre_scale, pre_bias, y, p, ho_out, wo_out, static_cast<cudaStream_t>(stream));
+                   pre_scale, pre_bias, y, p, ho_out, wo_out, 0, 1, static_cast<cudaStream_t>(stream));
   OP_END
 }
 
@@ -205,7 +209,22 @@ int lumi_op_conv2d_io(const float* x, int n, int h, int w, int cin, const float*
   LUMI_REQUIRE(!residual || res_h > 0, "conv2d_io: res_h and res_w are required with a residual");
   LUMI_REQUIRE(!pre_scale == !pre_bias, "conv2d_io: pre_scale and pre_bias go together");
   return op_conv2d(x, n, h, w, cin, wgt, kh, kw, cout, stride, rate, padding, scale, bias, residual, res_h, res_w,
-                   res_stride, act, impl, pre_scale, pre_bias, y, p, ho_out, wo_out, static_cast<cudaStream_t>(stream));
+                   res_stride, act, impl, pre_scale, pre_bias, y, p, ho_out, wo_out, 0, 1,
+                   static_cast<cudaStream_t>(stream));
+  OP_END
+}
+
+int lumi_op_conv2d_sched(const float* x, int n, int h, int w, int cin, const float* wgt, int kh, int kw, int cout,
+                         int stride, int rate, int padding, const float* scale, const float* bias, const float* residual,
+                         int res_h, int res_w, int res_stride, int act, int impl, const float* pre_scale,
+                         const float* pre_bias, int sm_limit, int launches, float* y, float* p, int* ho_out, int* wo_out,
+                         void* stream) {
+  OP_BEGIN
+  LUMI_REQUIRE(!residual || res_h > 0, "conv2d_sched: res_h and res_w are required with a residual");
+  LUMI_REQUIRE(!pre_scale == !pre_bias, "conv2d_sched: pre_scale and pre_bias go together");
+  return op_conv2d(x, n, h, w, cin, wgt, kh, kw, cout, stride, rate, padding, scale, bias, residual, res_h, res_w,
+                   res_stride, act, impl, pre_scale, pre_bias, y, p, ho_out, wo_out, sm_limit, launches,
+                   static_cast<cudaStream_t>(stream));
   OP_END
 }
 

@@ -867,11 +867,10 @@ static dim3 mask_grid(const NmsWorkspace& ws, int problems, int n_max) {
   // that exit at once, and their block-launch overhead dominated the step
   const long nw = (n_max + 63) / 64;
   long maxpairs = nw * (nw + 1) / 2;
-  long gx = ((long)device_sm_count() * 64 + problems - 1) / problems;
+  long gx = ((long)sm_budget(0, ws.sm_limit) * 64 + problems - 1) / problems;
   if (gx > 2048) gx = 2048;
   if (gx > maxpairs) gx = maxpairs;
   if (gx < 1) gx = 1;
-  (void)ws;
   return dim3((unsigned)gx, problems);
 }
 

@@ -51,6 +51,7 @@ SIGNATURES = {
     'lumi_last_launch_count': (ctypes.c_int, [ctypes.c_void_p]),
     'lumi_set_conv_impl': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
     'lumi_set_conv_streamk': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
+    'lumi_set_sm_limit': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
     'lumi_set_debug_taps': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
     'lumi_set_pipeline': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
     'lumi_set_graphs': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
@@ -78,6 +79,10 @@ SIGNATURES = {
     'lumi_op_conv2d_io': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] +
                           [ctypes.c_int] * 6 + [ctypes.c_void_p] * 3 + [ctypes.c_int] * 5 +
                           [ctypes.c_void_p] * 4 + [_c_int_p, _c_int_p, ctypes.c_void_p]),
+    'lumi_op_conv2d_sched': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] +
+                             [ctypes.c_int] * 6 + [ctypes.c_void_p] * 3 + [ctypes.c_int] * 5 +
+                             [ctypes.c_void_p] * 2 + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 2 +
+                             [_c_int_p, _c_int_p, ctypes.c_void_p]),
     'lumi_pack_conv_weights': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 4),
     'lumi_op_max_pool': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 7 + [ctypes.c_void_p, ctypes.c_void_p]),
     'lumi_op_max_pool_preact': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 7 + [ctypes.c_void_p] * 4),
@@ -238,6 +243,13 @@ class Engine(object):
         rc = self._lib.lumi_set_conv_streamk(self._h, {'off': 0, 'auto': 1, 'always': 2}.get(mode, mode))
         if rc != LUMI_OK:
             raise ValueError('stream-K mode must be "off", "auto" or "always"')
+
+    def set_sm_limit(self, sms):
+        """SMs the launch decisions count on (persistent conv grids, stream-K, the wide-tile rule, the NMS grid):
+        0 (default) the device's count; larger values are capped at it.  Runs what a GPU with fewer SMs would."""
+        rc = self._lib.lumi_set_sm_limit(self._h, int(sms))
+        if rc != LUMI_OK:
+            _raise(rc, self._lib.lumi_last_error(self._h))
 
     # ---- forward
     def predict_raw(self, images):
