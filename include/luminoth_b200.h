@@ -102,6 +102,35 @@ int lumi_predict_sizes(lumi_engine* e, const void* const* images, const int32_t*
                        int is_f32, int images_on_device, int n, float* boxes, float* scores, int32_t* labels,
                        int32_t* counts, int outputs_on_device);
 
+/* Sliced prediction of large images (no reference counterpart): nwin windows cut from n source images, each resized
+ * and predicted like lumi_predict_resize, their detections merged per source image on the GPU.
+ *   images, sizes, is_f32, images_on_device   the n sources, as lumi_predict_resize takes them; each is uploaded once
+ *               per call, however many windows read it
+ *   windows     int32 [nwin][7] host array {src, y0, x0, h, w, th, tw}: the h x w region of source src at (y0, x0)
+ *               (inside the source), resized to th x tw with the TF 1.x bilinear resize of lumi_predict_resize
+ *   scales      float [nwin][2] host array {s_y, s_x}: the window's scale_factor as predicting.target_size gives it
+ *               (Faster R-CNN: the same value twice; SSD: its pair)
+ * Windows run in the order given: each maximal run of consecutive windows with equal th x tw runs as forwards of up to
+ * max_batch windows on the lumi_predict_resize path (two-stream halves, CUDA graphs, stream-K).  Then, per source and
+ * label, the windows' detections -- boxes mapped to source pixels as x / s_x + x0, y / s_y + y0 in float32, in window
+ * order then rank -- are sorted by score (stable), suppressed by greedy NMS at iou_threshold (suppress when IoU >
+ * iou_threshold, tf.image.non_max_suppression) keeping class_max_detections per label, and the top
+ * total_max_detections of each source by score (ties: lower label, then earlier kept rank) are its outputs.  With
+ * with_rcnn = false there is one label, 0, and both caps are post_nms_top_n.  Outputs as lumi_predict, per SOURCE image
+ * ([n, kmax, ...], boxes in source pixels).  The call reads the windows' labels and counts back once (it synchronises
+ * the engine's stream midway).  LUMI_EINVAL: n or nwin below 1, a window naming no source, outside its source or with
+ * a size below 1, scales not finite and positive, an SSD target other than the fixed size, a record output set. */
+int lumi_predict_windows(lumi_engine* e, const void* const* images, const int32_t* sizes, int is_f32,
+                         int images_on_device, int n, const int32_t* windows, const float* scales, int nwin,
+                         float iou_threshold, float* boxes, float* scores, int32_t* labels, int32_t* counts,
+                         int outputs_on_device);
+
+/* Test query: the per-window detections of the last completed lumi_predict_windows (host arrays [nwin][kmax][4],
+ * [nwin][kmax], [nwin][kmax], [nwin]; each may be NULL) and merge_stats[4] = {bytes of the merge workspace, window
+ * detections merged, longest per-(source, label) list, list groups} (may be NULL). */
+int lumi_last_window_detections(lumi_engine* e, float* boxes, float* scores, int32_t* labels, int32_t* counts,
+                                int64_t* merge_stats);
+
 int lumi_max_detections(lumi_engine* e);
 
 /* Multi-GPU detection exchange (SURVEY 8e; the reference has no counterpart -- it predicts one image at a time,

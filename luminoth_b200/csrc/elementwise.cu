@@ -7,18 +7,19 @@ namespace lumi {
 // tf.image.resize_images(BILINEAR) of TF 1.x (legacy kernel: align_corners=False, src = dst * (in / out), no
 // half-pixel offset) -- luminoth/utils/image.py:94-97,139-142.  Same float32 operation order as the oracle
 // (tf_ops.resize_bilinear), no FMA contraction, so the result is bit-identical to it.  Pixel (y, x) of the h x w
-// output of the h0 x w0 HWC image src, hs = h0 / h and ws = w0 / w in float32.
+// output of the h0 x w0 HWC image src, hs = h0 / h and ws = w0 / w in float32; its rows start `pitch` pixels apart
+// (w0, or the width of the larger image a window lies in).
 template <typename PIX>
-__device__ __forceinline__ void bilinear_sample(const PIX* __restrict__ src, int h0, int w0, float hs, float ws, int y,
-                                                int x, float (&v)[3]) {
+__device__ __forceinline__ void bilinear_sample(const PIX* __restrict__ src, int h0, int w0, int pitch, float hs,
+                                                float ws, int y, int x, float (&v)[3]) {
   const float fy = __fmul_rn((float)y, hs), fx = __fmul_rn((float)x, ws);
   const int y0 = (int)floorf(fy), x0 = (int)floorf(fx);
   const int y1 = min(y0 + 1, h0 - 1), x1 = min(x0 + 1, w0 - 1);
   const float yl = __fsub_rn(fy, (float)y0), xl = __fsub_rn(fx, (float)x0);
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    const float tl = (float)src[((size_t)y0 * w0 + x0) * 3 + c], tr = (float)src[((size_t)y0 * w0 + x1) * 3 + c];
-    const float bl = (float)src[((size_t)y1 * w0 + x0) * 3 + c], br = (float)src[((size_t)y1 * w0 + x1) * 3 + c];
+    const float tl = (float)src[((size_t)y0 * pitch + x0) * 3 + c], tr = (float)src[((size_t)y0 * pitch + x1) * 3 + c];
+    const float bl = (float)src[((size_t)y1 * pitch + x0) * 3 + c], br = (float)src[((size_t)y1 * pitch + x1) * 3 + c];
     const float top = __fadd_rn(tl, __fmul_rn(__fsub_rn(tr, tl), xl));
     const float bot = __fadd_rn(bl, __fmul_rn(__fsub_rn(br, bl), xl));
     v[c] = __fadd_rn(top, __fmul_rn(__fsub_rn(bot, top), yl));
@@ -31,7 +32,7 @@ __global__ void resize_bilinear_kernel(const PIX* __restrict__ src, int h0, int 
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)h * w) return;
   float v[3];
-  bilinear_sample(src, h0, w0, hs, ws, (int)(i / w), (int)(i % w), v);
+  bilinear_sample(src, h0, w0, w0, hs, ws, (int)(i / w), (int)(i % w), v);
   dst[i * 3] = v[0]; dst[i * 3 + 1] = v[1]; dst[i * 3 + 2] = v[2];
 }
 void launch_resize_bilinear(const void* src, bool src_f32, int h0, int w0, float* dst, int h, int w, cudaStream_t st) {
@@ -72,7 +73,7 @@ struct ResizedPixels {
   }
   __device__ __forceinline__ void load(int ni, int y, int x, float (&v)[3]) const {
     const ResizeSrc t = table[ni];
-    bilinear_sample(reinterpret_cast<const PIX*>(base + t.off), t.h0, t.w0, t.hs, t.ws, y, x, v);
+    bilinear_sample(reinterpret_cast<const PIX*>(base + t.off), t.h0, t.w0, t.pitch, t.hs, t.ws, y, x, v);
   }
 };
 // Calls launch(pixels) with the source policy `src` describes.

@@ -173,6 +173,12 @@ struct lumi_engine {
   uint8_t* h_src = nullptr; size_t h_src_cap = 0;
   ResizeSrc* d_resize_tab = nullptr;             // [max_batch]
   cudaEvent_t ev_src[2] = {nullptr, nullptr};    // after each half's upload from h_src (h_src is reused once they pass)
+  // lumi_predict_windows: the windows' detections, window table and merged outputs (d_win), and the merge scratch
+  // (d_merge), both grown per call; what the last call held, for lumi_last_window_detections
+  uint8_t* d_win = nullptr; size_t win_cap = 0;
+  uint8_t* d_merge = nullptr; size_t merge_cap = 0;
+  int last_nwin = 0;
+  int64_t merge_stats[4] = {0, 0, 0, 0};         // merge scratch bytes, candidates, longest list, groups
   float* d_boxes = nullptr; float* d_scores = nullptr; int* d_labels = nullptr; int* d_counts = nullptr;
   int* d_prop_counts = nullptr;
   float* d_records = nullptr;   // caller-owned device buffer [max_batch][1 + 6*kmax] (lumi_set_record_output) or null
@@ -212,7 +218,7 @@ struct lumi_engine {
     cudaFree(d_anchor_ref); cudaFree(d_final_keys); cudaFree(d_ssd_anchors);
     for (auto& kv : anchor_grids) cudaFree(kv.second);
     cudaFree(arena.base); cudaFree(arena2.base); cudaFree(d_final_keys2); cudaFree(d_overflow); cudaFree(d_images);
-    cudaFree(d_src); cudaFree(d_resize_tab);
+    cudaFree(d_src); cudaFree(d_resize_tab); cudaFree(d_win); cudaFree(d_merge);
     if (h_src) cudaFreeHost(h_src);
     for (auto ev : ev_src) if (ev) cudaEventDestroy(ev);
     if (ev_fork) cudaEventDestroy(ev_fork);
@@ -1536,6 +1542,8 @@ struct PredictInput {
                                       // at the top left of the h x w canvas; null: every image is h x w
   int esz = 1;                  // bytes per channel value: 1 uint8, 4 float32
   int on_device = 0;
+  const ResizeSrc* rows = nullptr;    // windows (lumi_predict_windows): the n table rows of this chunk, in the pinned
+                                      // buffer; the sources are already in e->d_src
 };
 
 // One copy of a half-batch's upload; with `pack`, the host source is first copied from there into src (pinned), so
@@ -1583,7 +1591,7 @@ static void stage_resize(lumi_engine* e, const PredictInput& in, int n, int nA, 
   for (int i = 0; i < n; ++i) {
     const int h0 = in.sizes[2 * i], w0 = in.sizes[2 * i + 1];
     const int th = in.targets ? in.targets[2 * i] : h, tw = in.targets ? in.targets[2 * i + 1] : w;
-    rows[i] = ResizeSrc{(long long)off[i], h0, w0, (float)h0 / (float)th, (float)w0 / (float)tw, th, tw};  // as launch_resize_bilinear
+    rows[i] = ResizeSrc{(long long)off[i], h0, w0, (float)h0 / (float)th, (float)w0 / (float)tw, th, tw, w0};  // as launch_resize_bilinear
   }
   const int bounds[3] = {0, nA, n};
   for (int k = 0; k < 2; ++k) {
@@ -1598,16 +1606,23 @@ static void stage_resize(lumi_engine* e, const PredictInput& in, int n, int nA, 
   }
 }
 
-static int predict_impl(lumi_engine* e, const PredictInput& in, int n, int h, int w, float* boxes, float* scores,
+// lumi_predict_windows's staging of one chunk: the table rows of windows [0, nA) in up[0], of [nA, n) in up[1]
+static void stage_window_rows(lumi_engine* e, const PredictInput& in, int n, int nA, std::vector<Upload> (&up)[2]) {
+  const int bounds[3] = {0, nA, n};
+  for (int k = 0; k < 2; ++k)
+    if (bounds[k] < bounds[k + 1])
+      up[k].push_back({e->d_resize_tab + bounds[k], in.rows + bounds[k],
+                       (size_t)(bounds[k + 1] - bounds[k]) * sizeof(ResizeSrc), cudaMemcpyHostToDevice});
+}
+
+static void predict_run(lumi_engine* e, const PredictInput& in, int n, int h, int w, float* boxes, float* scores,
                         int* labels, int* counts, int outputs_on_device) {
-  if (!e) return LUMI_EINVAL;
-  LUMI_API_BEGIN
   if (!e->finalized) throw Error(LUMI_ESTATE, "lumi_predict before lumi_finalize");
   const bool resize = in.sources != nullptr, packed = in.targets != nullptr;
   LUMI_REQUIRE((in.images || resize) && boxes && scores && labels && counts, "lumi_predict: null buffer");
   LUMI_REQUIRE(n > 0 && n <= e->max_batch, "lumi_predict: batch size exceeds max_batch");
   LUMI_REQUIRE(h > 0 && w > 0, "lumi_predict: empty image");
-  if (resize) {
+  if (resize && !in.rows) {
     LUMI_REQUIRE(in.sizes, "lumi_predict_resize: null sizes");
     for (int i = 0; i < n; ++i) {
       const int h0 = in.sizes[2 * i], w0 = in.sizes[2 * i + 1];
@@ -1640,7 +1655,8 @@ static int predict_impl(lumi_engine* e, const PredictInput& in, int n, int h, in
   std::vector<Upload> up[2];
   const uint8_t *img_a, *img_b;
   if (resize) {
-    stage_resize(e, in, n, nA, h, w, up);
+    if (in.rows) stage_window_rows(e, in, n, nA, up);
+    else stage_resize(e, in, n, nA, h, w, up);
     img_a = img_b = e->d_src;                      // the table rows hold the offsets
   } else {
     const size_t img_bytes = (size_t)n * h * w * 3 * in.esz;
@@ -1709,6 +1725,13 @@ static int predict_impl(lumi_engine* e, const PredictInput& in, int n, int h, in
       throw Error(LUMI_EOVERFLOW, "an activation exceeded the fp16x2 split range (|x| > 65504); results are invalid");
     }
   }
+}
+
+static int predict_impl(lumi_engine* e, const PredictInput& in, int n, int h, int w, float* boxes, float* scores,
+                        int* labels, int* counts, int outputs_on_device) {
+  if (!e) return LUMI_EINVAL;
+  LUMI_API_BEGIN
+  predict_run(e, in, n, h, w, boxes, scores, labels, counts, outputs_on_device);
   return LUMI_OK;
   LUMI_API_END(e)
 }
@@ -1762,6 +1785,194 @@ int lumi_predict_sizes(lumi_engine* e, const void* const* images, const int32_t*
     in.targets = targets;
   }
   return predict_impl(e, in, n, hc, wc, boxes, scores, labels, counts, outputs_on_device);
+}
+
+// A device buffer of at least `need` bytes that no graph points into: grown after the streams drain.
+static void ensure_scratch(lumi_engine* e, uint8_t*& buf, size_t& cap, size_t need) {
+  if (need <= cap) return;
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+  if (e->stream2) LUMI_CUDA_CHECK(cudaStreamSynchronize(e->stream2));
+  cudaFree(buf);
+  buf = nullptr; cap = 0;
+  LUMI_CUDA_CHECK(cudaMalloc(&buf, need));
+  cap = need;
+}
+
+int lumi_predict_windows(lumi_engine* e, const void* const* images, const int32_t* sizes, int is_f32,
+                         int images_on_device, int n, const int32_t* windows, const float* scales, int nwin,
+                         float iou_threshold, float* boxes, float* scores, int32_t* labels, int32_t* counts,
+                         int outputs_on_device) {
+  if (!e) return LUMI_EINVAL;
+  LUMI_API_BEGIN
+  if (!e->finalized) throw Error(LUMI_ESTATE, "lumi_predict_windows before lumi_finalize");
+  LUMI_REQUIRE(images && sizes && windows && scales && boxes && scores && labels && counts,
+               "lumi_predict_windows: null buffer");
+  LUMI_REQUIRE(n >= 1, "lumi_predict_windows: no source images");
+  LUMI_REQUIRE(nwin >= 1, "lumi_predict_windows: no windows");
+  LUMI_REQUIRE(!e->d_records, "lumi_predict_windows: a record output is set (lumi_set_record_output); tiled "
+                              "prediction writes no records");
+  LUMI_REQUIRE(iou_threshold >= 0.f, "lumi_predict_windows: iou_threshold must be >= 0");
+  const int esz = is_f32 ? 4 : 1;
+  std::vector<size_t> off(n + 1, 0);
+  for (int i = 0; i < n; ++i) {
+    const int h0 = sizes[2 * i], w0 = sizes[2 * i + 1];
+    LUMI_REQUIRE(h0 >= 1 && w0 >= 1, "lumi_predict_windows: source image " + std::to_string(i) + " is " +
+                                         std::to_string(h0) + " x " + std::to_string(w0) + ", sizes must be >= 1");
+    LUMI_REQUIRE((long long)h0 * w0 < (1LL << 30), "lumi_predict_windows: source image too large");
+    LUMI_REQUIRE(images[i], "lumi_predict_windows: null source image " + std::to_string(i));
+    off[i + 1] = off[i] + round16((size_t)h0 * w0 * 3 * esz);
+  }
+  for (int k = 0; k < nwin; ++k) {
+    const int32_t* wk = windows + 7 * k;
+    const std::string name = "lumi_predict_windows: window " + std::to_string(k);
+    LUMI_REQUIRE(wk[0] >= 0 && wk[0] < n, name + " names source " + std::to_string(wk[0]) + " of " + std::to_string(n));
+    LUMI_REQUIRE(wk[3] >= 1 && wk[4] >= 1 && wk[5] >= 1 && wk[6] >= 1, name + ": sizes must be >= 1");
+    const int H = sizes[2 * wk[0]], W = sizes[2 * wk[0] + 1];
+    LUMI_REQUIRE(wk[1] >= 0 && wk[2] >= 0 && (long long)wk[1] + wk[3] <= H && (long long)wk[2] + wk[4] <= W,
+                 name + " is not inside its " + std::to_string(H) + " x " + std::to_string(W) + " source");
+    LUMI_REQUIRE(e->type == "fasterrcnn" || (wk[5] == e->fixed_h && wk[6] == e->fixed_w),
+                 name + ": SSD runs at its fixed size only");
+    LUMI_REQUIRE(scales[2 * k] > 0.f && scales[2 * k + 1] > 0.f && std::isfinite(scales[2 * k]) &&
+                 std::isfinite(scales[2 * k + 1]), name + ": scales must be finite and > 0");
+  }
+  LUMI_CUDA_CHECK(cudaSetDevice(e->device));
+  const size_t K = (size_t)e->kmax;
+
+  // every source once into e->d_src; every window's table row into the pinned buffer, ahead of its sources
+  ensure_device_buffer(e, e->d_src, e->src_cap, off[n]);
+  if (!e->d_resize_tab) {
+    LUMI_CUDA_CHECK(cudaMalloc(&e->d_resize_tab, (size_t)e->max_batch * sizeof(ResizeSrc)));
+    for (auto& ev : e->ev_src) LUMI_CUDA_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  }
+  const size_t tab_bytes = round16((size_t)nwin * sizeof(ResizeSrc));
+  const size_t pinned = tab_bytes + (images_on_device ? 0 : off[n]);
+  for (auto ev : e->ev_src) LUMI_CUDA_CHECK(cudaEventSynchronize(ev));
+  if (pinned > e->h_src_cap) {
+    if (e->h_src) cudaFreeHost(e->h_src);
+    e->h_src = nullptr; e->h_src_cap = 0;
+    LUMI_CUDA_CHECK(cudaHostAlloc((void**)&e->h_src, pinned, cudaHostAllocDefault));
+    e->h_src_cap = pinned;
+  }
+  ResizeSrc* rows = reinterpret_cast<ResizeSrc*>(e->h_src);
+  std::vector<float4> wmap(nwin);
+  std::vector<int> win_src(nwin);
+  for (int k = 0; k < nwin; ++k) {
+    const int32_t* wk = windows + 7 * k;
+    const int W = sizes[2 * wk[0] + 1];
+    const size_t first = off[wk[0]] + ((size_t)wk[1] * W + wk[2]) * 3 * esz;    // the window's top-left pixel
+    rows[k] = ResizeSrc{(long long)first, wk[3], wk[4], (float)wk[3] / (float)wk[5], (float)wk[4] / (float)wk[6],
+                        wk[5], wk[6], W};
+    wmap[k] = make_float4((float)wk[1], (float)wk[2], scales[2 * k], scales[2 * k + 1]);
+    win_src[k] = wk[0];
+  }
+  for (int i = 0; i < n; ++i) {
+    const size_t bytes = (size_t)sizes[2 * i] * sizes[2 * i + 1] * 3 * esz;
+    if (images_on_device) {
+      LUMI_CUDA_CHECK(cudaMemcpyAsync(e->d_src + off[i], images[i], bytes, cudaMemcpyDeviceToDevice, e->stream));
+    } else {
+      uint8_t* host = e->h_src + tab_bytes + off[i];
+      std::memcpy(host, images[i], bytes);
+      LUMI_CUDA_CHECK(cudaMemcpyAsync(e->d_src + off[i], host, bytes, cudaMemcpyHostToDevice, e->stream));
+    }
+  }
+
+  // the windows' detections [nwin][kmax], their map to source pixels [nwin], the merged outputs [n][kmax]
+  size_t o = 0;
+  auto carve = [&o](size_t bytes) { const size_t at = o; o += round16(bytes); return at; };
+  const size_t o_wb = carve(nwin * K * 16), o_ws = carve(nwin * K * 4), o_wl = carve(nwin * K * 4),
+               o_wc = carve(nwin * 4), o_map = carve(nwin * sizeof(float4)), o_ob = carve(n * K * 16),
+               o_os = carve(n * K * 4), o_ol = carve(n * K * 4), o_oc = carve(n * 4);
+  ensure_scratch(e, e->d_win, e->win_cap, o);
+  float* wboxes = reinterpret_cast<float*>(e->d_win + o_wb);
+  float* wscores = reinterpret_cast<float*>(e->d_win + o_ws);
+  int* wlabels = reinterpret_cast<int*>(e->d_win + o_wl);
+  int* wcounts = reinterpret_cast<int*>(e->d_win + o_wc);
+  float4* d_map = reinterpret_cast<float4*>(e->d_win + o_map);
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(d_map, wmap.data(), nwin * sizeof(float4), cudaMemcpyHostToDevice, e->stream));
+  e->last_nwin = 0;
+
+  // each maximal run of equal targets as forwards of up to max_batch windows, the lumi_predict_resize path
+  PredictInput in;
+  in.sources = images; in.esz = esz; in.on_device = images_on_device;
+  int launches = 0, replays = 0;
+  for (int a = 0; a < nwin;) {
+    int b = a + 1;
+    while (b < nwin && b - a < e->max_batch && windows[7 * b + 5] == windows[7 * a + 5] &&
+           windows[7 * b + 6] == windows[7 * a + 6])
+      ++b;
+    in.rows = rows + a;
+    predict_run(e, in, b - a, windows[7 * a + 5], windows[7 * a + 6], wboxes + a * K * 4, wscores + a * K,
+                wlabels + a * K, wcounts + a, 1);
+    launches += e->launches; replays += e->graph_replays;
+    a = b;
+  }
+  e->last_nwin = nwin;
+
+  // one read of the windows' labels and counts lays out the per-(source, label) lists
+  std::vector<int> hl(nwin * K), hc(nwin);
+  int ovf = 0;
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(hl.data(), wlabels, nwin * K * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(hc.data(), wcounts, nwin * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(&ovf, e->d_overflow, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+  if (ovf) {
+    LUMI_CUDA_CHECK(cudaMemset(e->d_overflow, 0, sizeof(int)));
+    throw Error(LUMI_EOVERFLOW, "an activation exceeded the fp16x2 split range (|x| > 65504); results are invalid");
+  }
+  const bool rpn_only = e->type == "fasterrcnn" && !e->with_rcnn;    // one label, post_nms_top_n (= kmax) per step
+  const int nc = rpn_only ? 1 : e->num_classes;
+  const int class_max = rpn_only ? e->kmax : e->det.class_max;
+  WindowMergePlan plan;
+  plan_window_merge(win_src.data(), hl.data(), hc.data(), nwin, e->kmax, n, nc, class_max, e->kmax, plan);
+  const size_t scratch = window_merge_bytes(plan);
+  const size_t o_slots = round16(scratch), o_lists = o_slots + round16(plan.slots.size() * sizeof(int));
+  ensure_scratch(e, e->d_merge, e->merge_cap, o_lists + round16(plan.lists.size() * sizeof(int)));
+  int* d_slots = reinterpret_cast<int*>(e->d_merge + o_slots);
+  int* d_lists = reinterpret_cast<int*>(e->d_merge + o_lists);
+  if (!plan.slots.empty())
+    LUMI_CUDA_CHECK(cudaMemcpyAsync(d_slots, plan.slots.data(), plan.slots.size() * sizeof(int),
+                                    cudaMemcpyHostToDevice, e->stream));
+  if (!plan.lists.empty())
+    LUMI_CUDA_CHECK(cudaMemcpyAsync(d_lists, plan.lists.data(), plan.lists.size() * sizeof(int),
+                                    cudaMemcpyHostToDevice, e->stream));
+  g_launch_count = 0;
+  float* obox = reinterpret_cast<float*>(e->d_win + o_ob);
+  float* oscore = reinterpret_cast<float*>(e->d_win + o_os);
+  int* olab = reinterpret_cast<int*>(e->d_win + o_ol);
+  int* ocount = reinterpret_cast<int*>(e->d_win + o_oc);
+  launch_window_merge(plan, d_slots, d_lists, wboxes, wscores, d_map, iou_threshold, e->sm_limit, e->d_merge, obox,
+                      oscore, olab, ocount, e->stream);
+  e->launches = launches + g_launch_count;
+  e->graph_replays = replays;
+  e->merge_stats[0] = (int64_t)(o_lists + plan.lists.size() * sizeof(int)); e->merge_stats[1] = plan.candidates;
+  e->merge_stats[2] = plan.longest; e->merge_stats[3] = (int64_t)plan.groups.size();
+  const cudaMemcpyKind kind = outputs_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(boxes, obox, n * K * 4 * sizeof(float), kind, e->stream));
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(scores, oscore, n * K * sizeof(float), kind, e->stream));
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(labels, olab, n * K * sizeof(int), kind, e->stream));
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(counts, ocount, n * sizeof(int), kind, e->stream));
+  if (!outputs_on_device) LUMI_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+  return LUMI_OK;
+  LUMI_API_END(e)
+}
+
+int lumi_last_window_detections(lumi_engine* e, float* boxes, float* scores, int32_t* labels, int32_t* counts,
+                                int64_t* merge_stats) {
+  if (!e) return LUMI_EINVAL;
+  LUMI_API_BEGIN
+  LUMI_REQUIRE(e->last_nwin > 0, "lumi_last_window_detections: no lumi_predict_windows call has completed");
+  LUMI_CUDA_CHECK(cudaSetDevice(e->device));
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+  const size_t nw = (size_t)e->last_nwin, K = (size_t)e->kmax;
+  const uint8_t* base = e->d_win;          // the layout lumi_predict_windows carves, in the same order
+  const size_t o_ws = round16(nw * K * 16), o_wl = o_ws + round16(nw * K * 4), o_wc = o_wl + round16(nw * K * 4);
+  if (boxes) LUMI_CUDA_CHECK(cudaMemcpy(boxes, base, nw * K * 16, cudaMemcpyDeviceToHost));
+  if (scores) LUMI_CUDA_CHECK(cudaMemcpy(scores, base + o_ws, nw * K * 4, cudaMemcpyDeviceToHost));
+  if (labels) LUMI_CUDA_CHECK(cudaMemcpy(labels, base + o_wl, nw * K * 4, cudaMemcpyDeviceToHost));
+  if (counts) LUMI_CUDA_CHECK(cudaMemcpy(counts, base + o_wc, nw * 4, cudaMemcpyDeviceToHost));
+  if (merge_stats) for (int i = 0; i < 4; ++i) merge_stats[i] = e->merge_stats[i];
+  return LUMI_OK;
+  LUMI_API_END(e)
 }
 
 int lumi_max_detections(lumi_engine* e) { return e ? e->kmax : 0; }

@@ -1,6 +1,7 @@
 // Launchers for the HBM-bound stages of the path (everything that is not a conv).
 #pragma once
 #include "common.cuh"
+#include <vector>
 
 namespace lumi {
 
@@ -8,12 +9,15 @@ namespace lumi {
 // One source image of a fused resize: its first byte at `off` in the source buffer, h0 x w0 RGB pixels, resized to its
 // target th x tw with the scale factors hs = (float)h0 / th, ws = (float)w0 / tw (as launch_resize_bilinear computes
 // them).  A uniform batch has th x tw = the batch's h x w; a packed batch (lumi_predict_sizes) places each image at the
-// top left of its h x w canvas, and the per-image kernels below read th x tw from this one table.
+// top left of its h x w canvas, and the per-image kernels below read th x tw from this one table.  pitch: pixels
+// between the starts of two source rows -- w0 for a whole image; a window of a larger source (lumi_predict_windows)
+// has `off` at its top-left pixel, h0 x w0 its own size and pitch the source's width.
 struct ResizeSrc {
   long long off;
   int h0, w0;
   float hs, ws;
   int th, tw;
+  int pitch;
 };
 // The pixels the input staging kernels read: with table == nullptr, img is the batch itself [n][h][w][3]; otherwise
 // image i of the batch is table[i]'s source in img, bilinearly resized on the fly.  f32: float32 pixels, else uint8.
@@ -140,6 +144,35 @@ void launch_class_detections(const float* boxes_in, long boxes_img_stride, const
                              float* records = nullptr /* optional packed rows [nimg][1 + 6*total_max], see postproc.cu */);
 void launch_pack_records(const float* boxes, const float* scores, const int* labels, const int* counts, int nimg,
                          int kmax, float* records, cudaStream_t st);
+
+// ---- cross-window merge of lumi_predict_windows (postproc.cu)
+// The per-(source, label) candidate lists of the window detections, laid out from their labels and counts on the host.
+// Lists with candidates run in groups: sorted by length (longest first), a group takes lists while their count times
+// the group's first (longest) length stays within the call's candidate total T, so every group's [problems][cap]
+// buffers hold at most T candidates, whatever the number of classes and windows (DESIGN section 4.2).
+struct WindowMergePlan {
+  struct Group { int problems, cap; long long slot0; int prob0; };
+  int nsrc = 0, nc = 0, class_max = 0, total_max = 0, kmax = 0;
+  long long candidates = 0;     // T: window detections in the call
+  int longest = 0;              // L: the longest list
+  long long elems = 0;          // largest group's problems x cap (<= T)
+  int pmax = 0;                 // most lists in one group
+  size_t mask_words = 0;        // largest group's NMS bit mask, in u64 words
+  std::vector<Group> groups;
+  std::vector<int> slots;       // per group [problems][cap]: candidate (window * kmax + rank) or -1 (padding)
+  std::vector<int> lists;       // per group [problems]: source * nc + label
+};
+// win_src [nwin] source of each window; labels [nwin][kmax], counts [nwin] (host) the windows' detections.
+void plan_window_merge(const int* win_src, const int* labels, const int* counts, int nwin, int kmax, int nsrc, int nc,
+                       int class_max, int total_max, WindowMergePlan& plan);
+size_t window_merge_bytes(const WindowMergePlan& plan);     // device scratch launch_window_merge needs
+// Maps each window detection to source pixels (x / s_x + x0, y / s_y + y0; wmap [nwin] = {y0, x0, s_y, s_x}), sorts
+// each list by score (stable), runs greedy NMS at thr keeping class_max per list, and writes per source the top
+// total_max of the kept detections, label-major on ties: boxes [nsrc][total_max][4], scores, labels, counts [nsrc].
+// d_slots / d_lists: plan.slots / plan.lists on the device.
+void launch_window_merge(const WindowMergePlan& plan, const int* d_slots, const int* d_lists, const float* wboxes,
+                         const float* wscores, const float4* wmap, float thr, int sm_limit, void* scratch,
+                         float* boxes, float* scores, int* labels, int* counts, cudaStream_t st);
 
 void launch_sort_desc(const float* scores, int n, int* idx_out, NmsWorkspace& ws, cudaStream_t st);
 void launch_nms_sorted(const float* boxes_sorted, int n, float thr, int max_out, NmsWorkspace& ws, int* keep,

@@ -12,6 +12,7 @@
 // (>=, >, iou > thr) must agree with the fp32 reference bit for bit on equal inputs.
 #include "ops.cuh"
 #include "conv.cuh"
+#include <algorithm>
 #include <cstdlib>
 
 namespace lumi {
@@ -1148,6 +1149,179 @@ void launch_class_detections(const float* boxes_in, long boxes_img_stride, const
   dim3 g4(cdiv(p.total_max, 128), nimg);
   det_output_kernel<<<g4, 128, 0, st>>>(ws.sboxes, ws.sscores, ws.keep, forder, fnvalid, p.nc, ws.ncap, p.class_max,
                                         p.total_max, objects, labels, probs, counts, records);
+  count_launch();
+  LUMI_CUDA_CHECK(cudaGetLastError());
+}
+
+// ------------------------------------------------------------------ cross-window merge (lumi_predict_windows)
+void plan_window_merge(const int* win_src, const int* labels, const int* counts, int nwin, int kmax, int nsrc, int nc,
+                       int class_max, int total_max, WindowMergePlan& plan) {
+  plan = WindowMergePlan();
+  plan.nsrc = nsrc; plan.nc = nc; plan.class_max = class_max; plan.total_max = total_max; plan.kmax = kmax;
+  const size_t P = (size_t)nsrc * nc;
+  std::vector<long long> len(P, 0);
+  for (int k = 0; k < nwin; ++k) {
+    LUMI_REQUIRE(counts[k] >= 0 && counts[k] <= kmax, "window merge: detection count out of range");
+    for (int r = 0; r < counts[k]; ++r) {
+      const int lab = labels[(size_t)k * kmax + r];
+      LUMI_REQUIRE(lab >= 0 && lab < nc, "window merge: detection label out of range");
+      len[(size_t)win_src[k] * nc + lab]++;
+    }
+  }
+  std::vector<long long> start(P + 1, 0);
+  for (size_t p = 0; p < P; ++p) start[p + 1] = start[p] + len[p];
+  plan.candidates = start[P];
+  // every list in window order, then rank within the window
+  std::vector<int> flat((size_t)plan.candidates);
+  std::vector<long long> fill(start.begin(), start.end() - 1);
+  for (int k = 0; k < nwin; ++k)
+    for (int r = 0; r < counts[k]; ++r)
+      flat[(size_t)fill[(size_t)win_src[k] * nc + labels[(size_t)k * kmax + r]]++] = k * kmax + r;
+  std::vector<int> order;
+  for (size_t p = 0; p < P; ++p) if (len[p]) order.push_back((int)p);
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return len[a] > len[b]; });
+  plan.longest = order.empty() ? 0 : (int)len[order[0]];
+  for (size_t i = 0; i < order.size();) {
+    const long long cap = len[order[i]];
+    const long long take = std::min<long long>((long long)order.size() - (long long)i,
+                                               std::max<long long>(1, plan.candidates / cap));
+    plan.groups.push_back({(int)take, (int)cap, (long long)plan.slots.size(), (int)plan.lists.size()});
+    for (long long j = 0; j < take; ++j) {
+      const int p = order[i + j];
+      plan.lists.push_back(p);
+      plan.slots.insert(plan.slots.end(), flat.begin() + start[p], flat.begin() + start[p] + len[p]);
+      plan.slots.insert(plan.slots.end(), (size_t)(cap - len[p]), -1);
+    }
+    plan.elems = std::max(plan.elems, take * cap);
+    plan.pmax = std::max(plan.pmax, (int)take);
+    plan.mask_words = std::max(plan.mask_words, (size_t)(take * cap) * (size_t)nms_words((int)cap));
+    i += (size_t)take;
+  }
+}
+
+namespace {
+struct MergeScratch {
+  NmsWorkspace ws;              // the groups' sort / NMS buffers, viewed per group as [problems][cap]
+  float* kboxes; float* kscores; int* kkeep; int* knkeep;   // kept detections per list [nsrc * nc][class_max]
+  float* final_keys;            // det_final_scratch_bytes(nsrc, nc, class_max)
+  size_t bytes;
+};
+// Carves the scratch of a plan out of `base` (nullptr: sizes only).
+MergeScratch carve_merge(const WindowMergePlan& pl, uint8_t* base) {
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    uint8_t* p = base ? base + off : nullptr;
+    off += (bytes + 255) / 256 * 256;
+    return p;
+  };
+  MergeScratch m{};
+  const size_t E = (size_t)std::max<long long>(pl.elems, 1), pm = (size_t)std::max(pl.pmax, 1);
+  const size_t lists = (size_t)pl.nsrc * pl.nc, kept = lists * pl.class_max;
+  m.ws.keys = (float*)take(E * 4);
+  m.ws.boxes = (float*)take(E * 16);
+  m.ws.order = (int*)take(E * 4);
+  m.ws.nvalid = (int*)take(pm * 4);
+  m.ws.sboxes = (float*)take(E * 16);
+  m.ws.sscores = (float*)take(E * 4);
+  m.ws.mask = (unsigned long long*)take(std::max<size_t>(pl.mask_words, 1) * 8);
+  m.ws.keep = (int*)take(pm * pl.class_max * 4);
+  m.ws.nkeep = (int*)take(pm * 4);
+  m.ws.sort_tmp = (unsigned long long*)take(E * 2 * 8);
+  if (pl.longest >= NMS_LAZY_MIN) {             // two-phase NMS scratch, as nms_workspace_alloc
+    m.ws.sboxes2 = (float*)take(E * 16);
+    m.ws.index_map = (int*)take(E * 4);
+    m.ws.alive = (unsigned char*)take(E);
+    m.ws.nvalid2 = (int*)take(pm * 4);
+  }
+  m.kboxes = (float*)take(kept * 16);
+  m.kscores = (float*)take(kept * 4);
+  m.kkeep = (int*)take(kept * 4);
+  m.knkeep = (int*)take(lists * 4);
+  m.final_keys = (float*)take(det_final_scratch_bytes(pl.nsrc, pl.nc, pl.class_max));
+  m.bytes = off;
+  return m;
+}
+}  // namespace
+
+size_t window_merge_bytes(const WindowMergePlan& plan) { return carve_merge(plan, nullptr).bytes; }
+
+// slot i of a group: its candidate's box in source pixels and its score, or key -1 for padding
+__global__ void window_gather_kernel(const float* __restrict__ wboxes, const float* __restrict__ wscores,
+                                     const float4* __restrict__ wmap, const int* __restrict__ slots, int kmax,
+                                     long long n, float* __restrict__ keys, float* __restrict__ boxes) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int c = slots[i];
+  if (c < 0) { keys[i] = -1.f; return; }
+  const float4 m = wmap[c / kmax];              // {y0, x0, s_y, s_x}
+  float4 b = reinterpret_cast<const float4*>(wboxes)[c];
+  b.x = __fadd_rn(__fdiv_rn(b.x, m.w), m.y);
+  b.y = __fadd_rn(__fdiv_rn(b.y, m.z), m.x);
+  b.z = __fadd_rn(__fdiv_rn(b.z, m.w), m.y);
+  b.w = __fadd_rn(__fdiv_rn(b.w, m.z), m.x);
+  reinterpret_cast<float4*>(boxes)[i] = b;
+  keys[i] = wscores[c];
+}
+
+// a group's NMS selections into their list's row of the kept buffers, in selection order (keep = identity there)
+__global__ void window_keep_kernel(const float* __restrict__ sboxes, const float* __restrict__ sscores,
+                                   const int* __restrict__ keep, const int* __restrict__ nkeep,
+                                   const int* __restrict__ lists, int cap, int class_max, float* __restrict__ kboxes,
+                                   float* __restrict__ kscores, int* __restrict__ kkeep, int* __restrict__ knkeep) {
+  const int p = blockIdx.y;
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  const int list = lists[p], nk = nkeep[p];
+  if (j == 0) knkeep[list] = nk;
+  if (j >= nk || j >= class_max) return;
+  const size_t src = (size_t)p * cap + keep[(size_t)p * class_max + j];
+  const size_t dst = (size_t)list * class_max + j;
+  reinterpret_cast<float4*>(kboxes)[dst] = reinterpret_cast<const float4*>(sboxes)[src];
+  kscores[dst] = sscores[src];
+  kkeep[dst] = j;
+}
+
+void launch_window_merge(const WindowMergePlan& plan, const int* d_slots, const int* d_lists, const float* wboxes,
+                         const float* wscores, const float4* wmap, float thr, int sm_limit, void* scratch,
+                         float* boxes, float* scores, int* labels, int* counts, cudaStream_t st) {
+  MergeScratch m = carve_merge(plan, static_cast<uint8_t*>(scratch));
+  const int lists = plan.nsrc * plan.nc, cm = plan.class_max;
+  if (!lists) return;
+  LUMI_CUDA_CHECK(cudaMemsetAsync(m.knkeep, 0, (size_t)lists * sizeof(int), st));
+  for (const WindowMergePlan::Group& g : plan.groups) {
+    NmsWorkspace ws = m.ws;
+    ws.problems = g.problems; ws.cap = ws.ncap = g.cap; ws.words = nms_words(g.cap);
+    ws.max_out = cm; ws.sm_limit = sm_limit;
+    const long long n = (long long)g.problems * g.cap;
+    window_gather_kernel<<<(unsigned)cdiv64(n, 256), 256, 0, st>>>(wboxes, wscores, wmap, d_slots + g.slot0,
+                                                                   plan.kmax, n, ws.keys, ws.boxes);
+    count_launch();
+    LUMI_CUDA_CHECK(cudaGetLastError());
+    run_sort(ws.keys, g.problems, g.cap, g.cap, nullptr, g.cap, ws.order, ws.nvalid, ws.sort_tmp, st);
+    gather_sorted_kernel<<<dim3(cdiv(g.cap, 256), g.problems), 256, 0, st>>>(ws.boxes, ws.keys, ws.order, ws.nvalid,
+                                                                              g.cap, g.cap, ws.sboxes, ws.sscores);
+    count_launch();
+    LUMI_CUDA_CHECK(cudaGetLastError());
+    run_nms(ws, g.problems, thr, cm, st);
+    window_keep_kernel<<<dim3(cdiv(cm, 128), g.problems), 128, 0, st>>>(ws.sboxes, ws.sscores, ws.keep, ws.nkeep,
+                                                                        d_lists + g.prob0, g.cap, cm, m.kboxes,
+                                                                        m.kscores, m.kkeep, m.knkeep);
+    count_launch();
+    LUMI_CUDA_CHECK(cudaGetLastError());
+  }
+  // the labels of each source, label-major, top total_max: the tail of the per-class detection chain
+  const int fcap = plan.nc * cm;
+  float* fkeys = m.final_keys;
+  int* forder = reinterpret_cast<int*>(fkeys + (size_t)plan.nsrc * fcap);
+  int* fnvalid = forder + (size_t)plan.nsrc * fcap;
+  unsigned long long* fscratch = reinterpret_cast<unsigned long long*>(
+      (reinterpret_cast<uintptr_t>(fnvalid + plan.nsrc) + 15) & ~(uintptr_t)15);
+  det_concat_kernel<<<dim3(cdiv(cm, 128), lists), 128, 0, st>>>(m.kscores, m.kkeep, m.knkeep, plan.nc, cm, cm, fkeys);
+  count_launch();
+  LUMI_CUDA_CHECK(cudaGetLastError());
+  run_sort(fkeys, plan.nsrc, fcap, fcap, nullptr, plan.total_max, forder, fnvalid, fscratch, st);
+  det_output_kernel<<<dim3(cdiv(plan.total_max, 128), plan.nsrc), 128, 0, st>>>(
+      m.kboxes, m.kscores, m.kkeep, forder, fnvalid, plan.nc, cm, cm, plan.total_max, boxes, labels, scores, counts,
+      nullptr);
   count_launch();
   LUMI_CUDA_CHECK(cudaGetLastError());
 }

@@ -44,6 +44,9 @@ SIGNATURES = {
                             [ctypes.c_void_p] * 4 + [ctypes.c_int]),
     'lumi_predict_sizes': (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 4 +
                            [ctypes.c_int]),
+    'lumi_predict_windows': (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 2 +
+                             [ctypes.c_int, ctypes.c_float] + [ctypes.c_void_p] * 4 + [ctypes.c_int]),
+    'lumi_last_window_detections': (ctypes.c_int, [ctypes.c_void_p] * 5 + [_c_i64_p]),
     'lumi_max_detections': (ctypes.c_int, [ctypes.c_void_p]),
     'lumi_set_record_output': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
     'lumi_stream': (ctypes.c_void_p, [ctypes.c_void_p]),
@@ -200,6 +203,7 @@ class Engine(object):
         self.max_batch = int(max_batch)
         self.max_detections = self._lib.lumi_max_detections(self._h)
         self._finalized = False
+        self._last_nwin = 0
 
     # ---- weights
     def weight_specs(self):
@@ -305,7 +309,40 @@ class Engine(object):
         targets = np.array(targets, np.int32).reshape(-1, 2) if len(targets) else np.zeros((0, 2), np.int32)
         return self._predict_sources('predict_sizes', images, targets, 0, 0)
 
-    def _predict_sources(self, name, images, targets, h, w):
+    def predict_windows(self, images, windows, scales, iou_threshold):
+        """Sliced prediction (``lumi_predict_windows``): windows[k] = (src, y0, x0, h, w, th, tw) is the h x w region
+        of images[src] at (y0, x0), resized to th x tw and predicted like ``predict_resize``; scales[k] = (s_y, s_x) is
+        its scale factor.  The windows' detections are mapped to source pixels and merged per source image on the GPU
+        (per-label greedy NMS at ``iou_threshold``, then the top ``max_detections`` by score).  Same image rules as
+        ``predict_resize``.  Returns numpy (boxes [n,K,4] in source pixels, scores [n,K], labels [n,K], counts [n])
+        for the n source images."""
+        windows = np.ascontiguousarray(np.asarray(windows, np.int32).reshape(-1, 7))
+        scales = np.ascontiguousarray(np.asarray(scales, np.float32).reshape(-1, 2))
+        if len(scales) != len(windows):
+            raise ValueError('predict_windows: %d windows but %d scale pairs' % (len(windows), len(scales)))
+        return self._predict_sources('predict_windows', images, None, 0, 0,
+                                     windows=(windows, scales, float(iou_threshold)))
+
+    def last_window_detections(self):
+        """The per-window detections of the last ``predict_windows`` call, in window pixels (boxes [nwin,K,4], scores
+        [nwin,K], labels [nwin,K], counts [nwin]), and its merge statistics {'workspace_bytes', 'candidates',
+        'longest_list', 'groups'}."""
+        stats = (ctypes.c_int64 * 4)()
+        nwin = self._last_nwin
+        k = self.max_detections
+        boxes = np.empty((nwin, k, 4), np.float32)
+        scores = np.empty((nwin, k), np.float32)
+        labels = np.empty((nwin, k), np.int32)
+        counts = np.empty((nwin,), np.int32)
+        with self._lock:
+            rc = self._lib.lumi_last_window_detections(self._h, *[a.ctypes.data_as(ctypes.c_void_p)
+                                                                  for a in (boxes, scores, labels, counts)], stats)
+            if rc != LUMI_OK:
+                _raise(rc, self._lib.lumi_last_error(self._h))
+        names = ('workspace_bytes', 'candidates', 'longest_list', 'groups')
+        return boxes, scores, labels, counts, dict(zip(names, (int(v) for v in stats)))
+
+    def _predict_sources(self, name, images, targets, h, w, windows=None):
         images = list(images)
         n = len(images)
         if n == 0:
@@ -352,7 +389,14 @@ class Engine(object):
                 ready.record(torch.cuda.current_stream(dev))
                 torch.cuda.ExternalStream(self.stream, device=dev).wait_event(ready)
             sz = sizes.ctypes.data_as(ctypes.c_void_p)
-            if targets is None:
+            if windows is not None:
+                wins, scl, thr = windows
+                rc = self._lib.lumi_predict_windows(self._h, ptr_arr, sz, int(f32[0]), int(on_dev[0]), n,
+                                                    wins.ctypes.data_as(ctypes.c_void_p),
+                                                    scl.ctypes.data_as(ctypes.c_void_p), len(wins), thr, *outs, 0)
+                if rc == LUMI_OK:
+                    self._last_nwin = len(wins)
+            elif targets is None:
                 rc = self._lib.lumi_predict_resize(self._h, ptr_arr, sz, int(f32[0]), int(on_dev[0]), n, h, w, *outs, 0)
             else:
                 rc = self._lib.lumi_predict_sizes(self._h, ptr_arr, sz, targets.ctypes.data_as(ctypes.c_void_p),

@@ -86,8 +86,10 @@ def draw_objects(image, objects):
     return im
 
 
-def predict_images(network, paths, only_classes=None, ignore_classes=None, save_dir=None, decode='pil', echo=print):
-    """All image files of a run as batched engine calls; returns [(path, objects or None)] in input order."""
+def predict_images(network, paths, only_classes=None, ignore_classes=None, save_dir=None, decode='pil', echo=print,
+                   tile=None):
+    """All image files of a run as batched engine calls; returns [(path, objects or None)] in input order.  ``tile``:
+    None, or the keyword arguments of ``PredictorNetwork.predict_tiled`` (sliced prediction, one call per image)."""
     images, ok_paths, results = [], [], {}
     for path in paths:
         try:
@@ -96,7 +98,11 @@ def predict_images(network, paths, only_classes=None, ignore_classes=None, save_
         except OSError as e:
             echo('Error while processing {}: {}'.format(path, e))
             results[path] = None
-    for path, image, objects in zip(ok_paths, images, network.predict_batch(images)):
+    if tile is None:
+        predictions = network.predict_batch(images)
+    else:
+        predictions = [network.predict_tiled([image], **tile)[0] for image in images]
+    for path, image, objects in zip(ok_paths, images, predictions):
         objects = filter_classes(objects, only_classes=only_classes, ignore_classes=ignore_classes)
         if save_dir:
             draw_objects(image, objects).save(os.path.join(save_dir, 'pred_{}'.format(os.path.basename(path))))
@@ -176,17 +182,31 @@ def main(argv=None):
     ap.add_argument('--ignore-class', '-K', action='append', default=None)
     ap.add_argument('--max-batch', default=8, type=int, help='images / frames per engine call')
     ap.add_argument('--pack-sizes', action='store_true', help='run images of different preprocessed sizes in one engine call, each at the top left of a shared canvas')
+    ap.add_argument('--tile', type=int, default=None,
+                    help='predict images in overlapping N x N windows at the model resolution, merged on the GPU')
+    ap.add_argument('--tile-overlap', type=float, default=0.2, help='share of a tile its neighbours overlap, in [0, 1)')
+    ap.add_argument('--no-full-image', dest='full_image', action='store_false',
+                    help='with --tile: do not also predict the whole image')
     ap.add_argument('--decode', default='pil', choices=['pil', 'nvjpeg'])
     ap.add_argument('--device', default=0, type=int)
     args = ap.parse_args(argv)
     if args.only_class and args.ignore_class:
         print('Only one of `only-class` or `ignore-class` may be specified.')
         return
+    tile = None
+    if args.tile is not None:
+        if args.tile < 1:
+            raise SystemExit('--tile must be >= 1, got {}'.format(args.tile))
+        if not 0.0 <= args.tile_overlap < 1.0:
+            raise SystemExit('--tile-overlap must be in [0, 1), got {}'.format(args.tile_overlap))
+        tile = {'tile': args.tile, 'overlap': args.tile_overlap, 'full_image': args.full_image}
     files = resolve_files(tuple(args.path_or_dir))
     if not files:
         print('No files to predict found. Accepted formats are: {}.'.format(', '.join(IMAGE_FORMATS + VIDEO_FORMATS)))
         return
     print('Found {} files to predict.'.format(len(files)), file=sys.stderr)
+    if tile is not None and any(get_file_type(f) == 'video' for f in files):
+        raise SystemExit('--tile predicts images only; video files were given')
     if not args.config_files:
         # the reference falls back to the downloadable `accurate` checkpoint (predict.py:236-241); there is no
         # network here, so a config is required
@@ -202,7 +222,7 @@ def main(argv=None):
     image_files = [f for f in files if get_file_type(f) == 'image']
     echo = lambda m: print(m, file=sys.stderr)
     for path, objects in predict_images(network, image_files, args.only_class, args.ignore_class, args.save_media_to,
-                                        args.decode, echo):
+                                        args.decode, echo, tile):
         if objects is not None:
             output.write(json.dumps({'file': path, 'objects': objects}) + '\n')
     for path in files:

@@ -125,6 +125,30 @@ def pack_groups(targets, max_batch, fill=PACK_FILL):
     return groups
 
 
+def _tile_starts(size, tile, step):
+    if size <= tile:
+        return [0]
+    return list(range(0, size - tile, step)) + [size - tile]      # the last one shifted inward, flush with the border
+
+
+def tile_grid(h, w, tile_h, tile_w, overlap):
+    """Overlapping windows covering an h x w image: [(y0, x0, wh, ww)] row by row.  Windows are tile_h x tile_w
+    (clipped to the image on a side no longer than a tile) and step by int(tile * (1 - overlap)), at least 1; the
+    last row and column are shifted inward so every window lies inside the image.  An image no larger than a tile
+    gives one whole-image window.  Windows are unique."""
+    h, w, tile_h, tile_w = int(h), int(w), int(tile_h), int(tile_w)
+    if h < 1 or w < 1:
+        raise ValueError('tile_grid: image is %d x %d, sides must be >= 1' % (h, w))
+    if tile_h < 1 or tile_w < 1:
+        raise ValueError('tile_grid: tile is %d x %d, sides must be >= 1' % (tile_h, tile_w))
+    if not 0.0 <= overlap < 1.0:
+        raise ValueError('tile_grid: overlap must be in [0, 1), got %r' % (overlap,))
+    step_h = max(1, int(tile_h * (1.0 - overlap)))
+    step_w = max(1, int(tile_w * (1.0 - overlap)))
+    wh, ww = min(tile_h, h), min(tile_w, w)
+    return [(y0, x0, wh, ww) for y0 in _tile_starts(h, tile_h, step_h) for x0 in _tile_starts(w, tile_w, step_w)]
+
+
 def load_checkpoint_weights(engine, job_dir, prefix=None):
     """The ``Saver.restore`` of ``predicting.py:51-63`` without TensorFlow: reads the latest Saver-V2 bundle under
     ``job_dir`` and returns {tf variable name: array} for exactly the variables the engine's plan uses (optimizer
@@ -234,3 +258,56 @@ class PredictorNetwork(object):
                 k = int(counts[j])
                 out[i] = (boxes[j, :k].copy(), labels[j, :k].copy(), scores[j, :k].copy(), sizes[i][2])
         return out
+
+    def merge_iou_threshold(self):
+        """The IoU threshold ``predict_tiled`` merges windows at by default: the model's class NMS threshold, or the
+        RPN's NMS threshold when Faster R-CNN runs without its RCNN."""
+        m = self.config.model
+        if m.type == 'ssd':
+            return float(m.proposals.class_nms_threshold)
+        if m.network.get('with_rcnn', False):
+            return float(m.rcnn.proposals.class_nms_threshold)
+        return float(m.rpn.proposals.nms_threshold)
+
+    def tile_windows(self, shape, tile, overlap=0.2, full_image=True):
+        """The windows ``predict_tiled`` runs for an image of ``shape``: ([(y0, x0, h, w, th, tw)], [(s_y, s_x)]),
+        the ``tile_grid`` windows with their targets and scale factors from ``target_size``, and with ``full_image``
+        the whole image last (unless the grid already is the whole image)."""
+        th_, tw_ = (tile, tile) if np.isscalar(tile) else tuple(tile)
+        h, w = int(shape[0]), int(shape[1])
+        grid = tile_grid(h, w, th_, tw_, overlap)
+        if full_image and (0, 0, h, w) not in grid:
+            grid.append((0, 0, h, w))
+        wins, scales = [], []
+        for y0, x0, wh, ww in grid:
+            nh, nw, s = target_size((wh, ww), self.config)
+            wins.append((y0, x0, wh, ww, nh, nw))
+            scales.append(tuple(s) if isinstance(s, tuple) else (s, s))
+        return wins, scales
+
+    def predict_tiled(self, images, tile, overlap=0.2, full_image=True, iou_threshold=None):
+        """Sliced prediction of large images: each image is cut into overlapping ``tile`` x ``tile`` windows
+        (``tile_grid``; ``tile`` may be an (h, w) pair), each window runs at the model's resolution
+        (``target_size``), and the windows' boxes are mapped back into the image and merged across the seams by
+        per-label NMS at ``iou_threshold`` (default ``merge_iou_threshold()``), all in one engine call
+        (``Engine.predict_windows``).  With ``full_image`` the whole image is also predicted at its own target size,
+        so objects larger than a tile are not lost at the seams.  Returns, per image, the ``predict_image`` format
+        with boxes in the image's own pixels."""
+        images = [np.asarray(im) for im in images]
+        for im in images:
+            if im.ndim != 3 or im.shape[2] != 3:
+                raise ValueError('expected an (H, W, 3) RGB image')
+        if not images:
+            return []
+        if iou_threshold is None:
+            iou_threshold = self.merge_iou_threshold()
+        windows, scales = [], []
+        for i, im in enumerate(images):
+            wins, scl = self.tile_windows(im.shape, tile, overlap, full_image)
+            windows += [(i,) + wdw for wdw in wins]
+            scales += scl
+        if any(im.dtype != np.uint8 for im in images):
+            images = [im.astype(np.float32, copy=False) for im in images]     # uint8 -> float32 is exact
+        boxes, scores, labels, counts = self.engine.predict_windows(images, windows, scales, iou_threshold)
+        return [format_predictions(boxes[i, :counts[i]], labels[i, :counts[i]], scores[i, :counts[i]], 1.0,
+                                   self.class_labels) for i in range(len(images))]
