@@ -330,6 +330,20 @@ int lumi_nms_path(int problems, int ncap, float iou_threshold);
 int lumi_op_nms_batched(const float* boxes_sorted, const int32_t* nvalid, int problems, int cap, float iou_threshold,
                         int max_out, int32_t* keep, int32_t* num_keep, void* stream);
 
+/* The cross-window merge of lumi_predict_windows on given window detections, through the code the engine runs after
+ * its window forwards: wboxes [nwin,kmax,4] (window pixels), wscores [nwin,kmax], wlabels [nwin,kmax] int32 and
+ * wcounts [nwin] int32 on DEVICE; win_src [nwin] int32 and wmap [nwin,4] float {y0, x0, s_y, s_x} on the HOST.  Per
+ * source and label the detections, mapped to source pixels, are sorted by score, suppressed by greedy NMS at
+ * iou_threshold keeping class_max, and each source's top total_max (ties: lower label) written to boxes
+ * [nsrc,total_max,4], scores [nsrc,total_max], labels [nsrc,total_max], counts [nsrc] on DEVICE.  sm_limit: the SMs the
+ * NMS mask grid is sized for (0: the device's).  merge_stats[4] (host, may be NULL): as lumi_last_window_detections.
+ * LUMI_EINVAL: a count outside [0, kmax], a counted label outside [0, nc), a source outside [0, nsrc), iou_threshold
+ * below 0 or NaN, or a size below 1. */
+int lumi_op_window_merge(const float* wboxes, const float* wscores, const int32_t* wlabels, const int32_t* wcounts,
+                         int nwin, int kmax, const int32_t* win_src, const float* wmap, int nsrc, int nc, int class_max,
+                         int total_max, float iou_threshold, int sm_limit, float* boxes, float* scores,
+                         int32_t* labels, int32_t* counts, int64_t* merge_stats, void* stream);
+
 /* The RPN proposal chain as the engine runs it on a (half-)batch: cls / box hold nimg images at the given per-image
  * strides (floats), each [na / A cells][channels]; anchor a of a cell reads its two class values at
  * cell * cls_stride + cls_off + 2a (logits = 1: softmax logits, 0: probabilities, foreground second) and its deltas at

@@ -1908,44 +1908,28 @@ int lumi_predict_windows(lumi_engine* e, const void* const* images, const int32_
   }
   e->last_nwin = nwin;
 
-  // one read of the windows' labels and counts lays out the per-(source, label) lists
-  std::vector<int> hl(nwin * K), hc(nwin);
+  // the merge reads the windows' labels and counts back once; the overflow flag comes back with them
   int ovf = 0;
-  LUMI_CUDA_CHECK(cudaMemcpyAsync(hl.data(), wlabels, nwin * K * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
-  LUMI_CUDA_CHECK(cudaMemcpyAsync(hc.data(), wcounts, nwin * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
   LUMI_CUDA_CHECK(cudaMemcpyAsync(&ovf, e->d_overflow, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
-  LUMI_CUDA_CHECK(cudaStreamSynchronize(e->stream));
-  if (ovf) {
-    LUMI_CUDA_CHECK(cudaMemset(e->d_overflow, 0, sizeof(int)));
-    throw Error(LUMI_EOVERFLOW, "an activation exceeded the fp16x2 split range (|x| > 65504); results are invalid");
-  }
   const bool rpn_only = e->type == "fasterrcnn" && !e->with_rcnn;    // one label, post_nms_top_n (= kmax) per step
   const int nc = rpn_only ? 1 : e->num_classes;
   const int class_max = rpn_only ? e->kmax : e->det.class_max;
-  WindowMergePlan plan;
-  plan_window_merge(win_src.data(), hl.data(), hc.data(), nwin, e->kmax, n, nc, class_max, e->kmax, plan);
-  const size_t scratch = window_merge_bytes(plan);
-  const size_t o_slots = round16(scratch), o_lists = o_slots + round16(plan.slots.size() * sizeof(int));
-  ensure_scratch(e, e->d_merge, e->merge_cap, o_lists + round16(plan.lists.size() * sizeof(int)));
-  int* d_slots = reinterpret_cast<int*>(e->d_merge + o_slots);
-  int* d_lists = reinterpret_cast<int*>(e->d_merge + o_lists);
-  if (!plan.slots.empty())
-    LUMI_CUDA_CHECK(cudaMemcpyAsync(d_slots, plan.slots.data(), plan.slots.size() * sizeof(int),
-                                    cudaMemcpyHostToDevice, e->stream));
-  if (!plan.lists.empty())
-    LUMI_CUDA_CHECK(cudaMemcpyAsync(d_lists, plan.lists.data(), plan.lists.size() * sizeof(int),
-                                    cudaMemcpyHostToDevice, e->stream));
   g_launch_count = 0;
   float* obox = reinterpret_cast<float*>(e->d_win + o_ob);
   float* oscore = reinterpret_cast<float*>(e->d_win + o_os);
   int* olab = reinterpret_cast<int*>(e->d_win + o_ol);
   int* ocount = reinterpret_cast<int*>(e->d_win + o_oc);
-  launch_window_merge(plan, d_slots, d_lists, wboxes, wscores, d_map, iou_threshold, e->sm_limit, e->d_merge, obox,
-                      oscore, olab, ocount, e->stream);
+  run_window_merge(wboxes, wscores, wlabels, wcounts, win_src.data(), d_map, nwin, e->kmax, n, nc, class_max, e->kmax,
+                   iou_threshold, e->sm_limit,
+                   [e](size_t bytes) { ensure_scratch(e, e->d_merge, e->merge_cap, bytes); return e->d_merge; }, obox,
+                   oscore, olab, ocount, e->merge_stats, e->stream);
+  if (ovf) {
+    LUMI_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+    LUMI_CUDA_CHECK(cudaMemset(e->d_overflow, 0, sizeof(int)));
+    throw Error(LUMI_EOVERFLOW, "an activation exceeded the fp16x2 split range (|x| > 65504); results are invalid");
+  }
   e->launches = launches + g_launch_count;
   e->graph_replays = replays;
-  e->merge_stats[0] = (int64_t)(o_lists + plan.lists.size() * sizeof(int)); e->merge_stats[1] = plan.candidates;
-  e->merge_stats[2] = plan.longest; e->merge_stats[3] = (int64_t)plan.groups.size();
   const cudaMemcpyKind kind = outputs_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
   LUMI_CUDA_CHECK(cudaMemcpyAsync(boxes, obox, n * K * 4 * sizeof(float), kind, e->stream));
   LUMI_CUDA_CHECK(cudaMemcpyAsync(scores, oscore, n * K * sizeof(float), kind, e->stream));

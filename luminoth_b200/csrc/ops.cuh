@@ -1,6 +1,7 @@
 // Launchers for the HBM-bound stages of the path (everything that is not a conv).
 #pragma once
 #include "common.cuh"
+#include <functional>
 #include <vector>
 
 namespace lumi {
@@ -173,6 +174,15 @@ size_t window_merge_bytes(const WindowMergePlan& plan);     // device scratch la
 void launch_window_merge(const WindowMergePlan& plan, const int* d_slots, const int* d_lists, const float* wboxes,
                          const float* wscores, const float4* wmap, float thr, int sm_limit, void* scratch,
                          float* boxes, float* scores, int* labels, int* counts, cudaStream_t st);
+// The whole merge after the window forwards, as lumi_predict_windows and lumi_op_window_merge run it: reads the
+// windows' labels and counts [nwin][kmax], [nwin] (device) back, synchronising st; checks them, thr and win_src [nwin]
+// (host); plans the lists; takes a device buffer of at least the bytes it asks `scratch` for; uploads the plan and
+// launches launch_window_merge.  wmap [nwin] on the device.  stats = {merge workspace bytes, candidates, longest list,
+// groups}.
+void run_window_merge(const float* wboxes, const float* wscores, const int* wlabels, const int* wcounts,
+                      const int* win_src, const float4* wmap, int nwin, int kmax, int nsrc, int nc, int class_max,
+                      int total_max, float thr, int sm_limit, const std::function<uint8_t*(size_t)>& scratch,
+                      float* boxes, float* scores, int* labels, int* counts, int64_t stats[4], cudaStream_t st);
 
 void launch_sort_desc(const float* scores, int n, int* idx_out, NmsWorkspace& ws, cudaStream_t st);
 void launch_nms_sorted(const float* boxes_sorted, int n, float thr, int max_out, NmsWorkspace& ws, int* keep,

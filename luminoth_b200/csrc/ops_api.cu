@@ -416,6 +416,29 @@ int lumi_op_nms_batched(const float* boxes_sorted, const int32_t* nvalid, int pr
   OP_END
 }
 
+int lumi_op_window_merge(const float* wboxes, const float* wscores, const int32_t* wlabels, const int32_t* wcounts,
+                         int nwin, int kmax, const int32_t* win_src, const float* wmap, int nsrc, int nc, int class_max,
+                         int total_max, float iou_threshold, int sm_limit, float* boxes, float* scores,
+                         int32_t* labels, int32_t* counts, int64_t* merge_stats, void* stream) {
+  OP_BEGIN
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  LUMI_REQUIRE(wboxes && wscores && wlabels && wcounts && win_src && wmap && boxes && scores && labels && counts,
+               "window_merge: null buffer");
+  LUMI_REQUIRE(nwin >= 1 && kmax >= 1 && sm_limit >= 0, "window_merge: need nwin, kmax >= 1 and sm_limit >= 0");
+  DevBuf map((size_t)nwin * sizeof(float4));
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(map.p, wmap, (size_t)nwin * sizeof(float4), cudaMemcpyHostToDevice, st));
+  std::unique_ptr<DevBuf> scratch;
+  int64_t stats[4];
+  run_window_merge(wboxes, wscores, wlabels, wcounts, win_src, map.as<float4>(), nwin, kmax, nsrc, nc, class_max,
+                   total_max, iou_threshold, sm_limit,
+                   [&scratch](size_t bytes) { scratch.reset(new DevBuf(bytes)); return scratch->as<uint8_t>(); },
+                   boxes, scores, labels, counts, stats, st);
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
+  if (merge_stats) for (int i = 0; i < 4; ++i) merge_stats[i] = stats[i];
+  return LUMI_OK;
+  OP_END
+}
+
 int lumi_op_rpn_proposals_batched(const float* cls, const float* box, int64_t img_stride_cls, int64_t img_stride_box,
                                   int A, const float* anchors, int nimg, int na, int cap, float im_h, float im_w,
                                   int pre_nms_top_n, int post_nms_top_n, float nms_threshold, float min_prob,

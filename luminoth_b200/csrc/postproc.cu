@@ -1158,9 +1158,13 @@ void plan_window_merge(const int* win_src, const int* labels, const int* counts,
                        int class_max, int total_max, WindowMergePlan& plan) {
   plan = WindowMergePlan();
   plan.nsrc = nsrc; plan.nc = nc; plan.class_max = class_max; plan.total_max = total_max; plan.kmax = kmax;
+  LUMI_REQUIRE(nwin >= 0 && kmax >= 1 && nsrc >= 1 && nc >= 1 && class_max >= 1 && total_max >= 1 &&
+                   (long long)nwin * kmax <= INT32_MAX,
+               "window merge: need nwin >= 0, kmax, nsrc, nc, class_max, total_max >= 1 and nwin * kmax < 2^31");
   const size_t P = (size_t)nsrc * nc;
   std::vector<long long> len(P, 0);
   for (int k = 0; k < nwin; ++k) {
+    LUMI_REQUIRE(win_src[k] >= 0 && win_src[k] < nsrc, "window merge: window source out of range");
     LUMI_REQUIRE(counts[k] >= 0 && counts[k] <= kmax, "window merge: detection count out of range");
     for (int r = 0; r < counts[k]; ++r) {
       const int lab = labels[(size_t)k * kmax + r];
@@ -1217,6 +1221,12 @@ MergeScratch carve_merge(const WindowMergePlan& pl, uint8_t* base) {
   MergeScratch m{};
   const size_t E = (size_t)std::max<long long>(pl.elems, 1), pm = (size_t)std::max(pl.pmax, 1);
   const size_t lists = (size_t)pl.nsrc * pl.nc, kept = lists * pl.class_max;
+  // the kept rows first: their place depends on (nsrc, nc, class_max) alone, so in a reused buffer whatever a list's
+  // row still holds is a kept row of an earlier call (never read: knkeep is cleared each call), not another buffer
+  m.kboxes = (float*)take(kept * 16);
+  m.kscores = (float*)take(kept * 4);
+  m.kkeep = (int*)take(kept * 4);
+  m.knkeep = (int*)take(lists * 4);
   m.ws.keys = (float*)take(E * 4);
   m.ws.boxes = (float*)take(E * 16);
   m.ws.order = (int*)take(E * 4);
@@ -1233,10 +1243,6 @@ MergeScratch carve_merge(const WindowMergePlan& pl, uint8_t* base) {
     m.ws.alive = (unsigned char*)take(E);
     m.ws.nvalid2 = (int*)take(pm * 4);
   }
-  m.kboxes = (float*)take(kept * 16);
-  m.kscores = (float*)take(kept * 4);
-  m.kkeep = (int*)take(kept * 4);
-  m.knkeep = (int*)take(lists * 4);
   m.final_keys = (float*)take(det_final_scratch_bytes(pl.nsrc, pl.nc, pl.class_max));
   m.bytes = off;
   return m;
@@ -1324,6 +1330,38 @@ void launch_window_merge(const WindowMergePlan& plan, const int* d_slots, const 
       nullptr);
   count_launch();
   LUMI_CUDA_CHECK(cudaGetLastError());
+}
+
+void run_window_merge(const float* wboxes, const float* wscores, const int* wlabels, const int* wcounts,
+                      const int* win_src, const float4* wmap, int nwin, int kmax, int nsrc, int nc, int class_max,
+                      int total_max, float thr, int sm_limit, const std::function<uint8_t*(size_t)>& scratch,
+                      float* boxes, float* scores, int* labels, int* counts, int64_t stats[4], cudaStream_t st) {
+  LUMI_REQUIRE(thr >= 0.f, "window merge: iou_threshold must be >= 0");     // NaN fails too
+  LUMI_REQUIRE(nwin >= 1 && kmax >= 1 && (long long)nwin * kmax <= INT32_MAX,
+               "window merge: need nwin, kmax >= 1 and nwin * kmax < 2^31");
+  // one read of the windows' labels and counts lays out the per-(source, label) lists
+  std::vector<int> hl((size_t)nwin * kmax), hc(nwin);
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(hl.data(), wlabels, hl.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+  LUMI_CUDA_CHECK(cudaMemcpyAsync(hc.data(), wcounts, hc.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
+  WindowMergePlan plan;
+  plan_window_merge(win_src, hl.data(), hc.data(), nwin, kmax, nsrc, nc, class_max, total_max, plan);
+  auto round16 = [](size_t b) { return (b + 15) / 16 * 16; };
+  const size_t o_slots = round16(window_merge_bytes(plan));
+  const size_t o_lists = o_slots + round16(plan.slots.size() * sizeof(int));
+  uint8_t* base = scratch(o_lists + round16(plan.lists.size() * sizeof(int)));
+  int* d_slots = reinterpret_cast<int*>(base + o_slots);
+  int* d_lists = reinterpret_cast<int*>(base + o_lists);
+  if (!plan.slots.empty())
+    LUMI_CUDA_CHECK(cudaMemcpyAsync(d_slots, plan.slots.data(), plan.slots.size() * sizeof(int),
+                                    cudaMemcpyHostToDevice, st));
+  if (!plan.lists.empty())
+    LUMI_CUDA_CHECK(cudaMemcpyAsync(d_lists, plan.lists.data(), plan.lists.size() * sizeof(int),
+                                    cudaMemcpyHostToDevice, st));
+  launch_window_merge(plan, d_slots, d_lists, wboxes, wscores, wmap, thr, sm_limit, base, boxes, scores, labels, counts,
+                      st);
+  stats[0] = (int64_t)(o_lists + plan.lists.size() * sizeof(int)); stats[1] = plan.candidates;
+  stats[2] = plan.longest; stats[3] = (int64_t)plan.groups.size();
 }
 
 // ------------------------------------------------------------------ stand-alone sort / NMS

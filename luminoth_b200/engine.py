@@ -108,7 +108,10 @@ SIGNATURES = {
     'lumi_nms_path': (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_float]),
     'lumi_op_nms_batched': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_float,
                                            ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
-    'lumi_op_rpn_proposals_batched': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64,
+    'lumi_op_window_merge': (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 2 +
+                             [ctypes.c_int] * 4 + [ctypes.c_float, ctypes.c_int] + [ctypes.c_void_p] * 4 +
+                             [_c_i64_p, ctypes.c_void_p]),
+    'lumi_op_rpn_proposals_batched':(ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64,
                                                      ctypes.c_int, ctypes.c_void_p] + [ctypes.c_int] * 3 +
                                       [ctypes.c_float] * 2 + [ctypes.c_int] * 2 + [ctypes.c_float] * 2 +
                                       [ctypes.c_int] * 8 + [ctypes.c_void_p] * 4),

@@ -158,6 +158,33 @@ def nms_batched(boxes, nvalid, thr, max_out):
     return [keep[p, :nk[p]] for p in range(P)]
 
 
+def window_merge(boxes, scores, labels, counts, win_src, wmap, nsrc, nc, class_max, total_max, thr, sm_limit=0):
+    """The cross-window merge (lumi_op_window_merge): window detections boxes [nwin, kmax, 4], scores / labels
+    [nwin, kmax], counts [nwin], win_src [nwin], wmap [nwin] = (y0, x0, s_y, s_x) -> (boxes [nsrc, total_max, 4],
+    scores, labels [nsrc, total_max], counts [nsrc], stats {'workspace_bytes', 'candidates', 'longest_list',
+    'groups'}).  Raises ValueError with the library's message on LUMI_EINVAL."""
+    lib = _lib()
+    nwin, kmax = np.asarray(scores).shape
+    bd, sd = _dev(boxes, np.float32), _dev(scores, np.float32)
+    ld, cd = _dev(labels, np.int32), _dev(counts, np.int32)
+    src = np.ascontiguousarray(win_src, np.int32)
+    m = np.ascontiguousarray(np.asarray(wmap, np.float32).reshape(nwin, 4))
+    ob = torch.zeros((nsrc, total_max, 4), dtype=torch.float32, device='cuda')
+    os_ = torch.zeros((nsrc, total_max), dtype=torch.float32, device='cuda')
+    ol = torch.zeros((nsrc, total_max), dtype=torch.int32, device='cuda')
+    oc = torch.zeros((nsrc,), dtype=torch.int32, device='cuda')
+    stats = (ctypes.c_int64 * 4)()
+    rc = lib.lumi_op_window_merge(_p(bd), _p(sd), _p(ld), _p(cd), nwin, kmax, src.ctypes.data_as(ctypes.c_void_p),
+                                  m.ctypes.data_as(ctypes.c_void_p), nsrc, nc, class_max, total_max, float(thr),
+                                  sm_limit, _p(ob), _p(os_), _p(ol), _p(oc), stats, None)
+    if rc == E.LUMI_EINVAL:
+        raise ValueError(lib.lumi_op_last_error().decode())
+    _check(rc)
+    names = ('workspace_bytes', 'candidates', 'longest_list', 'groups')
+    return (ob.cpu().numpy(), os_.cpu().numpy(), ol.cpu().numpy(), oc.cpu().numpy(),
+            dict(zip(names, (int(v) for v in stats))))
+
+
 def rpn_proposals_batched(heads, A, anchors, na, cap, im_shape, cfg, logits=True, cls_off=0, box_off=None):
     """heads [nimg, cells, hc]: the engine's fused head, class pair of anchor a at cls_off + 2a, deltas at
     box_off + 4a (default 2A).  Returns (proposals [nimg, post, 4], scores [nimg, post], counts [nimg])."""

@@ -8,7 +8,7 @@
 * End to end: two images through ``predict_tiled`` against the fp32 and float64 oracle run per window and merged by
   the same restatement, with the rule of test_gpu_photo_sizes.
 * Memory: a 4000 x 6000 photo at 600 px tiles, 80 classes and min_prob 0 completes with the merge workspace inside
-  the bound of DESIGN section 4.2.
+  the bound of DESIGN section 4.2, and its merged detections equal the restatement byte for byte.
 """
 import numpy as np
 import pytest
@@ -216,7 +216,15 @@ def test_large_photo_merge_workspace_is_bounded():
     net = PredictorNetwork(cfg, weights=wts, max_batch=8)
     res = net.predict_tiled(photo, 600)
     _, _, _, counts, stats = net.engine.last_window_detections()
+    # the merged detections themselves, against the restatement of the same call's window detections
+    wins, scales = net.tile_windows(photo[0].shape, 600)
+    windows = [(0,) + w for w in wins]
+    thr = net.merge_iou_threshold()
+    out = net.engine.predict_windows(photo, windows, scales, thr)
+    ref, _ = _merge_ref(net.engine, windows, scales, 1, 80, 100, net.engine.max_detections, thr)
     net.engine.close()
+    _assert_merge(out, ref, 'photo')
+    assert int(out[3][0]) == len(res[0])
     assert len(counts) == 9 * 13 + 1 and len(res) == 1 and len(res[0]) > 0
     assert stats['candidates'] == int(counts.sum()) > 0
     bound = merge_bound(stats, 1, 80, 100)

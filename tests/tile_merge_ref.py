@@ -25,6 +25,49 @@ def map_boxes(boxes, window):
     return out
 
 
+def list_lengths(labels, counts, win_src, nsrc, nc):
+    """Candidates per (source, label) list, indexed source * nc + label."""
+    n = np.zeros(nsrc * nc, np.int64)
+    for k, c in enumerate(counts):
+        np.add.at(n, int(win_src[k]) * nc + np.asarray(labels[k][:int(c)], np.int64), 1)
+    return n
+
+
+def plan_groups(lengths):
+    """The list groups of ``plan_window_merge``: the lists with candidates, longest first (stable on the list index),
+    taken in groups whose first list's length is the group's cap; a group takes max(1, T // cap) lists (T: all
+    candidates), or the rest.  Returns [(problems, cap)]."""
+    lengths = [int(v) for v in lengths]
+    order = sorted((p for p, v in enumerate(lengths) if v), key=lambda p: -lengths[p])
+    total = sum(lengths)
+    groups, i = [], 0
+    while i < len(order):
+        cap = lengths[order[i]]
+        take = min(len(order) - i, max(1, total // cap))
+        groups.append((take, cap))
+        i += take
+    return groups
+
+
+def nms_words(n):
+    """u64 words of one NMS mask row of an n-candidate list: ceil(n / 64) rounded up to even."""
+    return (-(-n // 64) + 1) & ~1
+
+
+def staged_fits(n):
+    """The staged scan takes an n-candidate list when its shared memory (the removed words plus two chunks of 64 mask
+    rows) fits in 200 KiB."""
+    w = nms_words(n)
+    return (w + 2 * 64 * w) * 8 <= 200 * 1024
+
+
+def nms_path(problems, cap, thr):
+    """``nms_path`` with LUMI_NMS_LAZY unset: 0 staged scan, 1 two-phase, 2 unstaged scan."""
+    if not staged_fits(cap):
+        return 2
+    return 1 if cap >= 4096 and 0 < thr < float('inf') and problems >= 3 else 0
+
+
 def merge_windows(boxes, scores, labels, counts, win_src, wmap, nsrc, nc, class_max, total_max, thr):
     """boxes [nwin][K][4], scores / labels [nwin][K], counts [nwin] (window pixels), win_src [nwin], wmap [nwin] =
     (y0, x0, s_y, s_x).  Returns per source (boxes (m, 4) float32, scores (m,) float32, labels (m,) int32)."""
