@@ -54,9 +54,33 @@ int lumi_weight_info(lumi_engine* e, int index, const char** name, int64_t* shap
 /* Fold BN, split weights into fp16 hi/lo planes, build TMA descriptors, allocate the workspace. */
 int lumi_finalize(lumi_engine* e);
 
+/* Pixel formats of the images the predict calls read (lumi_set_pixel_format).  One h x w image is
+ *   LUMI_PIXELS_RGB   [h][w][3] R, G, B, uint8 or float32 (the default)
+ *   LUMI_PIXELS_BGR   [h][w][3] B, G, R, uint8 or float32 (OpenCV's imread / VideoCapture order)
+ *   LUMI_PIXELS_NV12  uint8 Y plane [h][w], then [h/2][w/2] interleaved {U, V} pairs: h * w * 3 / 2 bytes, OpenCV's
+ *                     (3h/2, w) array (hardware video decoders, camera and ISP pipelines)
+ *   LUMI_PIXELS_I420  uint8 Y plane [h][w], then U [h/2][w/2], then V [h/2][w/2] (FFmpeg's yuv420p)
+ * NV12 and I420 need an even h and w.  They are converted to RGB with OpenCV's BT.601 limited-range integer formula
+ * (cv::cvtColor COLOR_YUV2RGB_NV12 / _I420, bit for bit): with yy = max(0, Y - 16) * 1220542 + (1 << 19),
+ * u = U - 128, v = V - 128, R = clamp((yy + 1673527 v) >> 20), G = clamp((yy - 852492 v - 409993 u) >> 20),
+ * B = clamp((yy + 2116026 u) >> 20), clamp to [0, 255].  The conversion happens per pixel in the kernels that stage
+ * the first conv's input, ahead of the resize and the mean subtraction, so a call on images in format F gives the
+ * same bytes as the call on their RGB conversions. */
+#define LUMI_PIXELS_RGB 0
+#define LUMI_PIXELS_BGR 1
+#define LUMI_PIXELS_NV12 2
+#define LUMI_PIXELS_I420 3
+
+/* The pixel format that lumi_predict, lumi_predict_f32, lumi_predict_resize, lumi_predict_sizes and
+ * lumi_predict_windows read their images in from now on (engine state; LUMI_PIXELS_RGB after lumi_create).  A call
+ * with float32 images in NV12 or I420, or with an odd NV12 / I420 size, returns LUMI_EINVAL before any device work;
+ * an unknown format returns LUMI_EINVAL here. */
+int lumi_set_pixel_format(lumi_engine* e, int format);
+
 /* Run the forward pass on n images of identical size h x w (already resized
  * like datasets/object_detection_dataset.py:71-83; lumi_predict_resize takes them at their original sizes), RGB, NHWC.
- *   images      uint8 [n,h,w,3]; host pointer (images_on_device = 0, copied H2D inside)
+ *   images      uint8 [n,h,w,3] (or n images of h x w one after the other in the engine's pixel format,
+ *               lumi_set_pixel_format); host pointer (images_on_device = 0, copied H2D inside)
  *               or device pointer (images_on_device = 1)
  *   boxes       float [n, kmax, 4]  (x1,y1,x2,y2) in resized-image pixels
  *   scores      float [n, kmax]
@@ -70,15 +94,17 @@ int lumi_predict(lumi_engine* e, const void* images, int images_on_device, int n
 
 /* Same call for float32 images [n,h,w,3]: what the reference's graph sees when the dataset preprocessing
  * resized the input (utils/image.py:38-147 produces non-integer pixel values; predicting.py:110-112 feeds them
- * as they are).  lumi_predict is the exact special case of integer-valued pixels. */
+ * as they are).  lumi_predict is the exact special case of integer-valued pixels.  The images are in the engine's
+ * pixel format, RGB or BGR (lumi_set_pixel_format). */
 int lumi_predict_f32(lumi_engine* e, const float* images, int images_on_device, int n, int h, int w,
                      float* boxes, float* scores, int32_t* labels, int32_t* counts, int outputs_on_device);
 
 /* Same call for n images of ANY sizes, resized inside the forward to one target size h x w: the TF 1.x bilinear resize
  * of utils/image.py:38-147 (lumi_op_resize_bilinear), fused into the kernels that stage the input of the first conv,
  * bit-identical to lumi_op_resize_bilinear followed by lumi_predict_f32.
- *   images      n pointers, images[i] RGB [h0_i, w0_i, 3]; all uint8 (is_f32 = 0) or all float32 (1); all host
- *               pointers (images_on_device = 0) or all device pointers (1)
+ *   images      n pointers, images[i] RGB [h0_i, w0_i, 3] (or h0_i x w0_i in the engine's pixel format,
+ *               lumi_set_pixel_format); all uint8 (is_f32 = 0) or all float32 (1); all host pointers
+ *               (images_on_device = 0) or all device pointers (1)
  *   sizes       int32 [n][2] host array {h0_i, w0_i}, each >= 1
  * h x w is the size the caller's preprocessing gives the batch (predicting.target_size); boxes come back in its
  * pixels.  The sources are packed into an engine-owned device buffer, host sources through an engine-owned pinned
@@ -97,15 +123,16 @@ int lumi_predict_resize(lumi_engine* e, const void* const* images, const int32_t
  * conv give it the zero padding it has alone, and pool1, the RPN, the ROI pool and the detections use its own size.
  * When every target is equal this is lumi_predict_resize (same kernels, same bytes).  Faster R-CNN only: SSD takes the
  * call only when every target is its fixed size.  A network with a layer whose padding would differ between an image
- * and the canvas returns LUMI_EINVAL.  The rest is as lumi_predict_resize. */
+ * and the canvas returns LUMI_EINVAL.  The rest, the engine's pixel format included, is as lumi_predict_resize. */
 int lumi_predict_sizes(lumi_engine* e, const void* const* images, const int32_t* sizes, const int32_t* targets,
                        int is_f32, int images_on_device, int n, float* boxes, float* scores, int32_t* labels,
                        int32_t* counts, int outputs_on_device);
 
 /* Sliced prediction of large images (no reference counterpart): nwin windows cut from n source images, each resized
  * and predicted like lumi_predict_resize, their detections merged per source image on the GPU.
- *   images, sizes, is_f32, images_on_device   the n sources, as lumi_predict_resize takes them; each is uploaded once
- *               per call, however many windows read it
+ *   images, sizes, is_f32, images_on_device   the n sources, as lumi_predict_resize takes them (in the engine's
+ *               pixel format); each is uploaded once per call, however many windows read it; a window of an NV12 or
+ *               I420 source may start at an odd row or column
  *   windows     int32 [nwin][7] host array {src, y0, x0, h, w, th, tw}: the h x w region of source src at (y0, x0)
  *               (inside the source), resized to th x tw with the TF 1.x bilinear resize of lumi_predict_resize
  *   scales      float [nwin][2] host array {s_y, s_x}: the window's scale_factor as predicting.target_size gives it
@@ -265,6 +292,10 @@ int lumi_pack_conv_weights(const float* w, int kdim, int cout, const float* scal
 /* tf.image.resize_images(BILINEAR) of TF 1.x (legacy kernel, align_corners=False) on one HWC image with 3 channels,
  * utils/image.py:94-97,139-142.  src: DEVICE uint8 (src_is_f32 = 0) or float32 (1) [h0,w0,3]; dst DEVICE float32 [h,w,3]. */
 int lumi_op_resize_bilinear(const void* src, int src_is_f32, int h0, int w0, float* dst, int h, int w, void* stream);
+/* One h x w image src in pixel format `format` (LUMI_PIXELS_*; uint8, or float32 with is_f32 = 1 for RGB / BGR) ->
+ * dst [h][w][3] RGB of the same dtype, through the pixel reader of the engine's input staging.  LUMI_EINVAL for an
+ * unknown format, float32 NV12 / I420 or an odd NV12 / I420 size. */
+int lumi_op_pixels_to_rgb(const void* src, int format, int is_f32, int h, int w, void* dst, void* stream);
 
 /* max_pool NHWC fp32. padding 0 VALID / 1 SAME. */
 int lumi_op_max_pool(const float* x, int n, int h, int w, int c, int k, int stride, int padding, float* y, void* stream);

@@ -1,27 +1,72 @@
 // HBM-bound elementwise / pooling / normalisation kernels (vectorised NHWC).
 #include "ops.cuh"
 #include <cstdint>
+#include <type_traits>
 
 namespace lumi {
+
+void check_pixel_format(int format, bool f32, int h, int w, const std::string& who) {
+  LUMI_REQUIRE(format >= PIX_RGB && format <= PIX_I420, who + ": unknown pixel format " + std::to_string(format) +
+                                                            " (0 RGB, 1 BGR, 2 NV12, 3 I420)");
+  if (!pix_yuv(format)) return;
+  const char* name = format == PIX_NV12 ? "NV12" : "I420";
+  LUMI_REQUIRE(!f32, who + ": " + name + " images are uint8");
+  LUMI_REQUIRE(h % 2 == 0 && w % 2 == 0, who + ": " + name + " needs an even height and width, the image is " +
+                                             std::to_string(h) + " x " + std::to_string(w));
+}
+
+// cv::cvtColor(COLOR_YUV2RGB_NV12 / _I420): BT.601 limited range in 20-bit fixed point, integer only.
+__device__ __forceinline__ void yuv_to_rgb(int Y, int U, int V, float (&v)[3]) {
+  const int uu = U - 128, vv = V - 128, yy = max(0, Y - 16) * 1220542 + (1 << 19);
+  v[0] = (float)min(max((yy + 1673527 * vv) >> 20, 0), 255);
+  v[1] = (float)min(max((yy - 852492 * vv - 409993 * uu) >> 20, 0), 255);
+  v[2] = (float)min(max((yy + 2116026 * uu) >> 20, 0), 255);
+}
+
+// The RGB value of pixel (row, col) of the image at p in format FMT: RGB / BGR rows start `pitch` pixels apart; a YUV
+// image's Y plane is plane_h rows of `pitch` bytes, its chroma planes follow (pitch and plane_h even).
+template <int FMT, typename PIX>
+__device__ __forceinline__ void load_pixel(const PIX* __restrict__ p, int pitch, int plane_h, int row, int col,
+                                           float (&v)[3]) {
+  if constexpr (FMT == PIX_RGB || FMT == PIX_BGR) {
+    const PIX* q = p + ((size_t)row * pitch + col) * 3;
+    const int r = FMT == PIX_RGB ? 0 : 2;
+    v[0] = (float)q[r]; v[1] = (float)q[1]; v[2] = (float)q[2 - r];
+  } else {
+    static_assert(sizeof(PIX) == 1, "YUV pixels are uint8");
+    const PIX* chroma = p + (size_t)plane_h * pitch;
+    const size_t half = (size_t)(row >> 1) * (pitch >> 1) + (col >> 1);
+    int u, v_;
+    if constexpr (FMT == PIX_NV12) {
+      u = chroma[2 * half]; v_ = chroma[2 * half + 1];
+    } else {
+      u = chroma[half]; v_ = chroma[(size_t)(plane_h >> 1) * (pitch >> 1) + half];
+    }
+    yuv_to_rgb(p[(size_t)row * pitch + col], u, v_, v);
+  }
+}
 
 // tf.image.resize_images(BILINEAR) of TF 1.x (legacy kernel: align_corners=False, src = dst * (in / out), no
 // half-pixel offset) -- luminoth/utils/image.py:94-97,139-142.  Same float32 operation order as the oracle
 // (tf_ops.resize_bilinear), no FMA contraction, so the result is bit-identical to it.  Pixel (y, x) of the h x w
-// output of the h0 x w0 HWC image src, hs = h0 / h and ws = w0 / w in float32; its rows start `pitch` pixels apart
-// (w0, or the width of the larger image a window lies in).
-template <typename PIX>
-__device__ __forceinline__ void bilinear_sample(const PIX* __restrict__ src, int h0, int w0, int pitch, float hs,
-                                                float ws, int y, int x, float (&v)[3]) {
+// output of the h0 x w0 image that starts at (oy, ox) of the image at src (load_pixel's pitch and plane_h), hs = h0 / h
+// and ws = w0 / w in float32.  The taps are RGB values, so a converted format resizes like its RGB image.
+template <int FMT, typename PIX>
+__device__ __forceinline__ void bilinear_sample(const PIX* __restrict__ src, int h0, int w0, int pitch, int plane_h,
+                                                int oy, int ox, float hs, float ws, int y, int x, float (&v)[3]) {
   const float fy = __fmul_rn((float)y, hs), fx = __fmul_rn((float)x, ws);
   const int y0 = (int)floorf(fy), x0 = (int)floorf(fx);
   const int y1 = min(y0 + 1, h0 - 1), x1 = min(x0 + 1, w0 - 1);
   const float yl = __fsub_rn(fy, (float)y0), xl = __fsub_rn(fx, (float)x0);
+  float tl[3], tr[3], bl[3], br[3];
+  load_pixel<FMT>(src, pitch, plane_h, oy + y0, ox + x0, tl);
+  load_pixel<FMT>(src, pitch, plane_h, oy + y0, ox + x1, tr);
+  load_pixel<FMT>(src, pitch, plane_h, oy + y1, ox + x0, bl);
+  load_pixel<FMT>(src, pitch, plane_h, oy + y1, ox + x1, br);
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    const float tl = (float)src[((size_t)y0 * pitch + x0) * 3 + c], tr = (float)src[((size_t)y0 * pitch + x1) * 3 + c];
-    const float bl = (float)src[((size_t)y1 * pitch + x0) * 3 + c], br = (float)src[((size_t)y1 * pitch + x1) * 3 + c];
-    const float top = __fadd_rn(tl, __fmul_rn(__fsub_rn(tr, tl), xl));
-    const float bot = __fadd_rn(bl, __fmul_rn(__fsub_rn(br, bl), xl));
+    const float top = __fadd_rn(tl[c], __fmul_rn(__fsub_rn(tr[c], tl[c]), xl));
+    const float bot = __fadd_rn(bl[c], __fmul_rn(__fsub_rn(br[c], bl[c]), xl));
     v[c] = __fadd_rn(top, __fmul_rn(__fsub_rn(bot, top), yl));
   }
 }
@@ -32,7 +77,7 @@ __global__ void resize_bilinear_kernel(const PIX* __restrict__ src, int h0, int 
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)h * w) return;
   float v[3];
-  bilinear_sample(src, h0, w0, w0, hs, ws, (int)(i / w), (int)(i % w), v);
+  bilinear_sample<PIX_RGB>(src, h0, w0, w0, h0, 0, 0, hs, ws, (int)(i / w), (int)(i % w), v);
   dst[i * 3] = v[0]; dst[i * 3 + 1] = v[1]; dst[i * 3 + 2] = v[2];
 }
 void launch_resize_bilinear(const void* src, bool src_f32, int h0, int w0, float* dst, int h, int w, cudaStream_t st) {
@@ -50,21 +95,21 @@ void launch_resize_bilinear(const void* src, bool src_f32, int h0, int w0, float
 }
 
 // Pixel sources of the input staging kernels: pixel (y, x) of image ni of the h x w batch the network sees.
-// DirectPixels: the batch itself, [n][h][w][3].
-template <typename PIX>
+// DirectPixels: the batch itself, n images of h x w in format FMT one after the other.
+template <typename PIX, int FMT>
 struct DirectPixels {
   const PIX* img;
   int h, w;
   __device__ __forceinline__ bool inside(int, int, int) const { return true; }
   __device__ __forceinline__ void load(int ni, int y, int x, float (&v)[3]) const {
-    const PIX* p = img + (((size_t)ni * h + y) * w + x) * 3;
-    v[0] = (float)p[0]; v[1] = (float)p[1]; v[2] = (float)p[2];
+    const size_t image = pix_yuv(FMT) ? (size_t)h * w * 3 / 2 : (size_t)h * w * 3;
+    load_pixel<FMT>(img + ni * image, w, h, y, x, v);
   }
 };
 // ResizedPixels: image ni is the source table[ni] locates in `base`, resized to its target on the fly -- the values
 // launch_resize_bilinear writes, so a fused staging is bit-identical to resize-then-stage.  PACKED: the batch is a
 // canvas, and only the pixels inside image ni's target th x tw are the image's.
-template <typename PIX, bool PACKED>
+template <typename PIX, bool PACKED, int FMT>
 struct ResizedPixels {
   const uint8_t* base;
   const ResizeSrc* table;
@@ -73,25 +118,66 @@ struct ResizedPixels {
   }
   __device__ __forceinline__ void load(int ni, int y, int x, float (&v)[3]) const {
     const ResizeSrc t = table[ni];
-    bilinear_sample(reinterpret_cast<const PIX*>(base + t.off), t.h0, t.w0, t.pitch, t.hs, t.ws, y, x, v);
+    bilinear_sample<FMT>(reinterpret_cast<const PIX*>(base + t.off), t.h0, t.w0, t.pitch, t.plane_h, t.oy, t.ox, t.hs,
+                         t.ws, y, x, v);
   }
 };
+// Calls f(format constant, pixel type) for the formats the readers are built for: RGB / BGR uint8 and float32, YUV
+// uint8.  Every caller has run check_pixel_format, which refuses the rest with its own message.
+template <typename F>
+void with_format(int format, bool f32, F&& f) {
+  using std::integral_constant;
+  LUMI_REQUIRE(format >= PIX_RGB && format <= PIX_I420 && !(f32 && pix_yuv(format)),
+               "with_format: unchecked pixel format " + std::to_string(format) + " (internal)");
+  switch (format) {
+    case PIX_RGB:
+      if (f32) f(integral_constant<int, PIX_RGB>{}, float{});
+      else f(integral_constant<int, PIX_RGB>{}, uint8_t{});
+      break;
+    case PIX_BGR:
+      if (f32) f(integral_constant<int, PIX_BGR>{}, float{});
+      else f(integral_constant<int, PIX_BGR>{}, uint8_t{});
+      break;
+    case PIX_NV12: f(integral_constant<int, PIX_NV12>{}, uint8_t{}); break;
+    case PIX_I420: f(integral_constant<int, PIX_I420>{}, uint8_t{}); break;
+  }
+}
 // Calls launch(pixels) with the source policy `src` describes.
 template <typename F>
 void with_pixels(const ImgSrc& src, int h, int w, F&& launch) {
-  if (src.table) {
-    const uint8_t* base = static_cast<const uint8_t*>(src.img);
-    if (src.packed) {
-      if (src.f32) launch(ResizedPixels<float, true>{base, src.table});
-      else launch(ResizedPixels<uint8_t, true>{base, src.table});
+  with_format(src.format, src.f32, [&](auto fmt, auto pix) {
+    using PIX = decltype(pix);
+    constexpr int FMT = decltype(fmt)::value;
+    if (src.table) {
+      const uint8_t* base = static_cast<const uint8_t*>(src.img);
+      if (src.packed) launch(ResizedPixels<PIX, true, FMT>{base, src.table});
+      else launch(ResizedPixels<PIX, false, FMT>{base, src.table});
     } else {
-      if (src.f32) launch(ResizedPixels<float, false>{base, src.table});
-      else launch(ResizedPixels<uint8_t, false>{base, src.table});
+      launch(DirectPixels<PIX, FMT>{static_cast<const PIX*>(src.img), h, w});
     }
-  } else {
-    if (src.f32) launch(DirectPixels<float>{static_cast<const float*>(src.img), h, w});
-    else launch(DirectPixels<uint8_t>{static_cast<const uint8_t*>(src.img), h, w});
-  }
+  });
+}
+
+// One image in any format -> [h][w][3] RGB of its dtype, through DirectPixels (the staging kernels' reader).
+template <typename PIX, int FMT>
+__global__ void pixels_to_rgb_kernel(DirectPixels<PIX, FMT> src, PIX* __restrict__ dst) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)src.h * src.w) return;
+  float v[3];
+  src.load(0, (int)(i / src.w), (int)(i % src.w), v);
+  dst[i * 3] = (PIX)v[0]; dst[i * 3 + 1] = (PIX)v[1]; dst[i * 3 + 2] = (PIX)v[2];     // exact: v holds PIX values
+}
+void launch_pixels_to_rgb(const void* src, int format, bool f32, int h, int w, void* dst, cudaStream_t st) {
+  check_pixel_format(format, f32, h, w, "pixels_to_rgb");
+  const size_t total = (size_t)h * w;
+  if (!total) return;
+  with_format(format, f32, [&](auto fmt, auto pix) {
+    using PIX = decltype(pix);
+    const DirectPixels<PIX, decltype(fmt)::value> px{static_cast<const PIX*>(src), h, w};
+    pixels_to_rgb_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(px, static_cast<PIX*>(dst));
+  });
+  count_launch();
+  LUMI_CUDA_CHECK(cudaGetLastError());
 }
 
 // RGB image -> (optionally mean-subtracted) fp16x2 planes, one pixel per thread.

@@ -112,6 +112,7 @@ struct lumi_engine {
   cudaStream_t stream = nullptr;
   bool finalized = false;
   int conv_impl = 1;
+  int pix_fmt = PIX_RGB;        // lumi_set_pixel_format: the format the predict calls read their images in
   int launches = 0;
   bool debug_taps = false;      // materialise intermediates that the fused path skips (roi_pool)
 
@@ -186,12 +187,13 @@ struct lumi_engine {
   int planned_n = 0, planned_h = 0, planned_w = 0;
   // CUDA graphs: one captured graph per (half-)batch forward, keyed by everything baked into its nodes
   struct GraphKey {
-    int half, n, h, w, esz, resize, packed, img_off, conv_impl, streamk, reserve, sm_limit;
+    int half, n, h, w, esz, pix_fmt, resize, packed, img_off, conv_impl, streamk, reserve, sm_limit;
     const void* records;
     bool operator<(const GraphKey& o) const {
-      return std::tie(half, n, h, w, esz, resize, packed, img_off, conv_impl, streamk, reserve, sm_limit, records) <
-             std::tie(o.half, o.n, o.h, o.w, o.esz, o.resize, o.packed, o.img_off, o.conv_impl, o.streamk, o.reserve,
-                      o.sm_limit, o.records);
+      return std::tie(half, n, h, w, esz, pix_fmt, resize, packed, img_off, conv_impl, streamk, reserve, sm_limit,
+                      records) <
+             std::tie(o.half, o.n, o.h, o.w, o.esz, o.pix_fmt, o.resize, o.packed, o.img_off, o.conv_impl, o.streamk,
+                      o.reserve, o.sm_limit, o.records);
     }
   };
   struct GraphEntry { cudaGraphExec_t exec = nullptr; int launches = 0; int seen = 0; };
@@ -764,6 +766,7 @@ struct Ctx {
   ConvWorkspace* sk = nullptr;  // stream-K scratch of this stream
   bool taps = true;             // record debug taps (first half only)
   bool img_f32 = false;         // input pixels are float32 (resized images) instead of uint8
+  int pix_fmt = PIX_RGB;        // the input pixels' format (PIX_*)
   const ResizeSrc* resize = nullptr;  // per-image source table of a fused resize (lumi_predict_resize), else null
   // A packed batch (lumi_predict_sizes): image i sits at the top left of the h x w canvas, resize[i] holds its size.
   // fstride: the feature stride of the trunk map the next run_conv reads (0 where nothing is packed: the stem, which
@@ -780,7 +783,7 @@ struct Ctx {
     return a;
   }
   float* f32(size_t count) { return (float*)arena->alloc(count * sizeof(float), dry); }
-  ImgSrc pixels(const void* images) const { return ImgSrc{images, img_f32, resize, packed}; }
+  ImgSrc pixels(const void* images) const { return ImgSrc{images, img_f32, resize, packed, pix_fmt}; }
   void tap_f32(const std::string& name, const float* p, int64_t a, int64_t b, int64_t c, int64_t d) {
     if (!taps) return;
     Tap t; t.ptr = p; t.kind = 0; t.shape[0] = a; t.shape[1] = b; t.shape[2] = c; t.shape[3] = d;
@@ -1500,8 +1503,8 @@ int lumi_finalize(lumi_engine* e) {
 static void run_forward(lumi_engine* e, Ctx& cx, int half, const void* images, int n, int h, int w, int esz) {
   const bool graphable = e->use_graphs && !e->profile && !e->debug_taps;
   if (!graphable) { forward(cx, images, n, h, w); return; }
-  lumi_engine::GraphKey key{half, n, h, w, esz, cx.resize != nullptr, cx.packed, cx.img_off, e->conv_impl,
-                            e->conv_streamk, cx.sm_reserve, e->sm_limit, e->d_records};
+  lumi_engine::GraphKey key{half, n, h, w, esz, cx.pix_fmt, cx.resize != nullptr, cx.packed, cx.img_off,
+                            e->conv_impl, e->conv_streamk, cx.sm_reserve, e->sm_limit, e->d_records};
   lumi_engine::GraphEntry& ent = e->graphs[key];
   if (ent.exec) {
     LUMI_CUDA_CHECK(cudaGraphLaunch(ent.exec, cx.st));
@@ -1541,6 +1544,7 @@ struct PredictInput {
   const int32_t* targets = nullptr;   // packed batch (lumi_predict_sizes): image i resized to targets[2i] x [2i+1]
                                       // at the top left of the h x w canvas; null: every image is h x w
   int esz = 1;                  // bytes per channel value: 1 uint8, 4 float32
+  int format = PIX_RGB;         // pixel format of the images (PIX_*)
   int on_device = 0;
   const ResizeSrc* rows = nullptr;    // windows (lumi_predict_windows): the n table rows of this chunk, in the pinned
                                       // buffer; the sources are already in e->d_src
@@ -1571,7 +1575,8 @@ static size_t round16(size_t b) { return (b + 15) / 16 * 16; }
 static void stage_resize(lumi_engine* e, const PredictInput& in, int n, int nA, int h, int w,
                          std::vector<Upload> (&up)[2]) {
   std::vector<size_t> off(n + 1, 0);
-  for (int i = 0; i < n; ++i) off[i + 1] = off[i] + round16((size_t)in.sizes[2 * i] * in.sizes[2 * i + 1] * 3 * in.esz);
+  for (int i = 0; i < n; ++i)
+    off[i + 1] = off[i] + round16(pixel_bytes(in.format, in.sizes[2 * i], in.sizes[2 * i + 1], in.esz));
   ensure_device_buffer(e, e->d_src, e->src_cap, off[n]);
   if (!e->d_resize_tab) {
     LUMI_CUDA_CHECK(cudaMalloc(&e->d_resize_tab, (size_t)e->max_batch * sizeof(ResizeSrc)));
@@ -1591,7 +1596,8 @@ static void stage_resize(lumi_engine* e, const PredictInput& in, int n, int nA, 
   for (int i = 0; i < n; ++i) {
     const int h0 = in.sizes[2 * i], w0 = in.sizes[2 * i + 1];
     const int th = in.targets ? in.targets[2 * i] : h, tw = in.targets ? in.targets[2 * i + 1] : w;
-    rows[i] = ResizeSrc{(long long)off[i], h0, w0, (float)h0 / (float)th, (float)w0 / (float)tw, th, tw, w0};  // as launch_resize_bilinear
+    rows[i] = ResizeSrc{(long long)off[i], h0, w0, (float)h0 / (float)th, (float)w0 / (float)tw, th, tw, w0,  // as launch_resize_bilinear
+                        0, 0, h0};
   }
   const int bounds[3] = {0, nA, n};
   for (int k = 0; k < 2; ++k) {
@@ -1599,7 +1605,7 @@ static void stage_resize(lumi_engine* e, const PredictInput& in, int n, int nA, 
     if (b == t) continue;
     up[k].push_back({e->d_resize_tab + b, rows + b, (size_t)(t - b) * sizeof(ResizeSrc), cudaMemcpyHostToDevice});
     for (int i = b; i < t; ++i) {
-      const size_t bytes = (size_t)in.sizes[2 * i] * in.sizes[2 * i + 1] * 3 * in.esz;
+      const size_t bytes = pixel_bytes(in.format, in.sizes[2 * i], in.sizes[2 * i + 1], in.esz);
       if (in.on_device) up[k].push_back({e->d_src + off[i], in.sources[i], bytes, cudaMemcpyDeviceToDevice});
       else up[k].push_back({e->d_src + off[i], host_src + off[i], bytes, cudaMemcpyHostToDevice, in.sources[i]});
     }
@@ -1622,6 +1628,7 @@ static void predict_run(lumi_engine* e, const PredictInput& in, int n, int h, in
   LUMI_REQUIRE((in.images || resize) && boxes && scores && labels && counts, "lumi_predict: null buffer");
   LUMI_REQUIRE(n > 0 && n <= e->max_batch, "lumi_predict: batch size exceeds max_batch");
   LUMI_REQUIRE(h > 0 && w > 0, "lumi_predict: empty image");
+  if (!resize) check_pixel_format(in.format, in.esz == 4, h, w, "lumi_predict");
   if (resize && !in.rows) {
     LUMI_REQUIRE(in.sizes, "lumi_predict_resize: null sizes");
     for (int i = 0; i < n; ++i) {
@@ -1630,6 +1637,7 @@ static void predict_run(lumi_engine* e, const PredictInput& in, int n, int h, in
                                            std::to_string(h0) + " x " + std::to_string(w0) + ", sizes must be >= 1");
       LUMI_REQUIRE((long long)h0 * w0 < (1LL << 30), "lumi_predict_resize: source image too large");
       LUMI_REQUIRE(in.sources[i], "lumi_predict_resize: null source image " + std::to_string(i));
+      check_pixel_format(in.format, in.esz == 4, h0, w0, "lumi_predict_resize: source image " + std::to_string(i));
     }
   }
   LUMI_CUDA_CHECK(cudaSetDevice(e->device));
@@ -1659,8 +1667,8 @@ static void predict_run(lumi_engine* e, const PredictInput& in, int n, int h, in
     else stage_resize(e, in, n, nA, h, w, up);
     img_a = img_b = e->d_src;                      // the table rows hold the offsets
   } else {
-    const size_t img_bytes = (size_t)n * h * w * 3 * in.esz;
-    const size_t bytes_a = (size_t)nA * h * w * 3 * in.esz;
+    const size_t img_bytes = n * pixel_bytes(in.format, h, w, in.esz);
+    const size_t bytes_a = nA * pixel_bytes(in.format, h, w, in.esz);
     // graphs read their pixels from the engine's own staging buffer (a caller's device pointer changes per call)
     const bool graphs_on = e->use_graphs && !e->profile && !e->debug_taps;
     const uint8_t* dimg = static_cast<const uint8_t*>(in.images);
@@ -1685,6 +1693,7 @@ static void predict_run(lumi_engine* e, const PredictInput& in, int n, int h, in
   if (e->type == "fasterrcnn") ensure_frcnn_anchors(e, h, w, e->stream);
   Ctx cx = make_ctx(e, false, 0);
   cx.img_f32 = in.esz == 4;
+  cx.pix_fmt = in.format;
   cx.resize = resize ? e->d_resize_tab : nullptr;
   cx.packed = packed;
   cx.sm_reserve = piped ? CONV_PIPELINE_SM_RESERVE : 0;
@@ -1694,6 +1703,7 @@ static void predict_run(lumi_engine* e, const PredictInput& in, int n, int h, in
     Ctx cb = make_ctx(e, false, 1);
     cb.img_off = nA;
     cb.img_f32 = cx.img_f32;
+    cb.pix_fmt = cx.pix_fmt;
     cb.resize = resize ? e->d_resize_tab + nA : nullptr;
     cb.packed = packed;
     cb.sm_reserve = cx.sm_reserve;
@@ -1739,14 +1749,14 @@ static int predict_impl(lumi_engine* e, const PredictInput& in, int n, int h, in
 int lumi_predict(lumi_engine* e, const void* images, int images_on_device, int n, int h, int w, float* boxes,
                  float* scores, int* labels, int* counts, int outputs_on_device) {
   PredictInput in;
-  in.images = images; in.esz = 1; in.on_device = images_on_device;
+  in.images = images; in.esz = 1; in.format = e ? e->pix_fmt : PIX_RGB; in.on_device = images_on_device;
   return predict_impl(e, in, n, h, w, boxes, scores, labels, counts, outputs_on_device);
 }
 
 int lumi_predict_f32(lumi_engine* e, const float* images, int images_on_device, int n, int h, int w, float* boxes,
                      float* scores, int* labels, int* counts, int outputs_on_device) {
   PredictInput in;
-  in.images = images; in.esz = 4; in.on_device = images_on_device;
+  in.images = images; in.esz = 4; in.format = e ? e->pix_fmt : PIX_RGB; in.on_device = images_on_device;
   return predict_impl(e, in, n, h, w, boxes, scores, labels, counts, outputs_on_device);
 }
 
@@ -1756,7 +1766,8 @@ int lumi_predict_resize(lumi_engine* e, const void* const* images, const int32_t
   if (!e) return LUMI_EINVAL;
   if (!images) return fail(e, LUMI_EINVAL, "lumi_predict_resize: null images");
   PredictInput in;
-  in.sources = images; in.sizes = sizes; in.esz = is_f32 ? 4 : 1; in.on_device = images_on_device;
+  in.sources = images; in.sizes = sizes; in.esz = is_f32 ? 4 : 1; in.format = e->pix_fmt;
+  in.on_device = images_on_device;
   return predict_impl(e, in, n, h, w, boxes, scores, labels, counts, outputs_on_device);
 }
 
@@ -1778,7 +1789,8 @@ int lumi_predict_sizes(lumi_engine* e, const void* const* images, const int32_t*
     hc = std::max(hc, th); wc = std::max(wc, tw);
   }
   PredictInput in;
-  in.sources = images; in.sizes = sizes; in.esz = is_f32 ? 4 : 1; in.on_device = images_on_device;
+  in.sources = images; in.sizes = sizes; in.esz = is_f32 ? 4 : 1; in.format = e->pix_fmt;
+  in.on_device = images_on_device;
   if (!uniform) {                                  // one h x w target is lumi_predict_resize itself
     if (e->type != "fasterrcnn")
       return fail(e, LUMI_EINVAL, "lumi_predict_sizes: SSD runs at its fixed size only");
@@ -1812,7 +1824,7 @@ int lumi_predict_windows(lumi_engine* e, const void* const* images, const int32_
   LUMI_REQUIRE(!e->d_records, "lumi_predict_windows: a record output is set (lumi_set_record_output); tiled "
                               "prediction writes no records");
   LUMI_REQUIRE(iou_threshold >= 0.f, "lumi_predict_windows: iou_threshold must be >= 0");
-  const int esz = is_f32 ? 4 : 1;
+  const int esz = is_f32 ? 4 : 1, fmt = e->pix_fmt;
   std::vector<size_t> off(n + 1, 0);
   for (int i = 0; i < n; ++i) {
     const int h0 = sizes[2 * i], w0 = sizes[2 * i + 1];
@@ -1820,7 +1832,8 @@ int lumi_predict_windows(lumi_engine* e, const void* const* images, const int32_
                                          std::to_string(h0) + " x " + std::to_string(w0) + ", sizes must be >= 1");
     LUMI_REQUIRE((long long)h0 * w0 < (1LL << 30), "lumi_predict_windows: source image too large");
     LUMI_REQUIRE(images[i], "lumi_predict_windows: null source image " + std::to_string(i));
-    off[i + 1] = off[i] + round16((size_t)h0 * w0 * 3 * esz);
+    check_pixel_format(fmt, is_f32 != 0, h0, w0, "lumi_predict_windows: source image " + std::to_string(i));
+    off[i + 1] = off[i] + round16(pixel_bytes(fmt, h0, w0, esz));
   }
   for (int k = 0; k < nwin; ++k) {
     const int32_t* wk = windows + 7 * k;
@@ -1858,15 +1871,18 @@ int lumi_predict_windows(lumi_engine* e, const void* const* images, const int32_
   std::vector<int> win_src(nwin);
   for (int k = 0; k < nwin; ++k) {
     const int32_t* wk = windows + 7 * k;
-    const int W = sizes[2 * wk[0] + 1];
-    const size_t first = off[wk[0]] + ((size_t)wk[1] * W + wk[2]) * 3 * esz;    // the window's top-left pixel
-    rows[k] = ResizeSrc{(long long)first, wk[3], wk[4], (float)wk[3] / (float)wk[5], (float)wk[4] / (float)wk[6],
-                        wk[5], wk[6], W};
+    const int H = sizes[2 * wk[0]], W = sizes[2 * wk[0] + 1];
+    const float hs = (float)wk[3] / (float)wk[5], ws = (float)wk[4] / (float)wk[6];
+    if (pix_yuv(fmt))           // the source's first byte and the window's origin: chroma rows are shared by row pairs
+      rows[k] = ResizeSrc{(long long)off[wk[0]], wk[3], wk[4], hs, ws, wk[5], wk[6], W, wk[1], wk[2], H};
+    else                        // the window's top-left pixel
+      rows[k] = ResizeSrc{(long long)(off[wk[0]] + ((size_t)wk[1] * W + wk[2]) * 3 * esz), wk[3], wk[4], hs, ws, wk[5],
+                          wk[6], W, 0, 0, H};
     wmap[k] = make_float4((float)wk[1], (float)wk[2], scales[2 * k], scales[2 * k + 1]);
     win_src[k] = wk[0];
   }
   for (int i = 0; i < n; ++i) {
-    const size_t bytes = (size_t)sizes[2 * i] * sizes[2 * i + 1] * 3 * esz;
+    const size_t bytes = pixel_bytes(fmt, sizes[2 * i], sizes[2 * i + 1], esz);
     if (images_on_device) {
       LUMI_CUDA_CHECK(cudaMemcpyAsync(e->d_src + off[i], images[i], bytes, cudaMemcpyDeviceToDevice, e->stream));
     } else {
@@ -1893,7 +1909,7 @@ int lumi_predict_windows(lumi_engine* e, const void* const* images, const int32_
 
   // each maximal run of equal targets as forwards of up to max_batch windows, the lumi_predict_resize path
   PredictInput in;
-  in.sources = images; in.esz = esz; in.on_device = images_on_device;
+  in.sources = images; in.esz = esz; in.format = fmt; in.on_device = images_on_device;
   int launches = 0, replays = 0;
   for (int a = 0; a < nwin;) {
     int b = a + 1;
@@ -2005,6 +2021,15 @@ int lumi_set_debug_taps(lumi_engine* e, int enable) {
   if (!e) return LUMI_EINVAL;
   e->debug_taps = enable != 0;
   e->planned_n = 0;          // the plan (arena layout) changes
+  return LUMI_OK;
+}
+
+int lumi_set_pixel_format(lumi_engine* e, int format) {
+  if (!e) return LUMI_EINVAL;
+  if (format < PIX_RGB || format > PIX_I420)
+    return fail(e, LUMI_EINVAL, "lumi_set_pixel_format: unknown pixel format " + std::to_string(format) +
+                                    " (0 RGB, 1 BGR, 2 NV12, 3 I420)");
+  e->pix_fmt = format;
   return LUMI_OK;
 }
 

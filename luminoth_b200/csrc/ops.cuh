@@ -7,28 +7,49 @@
 namespace lumi {
 
 // ---- format conversion / preprocessing (elementwise.cu)
-// One source image of a fused resize: its first byte at `off` in the source buffer, h0 x w0 RGB pixels, resized to its
+// Pixel formats of the images a predict call reads (LUMI_PIXELS_* of the C ABI).  RGB and BGR: [h][w][3] uint8 or
+// float32.  NV12: the Y plane [h][w], then [h/2][w/2] interleaved U, V pairs.  I420: Y [h][w], U [h/2][w/2], V
+// [h/2][w/2].  YUV is uint8 with even h and w, converted with OpenCV's BT.601 limited-range integer formula.
+enum { PIX_RGB = 0, PIX_BGR = 1, PIX_NV12 = 2, PIX_I420 = 3 };
+__host__ __device__ constexpr bool pix_yuv(int format) { return format == PIX_NV12 || format == PIX_I420; }
+// Bytes of one h x w image in `format` (esz: bytes per channel value of RGB / BGR).
+inline size_t pixel_bytes(int format, int h, int w, int esz) {
+  return pix_yuv(format) ? (size_t)h * w * 3 / 2 : (size_t)h * w * 3 * esz;
+}
+// Throws LUMI_EINVAL unless an h x w image (float32 when f32) can be read in `format`; `who` prefixes the message.
+void check_pixel_format(int format, bool f32, int h, int w, const std::string& who);
+
+// One source image of a fused resize: its first byte at `off` in the source buffer, h0 x w0 pixels, resized to its
 // target th x tw with the scale factors hs = (float)h0 / th, ws = (float)w0 / tw (as launch_resize_bilinear computes
 // them).  A uniform batch has th x tw = the batch's h x w; a packed batch (lumi_predict_sizes) places each image at the
 // top left of its h x w canvas, and the per-image kernels below read th x tw from this one table.  pitch: pixels
-// between the starts of two source rows -- w0 for a whole image; a window of a larger source (lumi_predict_windows)
-// has `off` at its top-left pixel, h0 x w0 its own size and pitch the source's width.
+// between the starts of two source rows -- w0 for a whole image.  A window of a larger source (lumi_predict_windows) is
+// h0 x w0 with pitch the source's width; RGB / BGR windows have `off` at their top-left pixel and oy = ox = 0.  4:2:0
+// chroma rows cannot be addressed from a window's odd origin, so YUV windows keep `off` at the source's first byte and
+// give the window's origin (oy, ox) in the source; plane_h is the source's height, the rows of its Y plane, which its
+// chroma planes follow.
 struct ResizeSrc {
   long long off;
   int h0, w0;
   float hs, ws;
   int th, tw;
   int pitch;
+  int oy, ox, plane_h;
 };
-// The pixels the input staging kernels read: with table == nullptr, img is the batch itself [n][h][w][3]; otherwise
-// image i of the batch is table[i]'s source in img, bilinearly resized on the fly.  f32: float32 pixels, else uint8.
-// packed: pixels outside image i's th x tw are the zero padding (0 after the mean subtraction).
+// The pixels the input staging kernels read: with table == nullptr, img is the batch itself, n images of h x w in
+// `format` one after the other; otherwise image i of the batch is table[i]'s source in img, bilinearly resized on the
+// fly.  f32: float32 pixels, else uint8.  packed: pixels outside image i's th x tw are the zero padding (0 after the
+// mean subtraction).
 struct ImgSrc {
   const void* img;
   bool f32;
   const ResizeSrc* table;
   bool packed;
+  int format = PIX_RGB;
 };
+// Stand-alone conversion (lumi_op_pixels_to_rgb): the h x w image src in `format` as [h][w][3] RGB of its dtype, read
+// through the staging kernels' pixel reader.
+void launch_pixels_to_rgb(const void* src, int format, bool f32, int h, int w, void* dst, cudaStream_t st);
 void launch_u8_to_act(ImgSrc src, Act out /*(n,h,w,3)*/, const float* means /*3 or nullptr*/, cudaStream_t st);
 void launch_f32_to_act(const float* x, Act out, cudaStream_t st);
 // x2: (n, Ho+3, Wo+3, 16) space-to-depth staging of the 7x7/2 stem input (see elementwise.cu)

@@ -249,6 +249,16 @@ int lumi_op_resize_bilinear(const void* src, int src_is_f32, int h0, int w0, flo
   OP_END
 }
 
+int lumi_op_pixels_to_rgb(const void* src, int format, int is_f32, int h, int w, void* dst, void* stream) {
+  OP_BEGIN
+  LUMI_REQUIRE(src && dst && h > 0 && w > 0, "pixels_to_rgb: bad arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  launch_pixels_to_rgb(src, format, is_f32 != 0, h, w, dst, st);
+  LUMI_CUDA_CHECK(cudaStreamSynchronize(st));
+  return LUMI_OK;
+  OP_END
+}
+
 int lumi_op_max_pool(const float* x, int n, int h, int w, int c, int k, int stride, int padding, float* y, void* stream) {
   OP_BEGIN
   cudaStream_t st = static_cast<cudaStream_t>(stream);

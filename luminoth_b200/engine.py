@@ -35,6 +35,7 @@ SIGNATURES = {
     'lumi_weight_info': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_char_p), _c_i64_p,
                                         _c_int_p]),
     'lumi_finalize': (ctypes.c_int, [ctypes.c_void_p]),
+    'lumi_set_pixel_format': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
     'lumi_predict': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                     ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                     ctypes.c_int]),
@@ -76,6 +77,7 @@ SIGNATURES = {
                                                                       ctypes.c_void_p]),
     'lumi_op_resize_bilinear': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+    'lumi_op_pixels_to_rgb': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] * 2),
     'lumi_op_conv2d_preact': (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] +
                               [ctypes.c_int] * 6 + [ctypes.c_void_p] * 3 + [ctypes.c_int] * 2 +
                               [ctypes.c_void_p] * 4 + [_c_int_p, _c_int_p, ctypes.c_void_p]),
@@ -164,6 +166,37 @@ def decode_jpeg(data, device=0):
     return out
 
 
+# LUMI_PIXELS_* of include/luminoth_b200.h
+PIXEL_FORMATS = {'rgb': 0, 'bgr': 1, 'nv12': 2, 'i420': 3}
+
+
+def pixel_format_code(pixel_format):
+    """The LUMI_PIXELS_* code of 'rgb', 'bgr', 'nv12' or 'i420'; ValueError for any other name."""
+    try:
+        return PIXEL_FORMATS[pixel_format]
+    except (KeyError, TypeError):
+        raise ValueError("pixel_format must be one of 'rgb', 'bgr', 'nv12', 'i420', got %r" % (pixel_format,))
+
+
+def pixel_size(shape, pixel_format='rgb', uint8=True):
+    """The (h, w) pixel size of one image array of ``shape`` in ``pixel_format``: RGB and BGR images are (h, w, 3);
+    NV12 and I420 images are the 2-D (3h/2, w) uint8 arrays OpenCV and video decoders give (Y plane, then chroma),
+    with h and w even.  ValueError for any other shape, and for an NV12 or I420 image that is not uint8."""
+    code = pixel_format_code(pixel_format)
+    shape = tuple(int(d) for d in shape)
+    name = pixel_format.upper()
+    if code < 2:
+        if len(shape) != 3 or shape[2] != 3:
+            raise ValueError('images must be (h, w, 3) %s, got shape %s' % (name, shape))
+        return shape[0], shape[1]
+    if not uint8:
+        raise ValueError('%s images must be uint8' % name)
+    if len(shape) != 2 or shape[0] % 3 or shape[1] % 2:
+        raise ValueError('%s images must be (3h/2, w) uint8 arrays with an even height h and width w, got shape %s'
+                         % (name, shape))
+    return shape[0] * 2 // 3, shape[1]
+
+
 def _raise(code, msg):
     msg = msg.decode() if isinstance(msg, bytes) else str(msg)
     if code in (LUMI_EINVAL, LUMI_ENOWEIGHT):
@@ -207,6 +240,7 @@ class Engine(object):
         self.max_detections = self._lib.lumi_max_detections(self._h)
         self._finalized = False
         self._last_nwin = 0
+        self._pixel_format = PIXEL_FORMATS['rgb']
 
     # ---- weights
     def weight_specs(self):
@@ -258,27 +292,43 @@ class Engine(object):
         if rc != LUMI_OK:
             _raise(rc, self._lib.lumi_last_error(self._h))
 
+    def _use_pixel_format(self, code):
+        """Sets the engine's pixel format to ``code`` when it differs (the caller holds the lock)."""
+        if code != self._pixel_format:
+            rc = self._lib.lumi_set_pixel_format(self._h, code)
+            if rc != LUMI_OK:
+                _raise(rc, self._lib.lumi_last_error(self._h))
+            self._pixel_format = code
+
     # ---- forward
-    def predict_raw(self, images):
+    def predict_raw(self, images, pixel_format='rgb'):
         """images: [n,h,w,3] uint8 (``lumi_predict``) or float32 (``lumi_predict_f32``: resized images keep their
         non-integer pixel values, like the reference's feed); numpy array -> host path, H2D inside the call;
-        CUDA torch tensor -> device path.  Returns numpy
+        CUDA torch tensor -> device path.  ``pixel_format`` 'bgr' reads [n,h,w,3] BGR images, 'nv12' and 'i420'
+        [n,3h/2,w] uint8 frames (``pixel_size``); the results equal those of their RGB conversions.  Returns numpy
         (boxes [n,K,4], scores [n,K], labels [n,K], counts [n])."""
+        code = pixel_format_code(pixel_format)
         on_dev = False
         if isinstance(images, np.ndarray):
             is_f32 = images.dtype != np.uint8
-            imgs = np.ascontiguousarray(images, dtype=np.float32 if is_f32 else np.uint8)
-            n, h, w, c = imgs.shape
-            ptr = imgs.ctypes.data
         else:                       # torch tensor
             import torch
             assert images.dtype in (torch.uint8, torch.float32) and images.is_contiguous()
             is_f32 = images.dtype == torch.float32
-            n, h, w, c = images.shape
             on_dev = images.is_cuda
+        shape = tuple(images.shape)
+        if code == 0:
+            n, h, w, c = shape
+            if c != 3:
+                raise ValueError('images must be [n,h,w,3] RGB')
+        else:                       # refuses float32 and odd-sized YUV before any conversion
+            n = shape[0]
+            h, w = pixel_size(shape[1:], pixel_format, not is_f32)
+        if isinstance(images, np.ndarray):
+            imgs = np.ascontiguousarray(images, dtype=np.float32 if is_f32 else np.uint8)
+            ptr = imgs.ctypes.data
+        else:
             ptr = images.data_ptr()
-        if c != 3:
-            raise ValueError('images must be [n,h,w,3] RGB')
         k = self.max_detections
         boxes = np.empty((n, k, 4), np.float32)
         scores = np.empty((n, k), np.float32)
@@ -286,6 +336,7 @@ class Engine(object):
         counts = np.empty((n,), np.int32)
         fn = self._lib.lumi_predict_f32 if is_f32 else self._lib.lumi_predict
         with self._lock:
+            self._use_pixel_format(code)
             rc = fn(self._h, ctypes.c_void_p(ptr), int(on_dev), n, h, w,
                     boxes.ctypes.data_as(ctypes.c_void_p), scores.ctypes.data_as(ctypes.c_void_p),
                     labels.ctypes.data_as(ctypes.c_void_p), counts.ctypes.data_as(ctypes.c_void_p), 0)
@@ -293,38 +344,40 @@ class Engine(object):
                 _raise(rc, self._lib.lumi_last_error(self._h))
         return boxes, scores, labels, counts
 
-    def predict_resize(self, images, h, w):
+    def predict_resize(self, images, h, w, pixel_format='rgb'):
         """Like ``predict_raw`` for a list of (h0, w0, 3) images of any sizes, resized to h x w inside the forward
         (``lumi_predict_resize``): bit-identical to ``lumi_op_resize_bilinear`` per image followed by ``predict_raw``
         on the float32 batch.  The images are all numpy arrays (host path) or all CUDA torch tensors (device path),
         and all uint8 or all float32 (numpy arrays of other dtypes are read as float32).  CUDA tensors must be on the
         engine's device and may be non-contiguous (they are copied); the engine reads them after the work queued so far
-        on torch's current stream of that device, which is what wrote them.  Returns numpy (boxes [n,K,4] in h x w
-        pixels, scores [n,K], labels [n,K], counts [n])."""
-        return self._predict_sources('predict_resize', images, None, int(h), int(w))
+        on torch's current stream of that device, which is what wrote them.  ``pixel_format`` as in ``predict_raw``:
+        'bgr' images are (h0, w0, 3), 'nv12' and 'i420' images (3 h0 / 2, w0) uint8.  Returns numpy (boxes [n,K,4] in
+        h x w pixels, scores [n,K], labels [n,K], counts [n])."""
+        return self._predict_sources('predict_resize', images, None, int(h), int(w), pixel_format=pixel_format)
 
-    def predict_sizes(self, images, targets):
+    def predict_sizes(self, images, targets, pixel_format='rgb'):
         """``predict_resize`` with one target size per image (``lumi_predict_sizes``): images[i] is resized to
         targets[i] = (h_i, w_i), every image runs in one forward at the top left of a canvas of the largest target
         height and width, and its results equal those of ``predict_resize([images[i]], h_i, w_i)``.  Same argument
         rules as ``predict_resize``; boxes come back in each image's own target pixels.  Faster R-CNN only (SSD takes
         only its fixed size)."""
         targets = np.array(targets, np.int32).reshape(-1, 2) if len(targets) else np.zeros((0, 2), np.int32)
-        return self._predict_sources('predict_sizes', images, targets, 0, 0)
+        return self._predict_sources('predict_sizes', images, targets, 0, 0, pixel_format=pixel_format)
 
-    def predict_windows(self, images, windows, scales, iou_threshold):
+    def predict_windows(self, images, windows, scales, iou_threshold, pixel_format='rgb'):
         """Sliced prediction (``lumi_predict_windows``): windows[k] = (src, y0, x0, h, w, th, tw) is the h x w region
         of images[src] at (y0, x0), resized to th x tw and predicted like ``predict_resize``; scales[k] = (s_y, s_x) is
         its scale factor.  The windows' detections are mapped to source pixels and merged per source image on the GPU
         (per-label greedy NMS at ``iou_threshold``, then the top ``max_detections`` by score).  Same image rules as
-        ``predict_resize``.  Returns numpy (boxes [n,K,4] in source pixels, scores [n,K], labels [n,K], counts [n])
+        ``predict_resize``, ``pixel_format`` included (windows are in pixels, and may start at odd rows and columns of
+        NV12 and I420 sources).  Returns numpy (boxes [n,K,4] in source pixels, scores [n,K], labels [n,K], counts [n])
         for the n source images."""
         windows = np.ascontiguousarray(np.asarray(windows, np.int32).reshape(-1, 7))
         scales = np.ascontiguousarray(np.asarray(scales, np.float32).reshape(-1, 2))
         if len(scales) != len(windows):
             raise ValueError('predict_windows: %d windows but %d scale pairs' % (len(windows), len(scales)))
         return self._predict_sources('predict_windows', images, None, 0, 0,
-                                     windows=(windows, scales, float(iou_threshold)))
+                                     windows=(windows, scales, float(iou_threshold)), pixel_format=pixel_format)
 
     def last_window_detections(self):
         """The per-window detections of the last ``predict_windows`` call, in window pixels (boxes [nwin,K,4], scores
@@ -345,7 +398,8 @@ class Engine(object):
         names = ('workspace_bytes', 'candidates', 'longest_list', 'groups')
         return boxes, scores, labels, counts, dict(zip(names, (int(v) for v in stats)))
 
-    def _predict_sources(self, name, images, targets, h, w, windows=None):
+    def _predict_sources(self, name, images, targets, h, w, windows=None, pixel_format='rgb'):
+        code = pixel_format_code(pixel_format)
         images = list(images)
         n = len(images)
         if n == 0:
@@ -371,11 +425,17 @@ class Engine(object):
             ptrs = [s.ctypes.data for s in srcs]
         if any(f32) != all(f32):
             raise ValueError('%s: the images of one call must share a dtype (uint8 or float32)' % name)
-        for s in srcs:
-            if len(s.shape) != 3 or s.shape[2] != 3:
-                raise ValueError('%s: images must be (h0, w0, 3) RGB' % name)
+        if code == 0:
+            for s in srcs:
+                if len(s.shape) != 3 or s.shape[2] != 3:
+                    raise ValueError('%s: images must be (h0, w0, 3) RGB' % name)
+            sizes = np.array([s.shape[:2] for s in srcs], np.int32)
+        else:
+            try:
+                sizes = np.array([pixel_size(s.shape, pixel_format, not f) for s, f in zip(srcs, f32)], np.int32)
+            except ValueError as ex:
+                raise ValueError('%s: %s' % (name, ex))
         ptr_arr = (ctypes.c_void_p * n)(*ptrs)
-        sizes = np.array([s.shape[:2] for s in srcs], np.int32)
         k = self.max_detections
         boxes = np.empty((n, k, 4), np.float32)
         scores = np.empty((n, k), np.float32)
@@ -383,6 +443,7 @@ class Engine(object):
         counts = np.empty((n,), np.int32)
         outs = [a.ctypes.data_as(ctypes.c_void_p) for a in (boxes, scores, labels, counts)]
         with self._lock:
+            self._use_pixel_format(code)
             if on_dev[0]:
                 # the engine's streams do not follow torch's: make its stream wait for the work torch has queued on
                 # the device's current stream (the caller's writes of the images, the copies of .contiguous()); the
@@ -412,6 +473,7 @@ class Engine(object):
         """Fully asynchronous device-resident call (CUDA torch tensors in and out)."""
         n, h, w, _ = images.shape
         with self._lock:
+            self._use_pixel_format(PIXEL_FORMATS['rgb'])
             rc = self._lib.lumi_predict(self._h, ctypes.c_void_p(images.data_ptr()), 1, n, h, w,
                                         ctypes.c_void_p(boxes.data_ptr()), ctypes.c_void_p(scores.data_ptr()),
                                         ctypes.c_void_p(labels.data_ptr()), ctypes.c_void_p(counts.data_ptr()), 1)

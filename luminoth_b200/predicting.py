@@ -25,7 +25,7 @@ import warnings
 import numpy as np
 
 from .config import get_model_type
-from .engine import Engine
+from .engine import Engine, pixel_format_code, pixel_size
 
 
 def _resize_bilinear_legacy(image, new_h, new_w):
@@ -95,6 +95,22 @@ def format_predictions(objects, labels, probs, scale_factor, class_labels=None):
 # Packing (``pack_sizes=True``) starts a new engine call when the images of the current one would cover less than this
 # share of their canvas (n x largest height x largest width): the canvas positions outside the images cost conv time.
 PACK_FILL = 0.75
+
+
+def _pixel_sizes(images, pixel_format):
+    """The (h, w) pixel size of each image (``engine.pixel_size``); RGB images keep their old error message."""
+    if pixel_format_code(pixel_format) == 0:
+        for im in images:
+            if im.ndim != 3 or im.shape[2] != 3:
+                raise ValueError('expected an (H, W, 3) RGB image')
+        return [im.shape[:2] for im in images]
+    return [pixel_size(im.shape, pixel_format, im.dtype == np.uint8) for im in images]
+
+
+def _format_kw(pixel_format):
+    """The engine calls' pixel_format keyword: none for RGB, the engine's default (engines stood in for by callers may
+    not take the keyword)."""
+    return {} if pixel_format_code(pixel_format) == 0 else {'pixel_format': pixel_format}
 
 
 def size_groups(targets, max_batch):
@@ -210,49 +226,51 @@ class PredictorNetwork(object):
         self.engine.load_weights(weights).finalize()
 
     # -- reference API
-    def predict_image(self, image):
-        return self.predict_batch([image])[0]
+    def predict_image(self, image, pixel_format='rgb'):
+        return self.predict_batch([image], pixel_format=pixel_format)[0]
 
     # -- batched extension
-    def predict_batch(self, images):
+    def predict_batch(self, images, pixel_format='rgb'):
         """Predictions for a list of (H, W, 3) images of ANY mix of sizes, in the caller's order.  Images are grouped
         by the size the preprocessing gives them (``target_size``); each group runs through the engine in chunks of
         ``max_batch`` -- a directory of equally sized frames (``predict.py:69-97``, video frames ``:100-171``) is
-        one batched call per chunk instead of one call per image."""
+        one batched call per chunk instead of one call per image.  ``pixel_format`` 'bgr' takes (H, W, 3) BGR images
+        (OpenCV's), 'nv12' and 'i420' (3H/2, W) uint8 frames (decoders'); they are converted to RGB in the engine's
+        input staging, with the results of their RGB conversions."""
         return [format_predictions(boxes, labels, probs, scale, self.class_labels)
-                for boxes, labels, probs, scale in self.predict_batch_raw(images)]
+                for boxes, labels, probs, scale in self.predict_batch_raw(images, pixel_format=pixel_format)]
 
-    def predict_batch_raw(self, images):
+    def predict_batch_raw(self, images, pixel_format='rgb'):
         """The network's fetches per image, before the Python post-step of ``predicting.py:114-148``:
         [(objects (K,4) float32 in PREPROCESSED-image pixels, labels (K,) int32, probs (K,) float32, scale_factor)]
-        in the caller's order (``lumi eval`` compares these with the scaled ground truth, ``eval.py:330-347``)."""
+        in the caller's order (``lumi eval`` compares these with the scaled ground truth, ``eval.py:330-347``).
+        ``pixel_format`` as in ``predict_batch``."""
         images = [np.asarray(im) for im in images]
         if not images:
             return []
-        for im in images:
-            if im.ndim != 3 or im.shape[2] != 3:
-                raise ValueError('expected an (H, W, 3) RGB image')
-        sizes = [target_size(im.shape, self.config) for im in images]
+        psizes = _pixel_sizes(images, pixel_format)
+        fmt = _format_kw(pixel_format)
+        sizes = [target_size(p, self.config) for p in psizes]
         targets = [(nh, nw) for nh, nw, _ in sizes]
         if self.pack_sizes:
             groups = pack_groups(targets, self.engine.max_batch)
         else:
             groups = size_groups(targets, self.engine.max_batch)
-        touched = set(t for t, im in zip(targets, images) if im.dtype != np.uint8 or im.shape[:2] != t)
+        touched = set(t for t, im, p in zip(targets, images, psizes) if im.dtype != np.uint8 or tuple(p) != t)
         out = [None] * len(images)
         for chunk in groups:
             shapes = set(targets[i] for i in chunk)
             srcs = [images[i] for i in chunk]
             if len(shapes) == 1 and not shapes & touched:
                 # integer pixels, no resize: the uint8 entry point (the benchmark shapes)
-                res = self.engine.predict_raw(np.stack(srcs))
+                res = self.engine.predict_raw(np.stack(srcs), **fmt)
             else:       # the reference feeds the resized FLOAT image (predicting.py:110-112): resized in the engine's
                 if any(im.dtype != np.uint8 for im in srcs):    # input staging, one call per group
                     srcs = [im.astype(np.float32, copy=False) for im in srcs]   # uint8 -> float32 is exact
                 if len(shapes) == 1:
-                    res = self.engine.predict_resize(srcs, *targets[chunk[0]])
+                    res = self.engine.predict_resize(srcs, *targets[chunk[0]], **fmt)
                 else:
-                    res = self.engine.predict_sizes(srcs, [targets[i] for i in chunk])
+                    res = self.engine.predict_sizes(srcs, [targets[i] for i in chunk], **fmt)
             boxes, scores, labels, counts = res
             for j, i in enumerate(chunk):
                 k = int(counts[j])
@@ -270,9 +288,9 @@ class PredictorNetwork(object):
         return float(m.rpn.proposals.nms_threshold)
 
     def tile_windows(self, shape, tile, overlap=0.2, full_image=True):
-        """The windows ``predict_tiled`` runs for an image of ``shape``: ([(y0, x0, h, w, th, tw)], [(s_y, s_x)]),
-        the ``tile_grid`` windows with their targets and scale factors from ``target_size``, and with ``full_image``
-        the whole image last (unless the grid already is the whole image)."""
+        """The windows ``predict_tiled`` runs for an image of pixel size ``shape`` (h, w, ...):
+        ([(y0, x0, h, w, th, tw)], [(s_y, s_x)]), the ``tile_grid`` windows with their targets and scale factors from
+        ``target_size``, and with ``full_image`` the whole image last (unless the grid already is the whole image)."""
         th_, tw_ = (tile, tile) if np.isscalar(tile) else tuple(tile)
         h, w = int(shape[0]), int(shape[1])
         grid = tile_grid(h, w, th_, tw_, overlap)
@@ -285,29 +303,28 @@ class PredictorNetwork(object):
             scales.append(tuple(s) if isinstance(s, tuple) else (s, s))
         return wins, scales
 
-    def predict_tiled(self, images, tile, overlap=0.2, full_image=True, iou_threshold=None):
+    def predict_tiled(self, images, tile, overlap=0.2, full_image=True, iou_threshold=None, pixel_format='rgb'):
         """Sliced prediction of large images: each image is cut into overlapping ``tile`` x ``tile`` windows
         (``tile_grid``; ``tile`` may be an (h, w) pair), each window runs at the model's resolution
         (``target_size``), and the windows' boxes are mapped back into the image and merged across the seams by
         per-label NMS at ``iou_threshold`` (default ``merge_iou_threshold()``), all in one engine call
         (``Engine.predict_windows``).  With ``full_image`` the whole image is also predicted at its own target size,
-        so objects larger than a tile are not lost at the seams.  Returns, per image, the ``predict_image`` format
-        with boxes in the image's own pixels."""
+        so objects larger than a tile are not lost at the seams.  ``pixel_format`` as in ``predict_batch``.  Returns,
+        per image, the ``predict_image`` format with boxes in the image's own pixels."""
         images = [np.asarray(im) for im in images]
-        for im in images:
-            if im.ndim != 3 or im.shape[2] != 3:
-                raise ValueError('expected an (H, W, 3) RGB image')
+        psizes = _pixel_sizes(images, pixel_format)
         if not images:
             return []
         if iou_threshold is None:
             iou_threshold = self.merge_iou_threshold()
         windows, scales = [], []
-        for i, im in enumerate(images):
-            wins, scl = self.tile_windows(im.shape, tile, overlap, full_image)
+        for i, p in enumerate(psizes):
+            wins, scl = self.tile_windows(p, tile, overlap, full_image)
             windows += [(i,) + wdw for wdw in wins]
             scales += scl
         if any(im.dtype != np.uint8 for im in images):
             images = [im.astype(np.float32, copy=False) for im in images]     # uint8 -> float32 is exact
-        boxes, scores, labels, counts = self.engine.predict_windows(images, windows, scales, iou_threshold)
+        boxes, scores, labels, counts = self.engine.predict_windows(images, windows, scales, iou_threshold,
+                                                                    **_format_kw(pixel_format))
         return [format_predictions(boxes[i, :counts[i]], labels[i, :counts[i]], scores[i, :counts[i]], 1.0,
                                    self.class_labels) for i in range(len(images))]
